@@ -283,18 +283,45 @@ py::bytes pack_sgd_descriptors(
   return py::bytes(reinterpret_cast<const char*>(v.data()), v.size() * sizeof(sky::SgdTensor));
 }
 void sgd_multi(uintptr_t d_tensors, int n, long long max_numel, float lr, float momentum,
-               float weight_decay, float grad_scale, bool zero_grad, uintptr_t stream) {
+               float weight_decay, float grad_scale, bool zero_grad, uintptr_t stream,
+               uintptr_t scalars) {
   check(sky::launch_sgd_multi(P<const sky::SgdTensor>(d_tensors), n, max_numel, lr, momentum,
-                              weight_decay, grad_scale, zero_grad, S(stream)),
+                              weight_decay, grad_scale, zero_grad, S(stream),
+                              P<const sky::OptimScalars>(scalars)),
         "sgd_multi");
 }
 void adam_multi(uintptr_t d_tensors, int n, long long max_numel, float lr, float beta1, float beta2,
                 float eps, float weight_decay, bool decoupled, uintptr_t step, float grad_scale,
-                bool zero_grad, uintptr_t stream) {
+                bool zero_grad, uintptr_t stream, uintptr_t scalars) {
   check(sky::launch_adam_multi(P<const sky::SgdTensor>(d_tensors), n, max_numel, lr, beta1, beta2,
                                eps, weight_decay, decoupled, P<const uint64_t>(step), grad_scale,
-                               zero_grad, S(stream)),
+                               zero_grad, S(stream), P<const sky::OptimScalars>(scalars)),
         "adam_multi");
+}
+void grad_sumsq_multi(uintptr_t d_tensors, int n, int blocks, float grad_scale, uintptr_t partials,
+                      uintptr_t stream) {
+  check(sky::launch_grad_sumsq_multi(P<const sky::SgdTensor>(d_tensors), n, blocks, grad_scale,
+                                     P<float>(partials), S(stream)),
+        "grad_sumsq_multi");
+}
+// regions: device array of the exchange regions' bases (0 = no cross-rank exchange)
+void optim_finalize(uintptr_t partials, int n_partials, uintptr_t extra_sumsq, uintptr_t regions,
+                    int n_ranks, int my_pos, uintptr_t epoch, uintptr_t error_flag, uintptr_t step,
+                    long long step_offset, int schedule, int warmup, int total, double base_lr, float max_norm,
+                    uintptr_t out, uintptr_t stream) {
+  sky::NormExchangeArgs ex;
+  if (regions != 0 && n_ranks > 1) {
+    ex.regions = P<void* const>(regions);
+    ex.n_ranks = n_ranks;
+    ex.my_pos = my_pos;
+    ex.epoch = P<const uint32_t>(epoch);
+    ex.error_flag = P<int>(error_flag);
+  }
+  check(sky::launch_optim_finalize(P<const float>(partials), n_partials,
+                                   P<const float>(extra_sumsq), ex, P<const uint64_t>(step),
+                                   step_offset, schedule, warmup, total, base_lr, max_norm,
+                                   P<sky::OptimScalars>(out), S(stream)),
+        "optim_finalize");
 }
 void cast_f32_to_bf16(uintptr_t src, uintptr_t dst, long long n, uintptr_t stream) {
   check(sky::launch_cast_f32_to_bf16(P<const float>(src), P<void>(dst), n, S(stream)), "cast");
@@ -450,11 +477,23 @@ PYBIND11_MODULE(_cuda, m) {
   m.def("pack_sgd_descriptors", &pack_sgd_descriptors);
   m.def("sgd_multi", &sgd_multi, py::arg("d_tensors"), py::arg("n"), py::arg("max_numel"),
         py::arg("lr"), py::arg("momentum") = 0.f, py::arg("weight_decay") = 0.f,
-        py::arg("grad_scale") = 1.f, py::arg("zero_grad") = true, py::arg("stream") = 0);
+        py::arg("grad_scale") = 1.f, py::arg("zero_grad") = true, py::arg("stream") = 0,
+        py::arg("scalars") = 0);
   m.def("adam_multi", &adam_multi, py::arg("d_tensors"), py::arg("n"), py::arg("max_numel"),
         py::arg("lr"), py::arg("beta1") = 0.9f, py::arg("beta2") = 0.999f, py::arg("eps") = 1e-8f,
         py::arg("weight_decay") = 0.f, py::arg("decoupled") = false, py::arg("step") = 0,
-        py::arg("grad_scale") = 1.f, py::arg("zero_grad") = true, py::arg("stream") = 0);
+        py::arg("grad_scale") = 1.f, py::arg("zero_grad") = true, py::arg("stream") = 0,
+        py::arg("scalars") = 0);
+  m.def("grad_sumsq_blocks", &sky::grad_sumsq_blocks, py::arg("max_numel"));
+  m.def("grad_sumsq_multi", &grad_sumsq_multi, py::arg("d_tensors"), py::arg("n"),
+        py::arg("blocks"), py::arg("grad_scale") = 1.f, py::arg("partials"), py::arg("stream") = 0);
+  m.def("optim_finalize", &optim_finalize, py::arg("partials") = 0, py::arg("n_partials") = 0,
+        py::arg("extra_sumsq") = 0, py::arg("regions") = 0, py::arg("n_ranks") = 1,
+        py::arg("my_pos") = 0, py::arg("epoch") = 0, py::arg("error_flag") = 0,
+        py::arg("step") = 0, py::arg("step_offset") = 0, py::arg("schedule") = 0, py::arg("warmup") = 0, py::arg("total") = 0,
+        py::arg("base_lr") = 0.0, py::arg("max_norm") = 0.f, py::arg("out"),
+        py::arg("stream") = 0);
+  m.attr("OPTIM_SCALARS_FLOATS") = static_cast<int>(sizeof(sky::OptimScalars) / sizeof(float));
   m.def("cast_f32_to_bf16", &cast_f32_to_bf16);
   m.def("cast_bf16_to_f32", &cast_bf16_to_f32);
 

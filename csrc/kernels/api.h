@@ -235,15 +235,54 @@ struct SgdTensor {
   int pad_;
   float* mom2;        // Adam second moment (null for SGD)
 };
+// Device-side optimizer scalars, written by launch_optim_finalize once per step.  When the
+// optimizer kernels get a non-null pointer to it they take `lr` from here (instead of the host
+// argument) and multiply the gradient by `clip_coef` first, so that a CUDA graph captured once
+// replays a learning-rate schedule and global-norm clipping correctly.
+struct OptimScalars {
+  float lr;
+  float clip_coef;    // min(1, max_norm / (grad_norm + 1e-6)); NaN / 0 propagate as in torch
+  float grad_norm;    // global L2 norm of the (scaled) gradients over every pipeline stage
+  float local_sumsq;  // this rank's share of grad_norm^2
+};
 int launch_sgd_multi(const SgdTensor* d_tensors, int n_tensors, long long max_numel, float lr,
                      float momentum, float weight_decay, float grad_scale, bool zero_grad,
-                     cudaStream_t stream);
+                     cudaStream_t stream, const OptimScalars* scalars = nullptr);
 // Multi-tensor fused Adam / AdamW (torch.optim.Adam(W) semantics, amsgrad=False): moments in
 // `mom` / `mom2`, the step count lives in DEVICE memory (`step`, advanced by the caller with
 // launch_advance_counter before this launch) so that the whole update is CUDA-graph capturable.
 int launch_adam_multi(const SgdTensor* d_tensors, int n_tensors, long long max_numel, float lr,
                       float beta1, float beta2, float eps, float weight_decay, bool decoupled,
-                      const uint64_t* step, float grad_scale, bool zero_grad, cudaStream_t stream);
+                      const uint64_t* step, float grad_scale, bool zero_grad, cudaStream_t stream,
+                      const OptimScalars* scalars = nullptr);
+// Sum of squares of g * grad_scale over the descriptors' gradients.  Grid (blocks, n_tensors);
+// block (x, y) writes its fp32 partial to partials[y * blocks + x] (no atomics: the result is the
+// same on every replay).  `blocks` must come from grad_sumsq_blocks(max_numel).
+int grad_sumsq_blocks(long long max_numel);
+int launch_grad_sumsq_multi(const SgdTensor* d_tensors, int n_tensors, int blocks,
+                            float grad_scale, float* partials, cudaStream_t stream);
+// Learning-rate schedules f(k) of launch_optim_finalize (lr = base_lr * f(k)).
+enum LrScheduleType : int { kLrNone = 0, kLrConstant = 1, kLrLinear = 2, kLrCosine = 3 };
+// Cross-rank exchange of the local sums of squares through peer memory (CUDA IPC).  Every rank
+// owns one region, mapped by all the others: `uint32 flags[n_ranks]` in the first 256 bytes, then
+// `float slots[2][n_ranks]`.  `regions` is a device array of the n_ranks region bases as mapped in
+// this process (own region included), indexed by pipeline position.
+struct NormExchangeArgs {
+  void* const* regions = nullptr;
+  int n_ranks = 0;
+  int my_pos = 0;
+  const uint32_t* epoch = nullptr;  // device step epoch, advanced once per step
+  int* error_flag = nullptr;        // set to 4 when a peer's slot did not arrive in time
+};
+// One block: sums `partials` in a fixed order (+ *extra_sumsq when non-null), optionally sums
+// the ranks' shares through `ex` in position order (bit-identical on every rank), then writes
+// *out: grad_norm, clip_coef (1 when max_norm <= 0) and lr = base_lr * f(k), k = *step (0 when
+// `step` is null) + step_offset.
+int launch_optim_finalize(const float* partials, int n_partials, const float* extra_sumsq,
+                          NormExchangeArgs ex, const uint64_t* step, long long step_offset,
+                          int schedule, int warmup,
+                          int total, double base_lr, float max_norm, OptimScalars* out,
+                          cudaStream_t stream);
 int launch_cast_f32_to_bf16(const float* src, void* dst, long long n, cudaStream_t stream);
 int launch_cast_bf16_to_f32(const void* src, float* dst, long long n, cudaStream_t stream);
 

@@ -1,7 +1,9 @@
 // Memory-bound sm_90a kernels: LayerNorm fwd/bwd (optionally gated on cross-GPU panel flags),
 // bias-gradient column sums, fused embedding gather+LN+dropout and its scatter backward, the
-// latency-bound pooler / classifier / cross-entropy heads, fused multi-tensor SGD, and the small
-// runtime kernels (RNG step, flag epochs, device-side throttle, peer copy + signal).
+// latency-bound pooler / classifier / cross-entropy heads, fused multi-tensor SGD / Adam with the
+// gradient-norm reduction and optimizer scalars they read (global-norm clipping, learning-rate
+// schedules), and the small runtime kernels (RNG step, flag epochs, device-side throttle, peer
+// copy + signal).
 //
 // Reference parity (what these replace):
 //   BertLayerNorm            scaelum/model/bert_layers.py:143-168   -> layernorm_{fwd,bwd}
@@ -721,10 +723,26 @@ softmax_ce_kernel(const float* __restrict__ logits, const int64_t* __restrict__ 
 // ------------------------------------------------------------------------------------------
 // Optimizer
 // ------------------------------------------------------------------------------------------
+// kScalars: lr and the clip coefficient come from the device-side OptimScalars (schedule / global
+// norm clipping); the gradient is clipped before weight decay and momentum, as torch does when
+// clip_grad_norm_ runs ahead of optimizer.step().  kScalars == false is the plain update.
+template <bool kScalars>
+__device__ __forceinline__ float scaled_grad(float g, float grad_scale, float clip) {
+  if constexpr (kScalars) return (g * grad_scale) * clip;
+  return g * grad_scale;
+}
+
+template <bool kScalars>
 __global__ void __launch_bounds__(256)
 sgd_multi_kernel(const SgdTensor* __restrict__ tensors, float lr, float momentum,
-                 float weight_decay, float grad_scale, int zero_grad) {
+                 float weight_decay, float grad_scale, int zero_grad,
+                 const OptimScalars* __restrict__ sc) {
   const SgdTensor t = tensors[blockIdx.y];
+  float clip = 1.f;
+  if constexpr (kScalars) {
+    lr = sc->lr;
+    clip = sc->clip_coef;
+  }
   const long long n4 = t.numel >> 2;
   float4* p4 = reinterpret_cast<float4*>(t.p);
   float4* g4 = reinterpret_cast<float4*>(t.g);
@@ -734,10 +752,10 @@ sgd_multi_kernel(const SgdTensor* __restrict__ tensors, float lr, float momentum
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     float4 p = p4[i];
     float4 g = g4[i];
-    g.x = g.x * grad_scale + weight_decay * p.x;
-    g.y = g.y * grad_scale + weight_decay * p.y;
-    g.z = g.z * grad_scale + weight_decay * p.z;
-    g.w = g.w * grad_scale + weight_decay * p.w;
+    g.x = scaled_grad<kScalars>(g.x, grad_scale, clip) + weight_decay * p.x;
+    g.y = scaled_grad<kScalars>(g.y, grad_scale, clip) + weight_decay * p.y;
+    g.z = scaled_grad<kScalars>(g.z, grad_scale, clip) + weight_decay * p.z;
+    g.w = scaled_grad<kScalars>(g.w, grad_scale, clip) + weight_decay * p.w;
     if (m4 != nullptr) {
       float4 m = m4[i];
       m.x = momentum * m.x + g.x;
@@ -759,7 +777,7 @@ sgd_multi_kernel(const SgdTensor* __restrict__ tensors, float lr, float momentum
   if (blockIdx.x == 0) {
     for (long long i = (n4 << 2) + threadIdx.x; i < t.numel; i += blockDim.x) {
       float p = t.p[i];
-      float g = t.g[i] * grad_scale + weight_decay * p;
+      float g = scaled_grad<kScalars>(t.g[i], grad_scale, clip) + weight_decay * p;
       if (t.mom != nullptr) {
         const float m = momentum * t.mom[i] + g;
         t.mom[i] = m;
@@ -777,11 +795,17 @@ sgd_multi_kernel(const SgdTensor* __restrict__ tensors, float lr, float momentum
 // accepts any torch.optim name): one launch per stage, moments + master + bf16 shadow + gradient
 // zeroing in one pass = 28 B / parameter.  The bias corrections come from a device-side step
 // counter, so a captured graph replays the right correction every step.
+template <bool kScalars>
 __global__ void __launch_bounds__(256)
 adam_multi_kernel(const SgdTensor* __restrict__ tensors, float lr, float beta1, float beta2,
                   float eps, float weight_decay, int decoupled, const uint64_t* __restrict__ step,
-                  float grad_scale, int zero_grad) {
+                  float grad_scale, int zero_grad, const OptimScalars* __restrict__ sc) {
   const SgdTensor t = tensors[blockIdx.y];
+  float clip = 1.f;
+  if constexpr (kScalars) {
+    lr = sc->lr;   // scales step_size and the decoupled decay, as torch's lr does
+    clip = sc->clip_coef;
+  }
   const float tstep = static_cast<float>(*step);
   const float bc1 = 1.f - powf(beta1, tstep);
   const float bc2_rsqrt = rsqrtf(1.f - powf(beta2, tstep));
@@ -790,7 +814,7 @@ adam_multi_kernel(const SgdTensor* __restrict__ tensors, float lr, float beta1, 
   const float l2 = decoupled ? 0.f : weight_decay;
   auto upd = [&](float& p, float gi, float& m, float& v) {
     p *= decay;
-    const float g = gi * grad_scale + l2 * p;
+    const float g = scaled_grad<kScalars>(gi, grad_scale, clip) + l2 * p;
     m = beta1 * m + (1.f - beta1) * g;
     v = beta2 * v + (1.f - beta2) * g * g;
     p -= step_size * m / (sqrtf(v) * bc2_rsqrt + eps);
@@ -826,6 +850,123 @@ adam_multi_kernel(const SgdTensor* __restrict__ tensors, float lr, float beta1, 
       if (zero_grad) t.g[i] = 0.f;
     }
   }
+}
+
+// Global-norm clipping, step 1: per-block sums of squares of g * grad_scale over the same
+// descriptors (4 B read per parameter).  Each block reduces in a fixed order and stores its own
+// partial, so a replay reproduces the result bit for bit.
+__global__ void __launch_bounds__(256)
+grad_sumsq_multi_kernel(const SgdTensor* __restrict__ tensors, float grad_scale,
+                        float* __restrict__ partials) {
+  const SgdTensor t = tensors[blockIdx.y];
+  const long long n4 = t.numel >> 2;
+  const float4* g4 = reinterpret_cast<const float4*>(t.g);
+  float acc = 0.f;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n4;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float4 g = g4[i];
+    const float x = g.x * grad_scale, y = g.y * grad_scale;
+    const float z = g.z * grad_scale, w = g.w * grad_scale;
+    acc += (x * x + y * y) + (z * z + w * w);
+  }
+  if (blockIdx.x == 0) {
+    for (long long i = (n4 << 2) + threadIdx.x; i < t.numel; i += blockDim.x) {
+      const float x = t.g[i] * grad_scale;
+      acc += x * x;
+    }
+  }
+  __shared__ float red[8];
+  acc = warp_sum(acc);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) s += red[w];
+    partials[static_cast<long long>(blockIdx.y) * gridDim.x + blockIdx.x] = s;
+  }
+}
+
+__device__ __forceinline__ void st_relaxed_sys_f32(float* addr, float v) {
+  asm volatile("st.relaxed.sys.global.f32 [%0], %1;" ::"l"(addr), "f"(v) : "memory");
+}
+__device__ __forceinline__ float ld_relaxed_sys_f32(const float* addr) {
+  float v;
+  asm volatile("ld.relaxed.sys.global.f32 %0, [%1];" : "=f"(v) : "l"(addr) : "memory");
+  return v;
+}
+
+__device__ double lr_factor(int schedule, double k, int warmup, int total) {
+  if (schedule == kLrNone) return 1.0;
+  if (k < warmup) return k / fmax(1.0, static_cast<double>(warmup));
+  if (schedule == kLrConstant) return 1.0;
+  const double span = fmax(1.0, static_cast<double>(total - warmup));
+  if (schedule == kLrLinear) return fmax(0.0, (total - k) / span);
+  const double prog = fmin(1.0, (k - warmup) / span);   // clamped: no rise again after T
+  return fmax(0.0, 0.5 * (1.0 + cos(3.14159265358979323846 * prog)));
+}
+
+// Global-norm clipping, step 2 (+ the learning-rate schedule): one block.
+//
+// Peer exchange (ex.n_ranks > 1): thread 0 stores this rank's share into slot [epoch & 1][my_pos]
+// of EVERY rank's region and bumps that region's flags[my_pos] with release semantics, then waits
+// (acquire) until flags[q] >= epoch for every q and sums slot [epoch & 1][q] in position order.
+// Flags count the steps a rank has published, so they equal the epoch after that step's store.
+// Why two slots per rank are enough: rank q can only store epoch e + 2 (same parity as e) after
+// its own step e + 1 finished the exchange, which needed this rank's epoch-(e + 1) store, and this
+// rank makes that store in a later launch than the one that reads epoch e's slots.
+__global__ void __launch_bounds__(256)
+optim_finalize_kernel(const float* __restrict__ partials, int n_partials,
+                      const float* __restrict__ extra_sumsq, NormExchangeArgs ex,
+                      const uint64_t* __restrict__ step, long long step_offset, int schedule,
+                      int warmup, int total, double base_lr, float max_norm, OptimScalars* __restrict__ out) {
+  __shared__ double red[256];
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < n_partials; i += blockDim.x) acc += partials[i];
+  red[threadIdx.x] = acc;
+  __syncthreads();
+  for (int s = 128; s > 0; s >>= 1) {
+    if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+    __syncthreads();
+  }
+  if (threadIdx.x != 0) return;
+  double local = red[0];
+  if (extra_sumsq != nullptr) local += static_cast<double>(*extra_sumsq);
+  const float local_f = static_cast<float>(local);
+  double total_sumsq = local_f;
+  if (ex.n_ranks > 1) {
+    const uint32_t e = *ex.epoch;
+    const int par = static_cast<int>(e & 1u) * ex.n_ranks;
+    for (int q = 0; q < ex.n_ranks; ++q) {
+      char* base = static_cast<char*>(ex.regions[q]);
+      st_relaxed_sys_f32(reinterpret_cast<float*>(base + 256) + par + ex.my_pos, local_f);
+      __threadfence_system();
+      red_release_sys_add(reinterpret_cast<uint32_t*>(base) + ex.my_pos, 1u);
+    }
+    const char* mine = static_cast<const char*>(ex.regions[ex.my_pos]);
+    const uint32_t* flags = reinterpret_cast<const uint32_t*>(mine);
+    const float* slots = reinterpret_cast<const float*>(mine + 256) + par;
+    total_sumsq = 0.0;
+    for (int q = 0; q < ex.n_ranks; ++q) {
+      if (!wait_flag_ge(flags + q, e, kFlagTimeoutNs)) {
+        if (ex.error_flag) atomicExch(ex.error_flag, 4);
+      }
+      total_sumsq += static_cast<double>(ld_relaxed_sys_f32(slots + q));
+    }
+  }
+  const float norm = static_cast<float>(sqrt(total_sumsq));
+  float coef = 1.f;
+  if (max_norm > 0.f) {
+    // torch.nn.utils.clip_grad_norm_: clamp(max_norm / (norm + 1e-6), max=1); NaN stays NaN
+    coef = __fdiv_rn(max_norm, __fadd_rn(norm, 1e-6f));
+    if (!(coef != coef)) coef = fminf(coef, 1.f);
+  }
+  const double k = static_cast<double>(step != nullptr ? static_cast<long long>(*step) : 0ll) +
+                   static_cast<double>(step_offset);
+  out->lr = static_cast<float>(base_lr * lr_factor(schedule, k, warmup, total));
+  out->clip_coef = coef;
+  out->grad_norm = norm;
+  out->local_sumsq = local_f;
 }
 
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ s, __nv_bfloat16* __restrict__ d,
@@ -1096,29 +1237,68 @@ int launch_softmax_ce(const float* logits, const int64_t* labels, float* loss, f
 
 int launch_sgd_multi(const SgdTensor* d_tensors, int n_tensors, long long max_numel, float lr,
                      float momentum, float weight_decay, float grad_scale, bool zero_grad,
-                     cudaStream_t stream) {
+                     cudaStream_t stream, const OptimScalars* scalars) {
   if (n_tensors <= 0) return 0;
   long long blocks = (max_numel / 4 + 255) / 256;
   if (blocks > num_sms() * 2) blocks = num_sms() * 2;
   if (blocks < 1) blocks = 1;
   dim3 grid(static_cast<unsigned>(blocks), n_tensors);
-  sgd_multi_kernel<<<grid, 256, 0, stream>>>(d_tensors, lr, momentum, weight_decay, grad_scale,
-                                             zero_grad ? 1 : 0);
+  if (scalars != nullptr)
+    sgd_multi_kernel<true><<<grid, 256, 0, stream>>>(d_tensors, lr, momentum, weight_decay,
+                                                     grad_scale, zero_grad ? 1 : 0, scalars);
+  else
+    sgd_multi_kernel<false><<<grid, 256, 0, stream>>>(d_tensors, lr, momentum, weight_decay,
+                                                      grad_scale, zero_grad ? 1 : 0, nullptr);
   SKY_LAUNCH_CHECK();
 }
 
 int launch_adam_multi(const SgdTensor* d_tensors, int n_tensors, long long max_numel, float lr,
                       float beta1, float beta2, float eps, float weight_decay, bool decoupled,
-                      const uint64_t* step, float grad_scale, bool zero_grad, cudaStream_t stream) {
+                      const uint64_t* step, float grad_scale, bool zero_grad, cudaStream_t stream,
+                      const OptimScalars* scalars) {
   if (n_tensors <= 0) return 0;
   if (step == nullptr) return 906;
   long long blocks = (max_numel / 4 + 255) / 256;
   if (blocks > num_sms() * 2) blocks = num_sms() * 2;
   if (blocks < 1) blocks = 1;
   dim3 grid(static_cast<unsigned>(blocks), n_tensors);
-  adam_multi_kernel<<<grid, 256, 0, stream>>>(d_tensors, lr, beta1, beta2, eps, weight_decay,
-                                              decoupled ? 1 : 0, step, grad_scale,
-                                              zero_grad ? 1 : 0);
+  if (scalars != nullptr)
+    adam_multi_kernel<true><<<grid, 256, 0, stream>>>(d_tensors, lr, beta1, beta2, eps,
+                                                      weight_decay, decoupled ? 1 : 0, step,
+                                                      grad_scale, zero_grad ? 1 : 0, scalars);
+  else
+    adam_multi_kernel<false><<<grid, 256, 0, stream>>>(d_tensors, lr, beta1, beta2, eps,
+                                                       weight_decay, decoupled ? 1 : 0, step,
+                                                       grad_scale, zero_grad ? 1 : 0, nullptr);
+  SKY_LAUNCH_CHECK();
+}
+
+int grad_sumsq_blocks(long long max_numel) {
+  long long blocks = (max_numel / 4 + 255) / 256;
+  if (blocks > num_sms() * 2) blocks = num_sms() * 2;
+  if (blocks < 1) blocks = 1;
+  return static_cast<int>(blocks);
+}
+
+int launch_grad_sumsq_multi(const SgdTensor* d_tensors, int n_tensors, int blocks,
+                            float grad_scale, float* partials, cudaStream_t stream) {
+  if (n_tensors <= 0) return 0;
+  if (blocks < 1 || partials == nullptr) return 907;
+  dim3 grid(static_cast<unsigned>(blocks), n_tensors);
+  grad_sumsq_multi_kernel<<<grid, 256, 0, stream>>>(d_tensors, grad_scale, partials);
+  SKY_LAUNCH_CHECK();
+}
+
+int launch_optim_finalize(const float* partials, int n_partials, const float* extra_sumsq,
+                          NormExchangeArgs ex, const uint64_t* step, long long step_offset,
+                          int schedule, int warmup, int total, double base_lr, float max_norm,
+                          OptimScalars* out, cudaStream_t stream) {
+  if (out == nullptr || n_partials < 0) return 908;
+  if (ex.n_ranks > 1 && (ex.regions == nullptr || ex.epoch == nullptr || ex.my_pos < 0 ||
+                         ex.my_pos >= ex.n_ranks))
+    return 909;
+  optim_finalize_kernel<<<1, 256, 0, stream>>>(partials, n_partials, extra_sumsq, ex, step,
+                                               step_offset, schedule, warmup, total, base_lr, max_norm, out);
   SKY_LAUNCH_CHECK();
 }
 

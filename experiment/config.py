@@ -27,6 +27,12 @@ MICRO_BATCHES = int(os.getenv("MICRO_BATCHES", "1"))
 MAX_ITERS = int(os.getenv("MAX_ITERS", "30"))
 SLOW_RANK = int(os.getenv("SLOW_RANK", "-1"))
 SLOWDOWN = float(os.getenv("SLOWDOWN", "0"))
+# optional learning-rate schedule (constant | linear | cosine, HF transformers formulas) and
+# global-norm gradient clipping; unset = constant lr, no clipping
+LR_SCHEDULE = os.getenv("LR_SCHEDULE")
+WARMUP_STEPS = int(os.getenv("WARMUP_STEPS", "0"))
+TOTAL_STEPS = int(os.getenv("TOTAL_STEPS", str(MAX_ITERS)))
+MAX_GRAD_NORM = float(os.getenv("MAX_GRAD_NORM")) if os.getenv("MAX_GRAD_NORM") else None
 TINY = os.getenv("TINY", "0") == "1"                          # shrink the geometry for CPU smoke runs
 
 _config = BertConfig.bert_large()                              # wwm_uncased_L-24_H-1024_A-16 geometry
@@ -114,6 +120,9 @@ allocator_config = dict(
 
 train_config = dict(
     optim_cfg=dict(optim_type="SGD", lr=0.001),
+    lr_schedule_cfg=(dict(type=LR_SCHEDULE, warmup_steps=WARMUP_STEPS, total_steps=TOTAL_STEPS)
+                     if LR_SCHEDULE else None),
+    grad_clip_cfg=dict(max_norm=MAX_GRAD_NORM) if MAX_GRAD_NORM is not None else None,
     loss_cfg=dict(type="CrossEntropyLoss"),
     runner_cfg=dict(max_epochs=1, max_iters=MAX_ITERS, micro_batches=MICRO_BATCHES),
     hook_config=[dict(type="StopHook", root=_LOG_ROOT), dict(type="DistributedTimerHelperHook")]

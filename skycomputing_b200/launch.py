@@ -177,7 +177,10 @@ def run_process(rank: int, world_size: int, rpc_config: dict, model_config: list
 
         model = RpcModel(worker_manager=worker_manager, this_rank=rank)
         info("created model")
-        optimizer = build_optimizer(model.optim_module, dict(train_config["optim_cfg"]))
+        # optional learning-rate schedule / global-norm gradient clipping (None = off)
+        step_cfg = dict(lr_schedule=train_config.get("lr_schedule_cfg"),
+                        grad_clip=train_config.get("grad_clip_cfg"))
+        optimizer = build_optimizer(model.optim_module, dict(train_config["optim_cfg"]), **step_cfg)
         info("created distrubted optimizer")
         runner = Runner(model=model, parameter_server=parameter_server,
                         worker_manager=worker_manager, optimizer=optimizer,
@@ -205,6 +208,8 @@ def run_process(rank: int, world_size: int, rpc_config: dict, model_config: list
                     continue
                 cfg.setdefault("allocator_factory", allocator_factory)
                 cfg.setdefault("optimizer_cfg", dict(train_config["optim_cfg"]))
+                cfg.setdefault("lr_schedule", step_cfg["lr_schedule"])
+                cfg.setdefault("grad_clip", step_cfg["grad_clip"])
                 cfg.setdefault("allocate_type", alloc_type)
             runner.register_hook(build_hook(cfg.pop("type"), **cfg))
         info("register hooks")

@@ -46,6 +46,47 @@ class EngineBase:
         self._trace_buf: Optional[torch.Tensor] = None
         self._trace_tags: list = []
         self._trace_capacity = 0
+        self._norm_exchange = None
+
+    # ------------------------------------------------------------------ global gradient norm
+    def _norm_info(self) -> tuple:
+        """(needs the global gradient norm, can reduce it through peer memory): gathered with the
+        other setup flags so that every rank picks the same reduction."""
+        from .optim import FusedSGD
+
+        needs = bool(getattr(self.optimizer, "needs_global_norm", False))
+        return needs, needs and isinstance(self.optimizer, FusedSGD)
+
+    def _setup_grad_norm(self, position: int, num_positions: int, rank_of_position,
+                         infos) -> None:
+        """Clipping needs the norm over every stage: a peer-memory exchange when the boundaries
+        are fused and every rank runs a fused optimizer (capturable), one all_reduce otherwise.
+        Created here, in setup, never during capture.  Collective."""
+        needs = {bool(i[0]) for i in infos}
+        if len(needs) > 1:
+            raise ValueError("gradient clipping must be configured on every pipeline rank or none")
+        if num_positions < 2 or not needs.pop():
+            return
+        if self.fused is not None and all(i[1] for i in infos):
+            from .p2p import GradNormExchange
+
+            self._norm_exchange = GradNormExchange(
+                position, num_positions, list(rank_of_position), self.device,
+                self.fused.epoch_ptr, self.fused.error_ptr, group=self.group)
+            self.optimizer.set_norm_reduction(group=self.group, exchange=self._norm_exchange)
+        else:
+            self.optimizer.set_norm_reduction(group=self.group, allreduce=True)
+
+    def _sends_before_optimizer(self) -> bool:
+        """The optimizer's reduction of the norm must not overtake outstanding p2p sends (an NCCL
+        all_reduce behind them would dead-lock): engines with such sends wait for them first."""
+        return bool(getattr(self.optimizer, "needs_global_norm", False))
+
+    def _close_grad_norm(self) -> None:
+        if self._norm_exchange is not None:
+            self._norm_exchange.close()
+            self._norm_exchange = None
+            self.optimizer.set_norm_reduction()
 
     # ------------------------------------------------------------------ backend
     def _native_active(self) -> bool:

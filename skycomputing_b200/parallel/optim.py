@@ -17,13 +17,85 @@ nesterov, dampening, amsgrad, maximize) to the named ``torch.optim`` class over 
 (the bf16 shadows are then refreshed lazily by version counter; such a step is NOT graph-safe and
 the engines run it eagerly).  Optimizer state lives with the stage, as with the reference's
 DistributedOptimizer.
+
+Learning-rate schedules and global-norm gradient clipping (``build_optimizer(..., lr_schedule=,
+grad_clip=)``, both opt-in).  The fused optimizers keep them on the device so that a captured step
+replays them: ``grad_sumsq_multi`` writes per-block sums of squares of the gradients,
+``optim_finalize`` adds them up in a fixed order (plus, in a pipeline, the other stages' shares:
+peer-memory slots or one ``all_reduce``, see ``set_norm_reduction``) and writes ``OptimScalars
+{lr, clip_coef, grad_norm}``, which ``sgd_multi`` / ``adam_multi`` read.  ``lr = base_lr * f(k)``
+with k = optimizer steps already taken, read from a device-side counter.
 """
 from __future__ import annotations
 
 from typing import Optional
 
+import math
+
 import torch
 import torch.nn as nn
+
+LR_SCHEDULES = {"constant": 1, "linear": 2, "cosine": 3}   # csrc/kernels/api.h LrScheduleType
+
+
+def lr_factor(schedule: Optional[dict], k: int) -> float:
+    """f(k) of the schedule (HF transformers formulas); lr = base_lr * f(k), k = steps taken."""
+    if not schedule:
+        return 1.0
+    w, t = schedule["warmup_steps"], schedule["total_steps"]
+    if k < w:
+        return k / max(1, w)
+    if schedule["type"] == "constant":
+        return 1.0
+    span = max(1, t - w)
+    if schedule["type"] == "linear":
+        return max(0.0, (t - k) / span)
+    prog = min(1.0, (k - w) / span)   # clamped: the rate does not rise again after T
+    return max(0.0, 0.5 * (1.0 + math.cos(math.pi * prog)))
+
+
+def check_lr_schedule(cfg: Optional[dict]) -> Optional[dict]:
+    """Normalised ``dict(type, warmup_steps, total_steps)`` or None; ValueError when invalid."""
+    if cfg is None:
+        return None
+    cfg = dict(cfg)
+    kind = cfg.pop("type", None)
+    if kind not in LR_SCHEDULES:
+        raise ValueError(f"lr_schedule type must be one of {sorted(LR_SCHEDULES)}, got {kind!r}")
+    w = int(cfg.pop("warmup_steps", 0) or 0)
+    t = cfg.pop("total_steps", None)
+    if cfg:
+        raise ValueError(f"unknown lr_schedule keys {sorted(cfg)}")
+    if w < 0:
+        raise ValueError(f"lr_schedule warmup_steps must be >= 0, got {w}")
+    if t is None:
+        if kind != "constant":
+            raise ValueError(f"lr_schedule {kind!r} needs total_steps")
+        t = w
+    t = int(t)
+    if kind != "constant" and t <= 0:
+        raise ValueError(f"lr_schedule total_steps must be > 0, got {t}")
+    if w > t:
+        raise ValueError(f"lr_schedule warmup_steps ({w}) > total_steps ({t})")
+    return dict(type=kind, warmup_steps=w, total_steps=t)
+
+
+def check_grad_clip(cfg: Optional[dict]) -> Optional[float]:
+    """``max_norm`` of ``dict(max_norm=x[, norm_type=2])`` or None; ValueError when invalid."""
+    if cfg is None:
+        return None
+    cfg = dict(cfg)
+    if "max_norm" not in cfg:
+        raise ValueError("grad_clip needs max_norm")
+    max_norm = float(cfg.pop("max_norm"))
+    norm_type = float(cfg.pop("norm_type", 2.0))
+    if cfg:
+        raise ValueError(f"unknown grad_clip keys {sorted(cfg)}")
+    if not max_norm > 0.0 or math.isinf(max_norm):
+        raise ValueError(f"grad_clip max_norm must be a positive finite number, got {max_norm}")
+    if norm_type != 2.0:
+        raise ValueError(f"grad_clip supports the L2 norm only (norm_type=2), got {norm_type}")
+    return max_norm
 
 
 class FusedSGD:
@@ -59,6 +131,9 @@ class FusedSGD:
 
         self._overwrite_ok = _os.environ.get("SKY_SGD_OVERWRITE", "1") != "0"
         self.param_groups = [dict(lr=lr, momentum=momentum, weight_decay=weight_decay)]
+        params = list(module.parameters())
+        self._device = self.banks[0].master().device if self.banks else (
+            params[0].device if params else torch.device("cpu"))
 
     @property
     def graph_safe(self) -> bool:
@@ -66,6 +141,123 @@ class FusedSGD:
         return self._rest_opt is None
 
     _mom2: list = []
+    # learning-rate schedule / gradient clipping (configure()); all None = the plain update
+    _step: Optional[torch.Tensor] = None          # device-side count of steps taken
+    _step_offset = 0                              # schedule steps taken by an earlier optimizer
+    _sched: Optional[dict] = None
+    _max_norm: Optional[float] = None
+    _scalars: Optional[torch.Tensor] = None       # device OptimScalars {lr, clip_coef, norm, local}
+    _partials: Optional[torch.Tensor] = None
+    _norm_allreduce = False
+    _norm_group = None
+    _norm_exchange = None
+    _stepped = False
+
+    def configure(self, lr_schedule: Optional[dict] = None, max_norm: Optional[float] = None) -> None:
+        """Device-side learning-rate schedule and / or global-norm clipping (validated configs,
+        see build_optimizer).  The step() of a captured graph then replays both correctly."""
+        self._sched, self._max_norm = lr_schedule, max_norm
+        if lr_schedule is None and max_norm is None:
+            return
+        self._scalars = torch.zeros(self._nat.ext().OPTIM_SCALARS_FLOATS, dtype=torch.float32,
+                                    device=self._device)
+        if lr_schedule is not None and self._step is None:
+            self._step = torch.zeros(1, dtype=torch.int64, device=self._device)
+
+    @property
+    def needs_global_norm(self) -> bool:
+        """True when step() needs the gradient norm over every pipeline stage."""
+        return self._max_norm is not None
+
+    @property
+    def reports_scalars(self) -> bool:
+        return self._scalars is not None
+
+    def set_norm_reduction(self, group=None, allreduce: bool = False, exchange=None) -> None:
+        """How step() adds up the stages' shares of the squared norm: ``exchange`` (a
+        p2p.GradNormExchange: peer-memory slots, capturable), ``allreduce`` (one fp32
+        ``dist.all_reduce`` over ``group``) or neither (single stage)."""
+        self._norm_exchange = exchange
+        self._norm_allreduce = bool(allreduce) and exchange is None
+        self._norm_group = group
+
+    def _compute_scalars(self, grad_scale: float, stream: int) -> None:
+        """grad_sumsq_multi + optim_finalize: writes lr / clip_coef / grad_norm for this step,
+        reading k from the step counter before the caller advances it."""
+        ext = self._nat.ext()
+        partials, n_part, extra = 0, 0, 0
+        if self._max_norm is not None:
+            if self.banks:
+                d = self._descriptors()
+                if self._partials is None:
+                    blocks = ext.grad_sumsq_blocks(self._max_numel)
+                    self._partials = torch.zeros(blocks * len(self.banks), dtype=torch.float32,
+                                                 device=self._device)
+                    self._sumsq_blocks = blocks
+                ext.grad_sumsq_multi(d.data_ptr(), len(self.banks), self._sumsq_blocks,
+                                     float(grad_scale), self._partials.data_ptr(), stream)
+                partials, n_part = self._partials.data_ptr(), self._partials.numel()
+            if self._rest_opt is not None:
+                # torch fallback layers (eager anyway: such an optimizer is not graph-safe)
+                grads = self._rest_grads()
+                self._rest_sumsq = (torch.stack([g.float().pow(2).sum() for g in grads]).sum()
+                                    if grads else torch.zeros((), device=self._device)).reshape(1)
+                extra = self._rest_sumsq.data_ptr()
+        sched = self._sched
+        common = dict(step=self._step.data_ptr() if self._step is not None else 0,
+                      step_offset=int(self._step_offset),
+                      schedule=LR_SCHEDULES[sched["type"]] if sched else 0,
+                      warmup=sched["warmup_steps"] if sched else 0,
+                      total=sched["total_steps"] if sched else 0,
+                      base_lr=float(self.param_groups[0]["lr"]),
+                      max_norm=float(self._max_norm or 0.0), out=self._scalars.data_ptr(),
+                      stream=stream)
+        ex = self._norm_exchange
+        if ex is not None and self._max_norm is not None:
+            ext.optim_finalize(partials, n_part, extra, regions=ex.regions_ptr, n_ranks=ex.n_ranks,
+                               my_pos=ex.position, epoch=ex.epoch_ptr, error_flag=ex.error_ptr,
+                               **common)
+        elif self._norm_allreduce and self._max_norm is not None:
+            import torch.distributed as dist
+
+            ext.optim_finalize(partials, n_part, extra, **common)    # this rank's share
+            dist.all_reduce(self._scalars[3:4], group=self._norm_group)
+            ext.optim_finalize(0, 0, self._scalars.data_ptr() + 12, **common)
+        else:
+            ext.optim_finalize(partials, n_part, extra, **common)
+
+    def _rest_grads(self) -> list:
+        return [p.grad for g in self._rest_opt.param_groups for p in g["params"]
+                if p.grad is not None]
+
+    def _rest_step(self) -> None:
+        if self._scalars is not None:
+            if self._max_norm is not None:
+                for g in self._rest_grads():
+                    g.mul_(self._scalars[1])
+            if self._sched is not None:
+                k = self.step_count() - 1      # the device counter was advanced for this step
+                for grp in self._rest_opt.param_groups:
+                    grp["lr"] = float(self.param_groups[0]["lr"]) * lr_factor(self._sched, k)
+        self._rest_opt.step()
+        self._rest_opt.zero_grad(set_to_none=False)
+
+    def scalars(self) -> dict:
+        """lr and global grad_norm of the last step (None where not configured / no step yet)."""
+        if self._scalars is None or not self._stepped:
+            return dict(lr=None, grad_norm=None)
+        lr, _coef, norm, _local = self._scalars.tolist()
+        return dict(lr=lr, grad_norm=norm if self._max_norm is not None else None)
+
+    def step_count(self) -> int:
+        """Optimizer steps taken, as the learning-rate schedule counts them."""
+        return (int(self._step.item()) if self._step is not None else 0) + self._step_offset
+
+    def set_step_count(self, k: int) -> None:
+        """Continue the schedule at step k (a rebuilt optimizer after a layer migration); the
+        device counter that also drives Adam's bias correction is left alone, because the moments
+        restart with the new optimizer."""
+        self._step_offset = int(k) - (int(self._step.item()) if self._step is not None else 0)
 
     def _descriptors(self) -> torch.Tensor:
         if self._desc_dev is None and self.banks:
@@ -82,6 +274,14 @@ class FusedSGD:
         return self._desc_dev
 
     def step(self, grad_scale: float = 1.0) -> None:
+        sc = 0
+        if self._scalars is not None:
+            stream = torch.cuda.current_stream().cuda_stream
+            self._compute_scalars(grad_scale, stream)
+            if self._step is not None:
+                self._nat.ext().advance_counter(self._step.data_ptr(), 1, stream)
+            sc = self._scalars.data_ptr()
+            self._stepped = True
         if self.banks:
             d = self._descriptors()
             self._nat.ext().sgd_multi(d_tensors=d.data_ptr(), n=len(self.banks),
@@ -89,13 +289,12 @@ class FusedSGD:
                                       momentum=float(self.momentum),
                                       weight_decay=float(self.weight_decay),
                                       grad_scale=float(grad_scale), zero_grad=True,
-                                      stream=torch.cuda.current_stream().cuda_stream)
+                                      stream=torch.cuda.current_stream().cuda_stream, scalars=sc)
             for b in self.banks:
                 if b.overwrite_first:
                     b.fresh = True
         if self._rest_opt is not None:
-            self._rest_opt.step()
-            self._rest_opt.zero_grad(set_to_none=False)
+            self._rest_step()
 
     def zero_grad(self, set_to_none: bool = False) -> None:
         for b in self.banks:
@@ -105,9 +304,14 @@ class FusedSGD:
             self._rest_opt.zero_grad(set_to_none=False)
 
     def state_dict(self) -> dict:
-        return dict(momentum=[None if m is None else m.detach().cpu() for m in self._mom],
-                    rest=None if self._rest_opt is None else self._rest_opt.state_dict(),
-                    param_groups=self.param_groups)
+        sd = dict(momentum=[None if m is None else m.detach().cpu() for m in self._mom],
+                  rest=None if self._rest_opt is None else self._rest_opt.state_dict(),
+                  param_groups=self.param_groups)
+        if self._step is not None:
+            sd["step"] = int(self._step.item())
+        if self._sched is not None:
+            sd["lr_schedule_step"] = self.step_count()
+        return sd
 
     def load_state_dict(self, sd: dict) -> None:
         for m, s in zip(self._mom, sd.get("momentum", [])):
@@ -116,6 +320,10 @@ class FusedSGD:
         if self._rest_opt is not None and sd.get("rest") is not None:
             self._rest_opt.load_state_dict(sd["rest"])
         self.param_groups = sd.get("param_groups", self.param_groups)
+        if self._step is not None and "step" in sd:
+            self._step.fill_(int(sd["step"]))
+        if "lr_schedule_step" in sd:
+            self.set_step_count(int(sd["lr_schedule_step"]))
 
 
 class FusedAdam(FusedSGD):
@@ -139,6 +347,11 @@ class FusedAdam(FusedSGD):
         self.param_groups = [dict(lr=lr, betas=self.betas, eps=eps, weight_decay=weight_decay)]
 
     def step(self, grad_scale: float = 1.0) -> None:
+        sc = 0
+        if self._scalars is not None:
+            self._compute_scalars(grad_scale, torch.cuda.current_stream().cuda_stream)
+            sc = self._scalars.data_ptr()
+            self._stepped = True
         if self.banks:
             d = self._descriptors()
             ext = self._nat.ext()
@@ -149,18 +362,19 @@ class FusedAdam(FusedSGD):
                            beta2=self.betas[1], eps=float(self.eps),
                            weight_decay=float(self.weight_decay), decoupled=bool(self.decoupled),
                            step=self._step.data_ptr(), grad_scale=float(grad_scale),
-                           zero_grad=True, stream=stream)
+                           zero_grad=True, stream=stream, scalars=sc)
             for b in self.banks:
                 if b.overwrite_first:
                     b.fresh = True
+        elif self._scalars is not None:
+            self._nat.ext().advance_counter(self._step.data_ptr(), 1,
+                                            torch.cuda.current_stream().cuda_stream)
         if self._rest_opt is not None:
-            self._rest_opt.step()
-            self._rest_opt.zero_grad(set_to_none=False)
+            self._rest_step()
 
     def state_dict(self) -> dict:
         sd = super().state_dict()
         sd["second_moment"] = [v.detach().cpu() for v in self._mom2]
-        sd["step"] = int(self._step.item())
         return sd
 
     def load_state_dict(self, sd: dict) -> None:
@@ -168,8 +382,6 @@ class FusedAdam(FusedSGD):
         for v, s_ in zip(self._mom2, sd.get("second_moment", [])):
             if s_ is not None:
                 v.copy_(s_)
-        if "step" in sd:
-            self._step.fill_(int(sd["step"]))
 
 
 class TorchOptimizerAdapter:
@@ -182,6 +394,48 @@ class TorchOptimizerAdapter:
     def __init__(self, optimizer: torch.optim.Optimizer):
         self.optimizer = optimizer
         self.param_groups = optimizer.param_groups
+        self._sched: Optional[dict] = None
+        self._scheduler = None
+        self._max_norm: Optional[float] = None
+        self._norm_allreduce = False
+        self._norm_group = None
+        self._last_lr: Optional[float] = None
+        self._last_norm: Optional[torch.Tensor] = None
+
+    def configure(self, lr_schedule: Optional[dict] = None, max_norm: Optional[float] = None) -> None:
+        """Learning-rate schedule (a LambdaLR stepped after every step()) and / or global-norm
+        clipping of ``p.grad`` before the step."""
+        self._sched, self._max_norm = lr_schedule, max_norm
+        if lr_schedule is not None:
+            self._scheduler = torch.optim.lr_scheduler.LambdaLR(
+                self.optimizer, lambda k: lr_factor(lr_schedule, k))
+
+    needs_global_norm = property(lambda self: self._max_norm is not None)
+    reports_scalars = property(lambda self: self._sched is not None or self._max_norm is not None)
+
+    def set_norm_reduction(self, group=None, allreduce: bool = False, exchange=None) -> None:
+        self._norm_allreduce = bool(allreduce) or exchange is not None
+        self._norm_group = group
+
+    def _clip(self) -> None:
+        """torch.nn.utils.clip_grad_norm_ over every stage: local sum of squares, all_reduce of
+        that one element, then the same coefficient on every rank."""
+        params = [p for g in self.optimizer.param_groups for p in g["params"]]
+        grads = [p.grad for p in params if p.grad is not None]
+        if grads:
+            sumsq = torch.stack([torch.linalg.vector_norm(g.detach(), 2.0) for g in grads]
+                                ).float().pow(2).sum()
+        else:
+            sumsq = torch.zeros((), dtype=torch.float32, device=params[0].device)
+        if self._norm_allreduce:
+            import torch.distributed as dist
+
+            dist.all_reduce(sumsq, group=self._norm_group)
+        norm = sumsq.sqrt()
+        coef = torch.clamp(self._max_norm / (norm + 1e-6), max=1.0)
+        for g in grads:
+            g.mul_(coef.to(g.dtype))
+        self._last_norm = norm
 
     def step(self, grad_scale: float = 1.0) -> None:
         if grad_scale != 1.0:
@@ -189,20 +443,59 @@ class TorchOptimizerAdapter:
                 for p in g["params"]:
                     if p.grad is not None:
                         p.grad.mul_(grad_scale)
+        if self._max_norm is not None:
+            self._clip()
+        self._last_lr = float(self.optimizer.param_groups[0]["lr"])
         self.optimizer.step()
         self.optimizer.zero_grad(set_to_none=False)
+        if self._scheduler is not None:
+            self._scheduler.step()
 
     def zero_grad(self, set_to_none: bool = False) -> None:
         self.optimizer.zero_grad(set_to_none=False)
 
+    def scalars(self) -> dict:
+        return dict(lr=self._last_lr if self.reports_scalars else None,
+                    grad_norm=None if self._last_norm is None else float(self._last_norm))
+
+    def step_count(self) -> int:
+        return int(self._scheduler.last_epoch) if self._scheduler is not None else 0
+
+    def set_step_count(self, k: int) -> None:
+        if self._scheduler is None:
+            return
+        self._scheduler.last_epoch = int(k)
+        for g in self.optimizer.param_groups:
+            g["lr"] = g["initial_lr"] * lr_factor(self._sched, int(k))
+        self._scheduler._last_lr = [g["lr"] for g in self.optimizer.param_groups]
+
     def state_dict(self):
-        return self.optimizer.state_dict()
+        sd = self.optimizer.state_dict()
+        if self._scheduler is not None:
+            sd = dict(sd, lr_schedule_step=self.step_count())
+        return sd
 
     def load_state_dict(self, sd):
+        sd = dict(sd)
+        k = sd.pop("lr_schedule_step", None)
         self.optimizer.load_state_dict(sd)
+        if k is not None:
+            self.set_step_count(int(k))
 
 
-def build_optimizer(module: nn.Module, optim_cfg: dict, prefer_fused: bool = True):
+def build_optimizer(module: nn.Module, optim_cfg: dict, prefer_fused: bool = True,
+                    lr_schedule: Optional[dict] = None, grad_clip: Optional[dict] = None):
+    """``lr_schedule = dict(type="constant"|"linear"|"cosine", warmup_steps=W, total_steps=T)``,
+    ``grad_clip = dict(max_norm=x)`` (L2): both optional, invalid values raise ValueError here."""
+    sched = check_lr_schedule(lr_schedule)
+    max_norm = check_grad_clip(grad_clip)
+    opt = _build_optimizer(module, optim_cfg, prefer_fused)
+    if sched is not None or max_norm is not None:
+        opt.configure(sched, max_norm)
+    return opt
+
+
+def _build_optimizer(module: nn.Module, optim_cfg: dict, prefer_fused: bool):
     cfg = dict(optim_cfg)
     optim_type = cfg.pop("optim_type", "SGD")
     params = [p for p in module.parameters() if p.requires_grad]

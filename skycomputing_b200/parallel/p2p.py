@@ -308,3 +308,60 @@ class FusedBoundaryManager:
         for r in self._regions:
             r.free()
         self._regions = []
+
+
+class GradNormExchange:
+    """Peer-memory all-reduce of ONE fp32 per step: the stages' shares of the squared gradient
+    norm, summed in pipeline-position order so that every rank computes a bit-identical clip
+    coefficient.  Runs inside the captured step (``optim_finalize`` kernel, csrc/kernels/
+    elementwise_sm100.cu, which also documents the slot protocol).
+
+    Every rank owns one small region in its own HBM (``flags[P]`` in the first 256 bytes, then
+    ``slots[2][P]`` fp32, double-buffered by epoch parity) and maps the regions of ALL other ranks,
+    not only of its neighbours.  The flag epoch and the error word are the boundary manager's: a
+    peer that never publishes makes the wait time out and sets error 4, which
+    ``Runner._check_boundary_health`` reports.  Collective: every rank of ``group`` constructs it.
+    """
+
+    def __init__(self, position: int, num_positions: int, rank_of_position: List[int],
+                 device: torch.device, epoch_ptr: int, error_ptr: int, group=None):
+        ext = nat.ext()
+        self.position, self.n_ranks = position, num_positions
+        self.device = device
+        self.epoch_ptr, self.error_ptr = epoch_ptr, error_ptr
+        self.nbytes = 256 + ((2 * num_positions * 4 + 255) // 256) * 256
+        self.ptr, handle = ext.ipc_alloc(self.nbytes)
+        self._opened: List[int] = []
+        mine = {"rank": dist.get_rank(group), "gpu": FusedBoundaryManager._gpu_uuid(device),
+                "handle": handle}
+        gathered: List[dict] = [None] * dist.get_world_size(group)  # type: ignore[list-item]
+        dist.all_gather_object(gathered, mine, group=group)
+        by_rank = {g["rank"]: g for g in gathered}
+        bases = []
+        for pos in range(num_positions):
+            r = rank_of_position[pos]
+            if pos == position:
+                bases.append(self.ptr)
+                continue
+            ext.enable_peer_access(FusedBoundaryManager._local_device_of(by_rank[r]["gpu"], r))
+            base = ext.ipc_open(by_rank[r]["handle"])
+            self._opened.append(base)
+            bases.append(base)
+        self._bases = torch.tensor(bases, dtype=torch.int64, device=device)
+        self.regions_ptr = self._bases.data_ptr()
+        torch.cuda.synchronize(device)
+        dist.barrier(group=group)   # every region is mapped before anybody may write into it
+
+    def close(self) -> None:
+        if not self.ptr:
+            return
+        ext = nat.ext()
+        torch.cuda.synchronize(self.device)
+        for p in self._opened:
+            try:
+                ext.ipc_close(p)
+            except Exception:
+                pass
+        self._opened = []
+        ext.dev_free(self.ptr)
+        self.ptr = 0

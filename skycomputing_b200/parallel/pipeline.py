@@ -117,7 +117,8 @@ class PipelineEngine(EngineBase):
             in_ok, out_ok = in_ok and shape_ok, out_ok and shape_ok
         if multi:
             flags: List[tuple] = [None] * dist.get_world_size(self.group)  # type: ignore[list-item]
-            dist.all_gather_object(flags, (self.s, in_ok, out_ok, hidden), group=self.group)
+            dist.all_gather_object(flags, (self.s, in_ok, out_ok, hidden, self._norm_info()),
+                                   group=self.group)
             by_stage = {f[0]: f for f in flags}
             if not self.is_first:
                 self.in_fused = want_fused and by_stage[self.s - 1][2] and in_ok
@@ -137,6 +138,7 @@ class PipelineEngine(EngineBase):
                 from .comm import TorchDistComm
 
                 self.comm = TorchDistComm(self.device, group=self.group)
+            self._setup_grad_norm(self.s, self.P, self.stage_to_rank, [f[4] for f in flags])
         # only an optimizer whose step() is pure device work may be captured (a torch.optim class
         # behind TorchOptimizerAdapter keeps host-side state and refreshes the bf16 shadows through
         # a host-side version check: replaying it would train on stale weights)
@@ -352,6 +354,9 @@ class PipelineEngine(EngineBase):
         if self.fused is not None:
             self.fused.end_of_backward()
         self._mark(("OPT", 0, "begin"))
+        if self.comm is not None and self._sends_before_optimizer():
+            self.comm.wait(self._pending_sends)
+            self._pending_sends = []
         self.optimizer.step()
         self._mark(("OPT", 0, "end"))
         if self.comm is not None:
@@ -422,6 +427,7 @@ class PipelineEngine(EngineBase):
     def close(self) -> None:
         if self.device.type == "cuda":
             torch.cuda.synchronize(self.device)  # nothing of ours may still touch a peer region
+        self._close_grad_norm()
         if self.fused is not None:
             self.fused.close()
             self.fused = None

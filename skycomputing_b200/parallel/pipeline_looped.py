@@ -143,7 +143,7 @@ class LoopedPipelineEngine(EngineBase):
             ok = ok and self.seq % 8 == 0 and hidden > 0 and hidden % 64 == 0 and \
                 (self.mb_batch * self.seq) % 128 == 0
         flags = [None] * dist.get_world_size(self.group)
-        dist.all_gather_object(flags, (bool(ok), int(hidden)), group=self.group)
+        dist.all_gather_object(flags, (bool(ok), int(hidden), self._norm_info()), group=self.group)
         if want_fused and all(f[0] for f in flags):
             from .p2p import FusedBoundaryManager
 
@@ -160,6 +160,8 @@ class LoopedPipelineEngine(EngineBase):
         if self.fused is None:
             # collective: one communicator per direction so crossed sends cannot dead-lock NCCL
             self._comm = TorchDistComm(self.device, group=self.group, directional=True)
+        # one optimizer over all local chunks (optim_module): one share of the norm per position
+        self._setup_grad_norm(self.pos, self.P, self.ring, [f[2] for f in flags])
         self._setup_done = True
 
     def _fused_inputs(self, slot: int):
@@ -303,6 +305,9 @@ class LoopedPipelineEngine(EngineBase):
                                                     with_meta=False)
         self._flush_wgrads()
         self._join_wgrads()
+        if self._sends_before_optimizer():
+            self.comm.wait(self._pending)
+            self._pending = []
         self.optimizer.step()
         self.comm.wait(self._pending)
         self._pending = []
@@ -360,6 +365,7 @@ class LoopedPipelineEngine(EngineBase):
     def close(self) -> None:
         if self.device.type == "cuda":
             torch.cuda.synchronize(self.device)
+        self._close_grad_norm()
         if self.fused is not None:
             self.fused.close()
             self.fused = None

@@ -14,7 +14,9 @@ WorkerManager carries unused elastic scaffolding (SURVEY §5.3).  This hook clos
    (``Runner.rebuild``).
 
 Everything is collective and deterministic (all ranks compute the same allocation from the same
-gathered numbers).  Plain-SGD state is nothing; momentum buffers are reset by a migration.
+gathered numbers).  Plain-SGD state is nothing; momentum buffers are reset by a migration.  The
+rebuilt optimizer gets the same learning-rate schedule / gradient clipping and continues the
+schedule at the step count of the old one (no second warmup).
 """
 import copy
 from typing import Callable, Optional
@@ -56,7 +58,8 @@ def _bottleneck(worker_manager, device_times: dict, layer_cost: list) -> float:
 class ReallocateHook(Hook):
     def __init__(self, interval: int, allocator_factory: Callable, optimizer_cfg: dict,
                  allocate_type: str = "dynamic", min_gain: float = 0.05,
-                 on_migrate: Optional[Callable] = None):
+                 on_migrate: Optional[Callable] = None, lr_schedule: Optional[dict] = None,
+                 grad_clip: Optional[dict] = None):
         """``allocator_factory(worker_manager) -> Allocator`` builds an allocator (with its model
         and device benchmarkers) around the given pool copy; ``optimizer_cfg`` is the
         ``train_config['optim_cfg']`` dict used to rebuild the optimizer after a migration."""
@@ -64,6 +67,8 @@ class ReallocateHook(Hook):
         self._interval = interval
         self._factory = allocator_factory
         self._optimizer_cfg = dict(optimizer_cfg)
+        self._lr_schedule = lr_schedule
+        self._grad_clip = grad_clip
         self._type = allocate_type
         self._min_gain = min_gain
         self._on_migrate = on_migrate
@@ -120,7 +125,11 @@ class ReallocateHook(Hook):
                 b, e = module.layer_range
                 module.load_weights([per_layer[i] for i in range(b, e)])
         model.train(True)
-        optimizer = build_optimizer(model.optim_module, dict(self._optimizer_cfg))
+        optimizer = build_optimizer(model.optim_module, dict(self._optimizer_cfg),
+                                    lr_schedule=self._lr_schedule, grad_clip=self._grad_clip)
+        old = runner.optimizer
+        if old is not None and hasattr(old, "step_count") and hasattr(optimizer, "set_step_count"):
+            optimizer.set_step_count(old.step_count())
         runner.rebuild(model, optimizer, worker_manager=new_wm)
         self.migrations += 1
         if self._on_migrate is not None:

@@ -351,8 +351,20 @@ class Runner:
         nseq = int(first.shape[0]) if torch.is_tensor(first) else 0
         if loss is not None:
             self._log("loss: {}".format(loss))
+        extra = {}
+        if getattr(self.optimizer, "reports_scalars", False):
+            # learning-rate schedule / clipping: this step's device scalars (the step has been
+            # synchronised above; the global norm is the same on every rank)
+            sc = self.optimizer.scalars()
+            if sc["lr"] is not None:
+                self._log("lr: {}".format(sc["lr"]))
+                extra["lr"] = sc["lr"]
+            if sc["grad_norm"] is not None:
+                self._log("grad norm: {}".format(sc["grad_norm"]))
+                extra["grad_norm"] = sc["grad_norm"]
         if self._metrics_path is not None:
             with open(self._metrics_path, "a") as f:
                 f.write(json.dumps(dict(epoch=self._epoch, iter=self._iter, step_seconds=step_s,
                                         sequences_per_s=(nseq / step_s if step_s > 0 else None),
-                                        forward_seconds=fwd, backward_seconds=bwd, loss=loss)) + "\n")
+                                        forward_seconds=fwd, backward_seconds=bwd, loss=loss,
+                                        **extra)) + "\n")

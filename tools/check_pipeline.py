@@ -30,6 +30,10 @@ def main():
     ap.add_argument("--virtual-stages", type=int, default=1)
     # "layer": the reference's granularity (cuts may fall after BertLayer_Head / Body)
     ap.add_argument("--granularity", default="block", choices=["block", "layer"])
+    # opt-in global-norm clipping / learning-rate schedule (warmup 2 steps, total = --steps):
+    # every rank then reports its grad_norm per step, which must be the same on all of them
+    ap.add_argument("--max-grad-norm", type=float, default=None)
+    ap.add_argument("--lr-schedule", default=None, choices=["constant", "linear", "cosine"])
     a = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -71,7 +75,11 @@ def main():
                 for n, p in layer.named_parameters():
                     if n.endswith("LayerNorm.weight"):
                         p.fill_(1.0)
-    opt = sky.build_optimizer(model.optim_module, dict(optim_type="SGD", lr=0.01))
+    step_cfg = dict(
+        lr_schedule=(dict(type=a.lr_schedule, warmup_steps=2, total_steps=a.steps)
+                     if a.lr_schedule else None),
+        grad_clip=dict(max_norm=a.max_grad_norm) if a.max_grad_norm is not None else None)
+    opt = sky.build_optimizer(model.optim_module, dict(optim_type="SGD", lr=0.01), **step_cfg)
     runner = sky.Runner(model=model, parameter_server=None, worker_manager=wm, optimizer=opt,
                         max_epochs=1, max_iters=10 ** 9, loss_cfg=dict(type="CrossEntropyLoss"),
                         timer_cfg=dict(root="/tmp/sky_check"), logging_cfg=None,
@@ -79,20 +87,23 @@ def main():
                         use_cuda_graph=not a.no_graph, device=dev)
     model.train(True)
     ds = sky.SynthMNLIDataset(num_samples=a.batch * 2, max_seq_length=128, seed=3, full_length=False)
-    losses = []
+    losses, norms = [], []
     for step in range(a.steps):
         sl = slice((step % 2) * a.batch, (step % 2 + 1) * a.batch)
         data = [ds.input_ids[sl], ds.segment_ids[sl], ds.input_mask[sl]]
         out = runner.train_iteration(data, ds.labels[sl])
         if out is not None:
             losses.append(round(out, 5))
+        if a.max_grad_norm is not None:
+            torch.cuda.synchronize()
+            norms.append(runner.optimizer.scalars()["grad_norm"])
     torch.cuda.synchronize()
     eng = runner.engine
     info = dict(tag=a.tag, world=world, boundary=a.boundary, schedule=eng.schedule,
                 virtual_stages=a.virtual_stages, fused=(eng.in_fused or eng.out_fused),
                 layers=[len(w.model_config) for w in wm.worker_pool],
                 graph=eng._graph is not None, mb=a.micro_batches, losses=losses,
-                err=eng.fused.error_code() if eng.fused is not None else 0)
+                err=eng.fused.error_code() if eng.fused is not None else 0, norms=norms)
     gathered = [None] * world
     dist.all_gather_object(gathered, info)
     if rank == 0:
@@ -100,6 +111,9 @@ def main():
         last["fused_any"] = any(g["fused"] for g in gathered)
         last["graph_all"] = all(g["graph"] for g in gathered)
         last["err_any"] = max(g["err"] for g in gathered)
+        if a.max_grad_norm is not None:
+            last["rank_norms"] = [g["norms"] for g in gathered]
+            last["norms_identical"] = all(g["norms"] == gathered[0]["norms"] for g in gathered)
         print("CHECK " + json.dumps(last), flush=True)
     eng.close()
     dist.destroy_process_group()
