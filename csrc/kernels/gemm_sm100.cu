@@ -2,15 +2,15 @@
 //
 //   out[M,N] = epilogue( sum_k A[m,k] * B[n,k] )      bf16 x bf16 -> fp32 (registers) -> bf16 | fp32
 //
-//   * operands staged by TMA (cp.async.bulk.tensor, SWIZZLE_128B) into a 3..5 deep smem ring by one
+//   * operands staged by TMA (cp.async.bulk.tensor, SWIZZLE_128B) into a 4..6 deep smem ring by one
 //     producer warp,
 //   * two consumer warpgroups, each issuing wgmma.mma_async m64 x BLOCK_N x 16 for its 64 rows of
 //     the 128 x BLOCK_N tile; the accumulators live in registers (setmaxnreg moves the producer
 //     warpgroup's registers to the consumers),
-//   * the epilogue walks the tile in 64-column groups: the fragments are transposed through a small
-//     fp32 staging tile in shared memory so that every thread owns 32 consecutive columns of ONE
-//     row, then bias / erf-GELU / GELU' / dropout / residual add are applied and the result is
-//     stored straight to global memory -- which may be the NEXT PIPELINE STAGE's HBM (peer pointer
+//   * the epilogue walks the tile in 64-column groups and applies bias / erf-GELU / GELU' /
+//     dropout / residual add to the accumulator fragments in registers; bf16 results pass a small
+//     per-warp staging buffer so that global stores stay whole 128-byte rows, fp32 results leave
+//     straight from the fragments.  The target may be the NEXT PIPELINE STAGE's HBM (peer pointer
 //     over NVLink); a per-128-row-panel flag is then bumped with red.release.sys so the consumer
 //     GPU can start on that panel while we still compute,
 //   * symmetric consumer side: the TMA producer can ld.acquire.sys-poll such flags before it
@@ -47,24 +47,120 @@ constexpr int MMA_K = 16;
 // warpgroups 1, 2 (warps 4-11): wgmma consumers + epilogue, 64 rows of the tile each
 constexpr int kNumThreads = 384;
 constexpr int kEpiWarp0 = 4;
-constexpr int kAccLd = 68;  // floats per row of the fp32 staging tile (64 columns + 16 B pad)
 constexpr uint64_t kFlagTimeoutNs = 4000000000ull;  // 4 s
+constexpr int kMaxSmemBytes = 227 * 1024;           // opt-in dynamic shared memory per block (H100)
+
+// Per-warp bf16 staging buffer of the epilogues: the warp's 16 fragment rows x 64 columns, rows
+// 144 B apart (128 B + 16 B pad).  With that stride both the fragment side (4-byte column pairs,
+// 8 rows x 4 lanes) and the global side (16-byte pieces, 8 lanes per row) are bank-conflict free.
+constexpr int kStageLd = 144;
+constexpr int kWarpStageBytes = 16 * kStageLd;
 
 template <int BLOCK_N>
 struct Cfg {
-  static constexpr int kStages = BLOCK_N == 256 ? 3 : 5;
+  static constexpr int kStages = BLOCK_N == 256 ? 4 : 6;
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
   static constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kBiasBytes = 2 * BLOCK_N * 4;  // double-buffered bias tile
-  static constexpr int kOutStageBytes = 8 * 32 * 80;  // per epilogue warp: 32 rows x (64+16) B
-  static constexpr int kAccStageBytes = BLOCK_M * kAccLd * 4;
+  static constexpr int kOutStageBytes = 8 * kWarpStageBytes;  // one buffer per epilogue warp
   static constexpr int kOffBars = kStages * kStageBytes;
   static constexpr int kOffBias = kOffBars + 256;
   static constexpr int kOffOut = kOffBias + kBiasBytes;
-  static constexpr int kOffAcc = kOffOut + kOutStageBytes;
-  static constexpr int kSmemBytes = kOffAcc + kAccStageBytes + 1024 /*align slack*/;
+  static constexpr int kSmemBytes = kOffOut + kOutStageBytes + 1024 /*align slack*/;
+  static_assert(kSmemBytes <= kMaxSmemBytes, "GEMM shared memory over the per-block limit");
 };
+
+// ---- epilogue on accumulator fragments ----
+// A consumer thread holds, of each 64-column group of its warpgroup's 64 x BLOCK_N accumulator,
+// f[4j], f[4j+1] = (row fr, columns 8j + fc + {0,1}) and f[4j+2], f[4j+3] = (row fr + 8, the same
+// columns), j = 0..7, with fr = lane / 4 and fc = 2 (lane % 4) (see acc_store_smem in
+// sm100_ptx.cuh).  Global memory is reached through the warp's staging buffer `s` for bf16 tiles
+// (coalesced 128-byte rows) and straight from the fragments for fp32 (a quad covers 32 contiguous
+// bytes of a row).  Column bounds are checked per 8-column block (one 16-byte bf16 piece, or the
+// block's column pairs in the fp32 stores); that is exact only because the launchers require
+// N % 8 == 0.  Relaxing that host check needs per-pair checks here first, or ragged tiles would
+// write past column N.
+
+// f (16 rows x 64 columns, bf16) -> gout rows grow0 .. grow0 + 15, columns col0 .. col0 + 63;
+// rows >= m and 8-column pieces >= n are skipped
+__device__ __forceinline__ void frag_store_bf16(const float (&f)[32], uint8_t* s, int lane,
+                                                __nv_bfloat16* gout, long long ld, long long grow0,
+                                                int m, int col0, int n) {
+  uint8_t* mine = s + (lane >> 2) * kStageLd + (lane & 3) * 4;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    *reinterpret_cast<uint32_t*>(mine + j * 16) = pack_bf16x2(f[4 * j], f[4 * j + 1]);
+    *reinterpret_cast<uint32_t*>(mine + 8 * kStageLd + j * 16) =
+        pack_bf16x2(f[4 * j + 2], f[4 * j + 3]);
+  }
+  __syncwarp();
+  const int piece = lane & 7;
+  if (col0 + piece * 8 < n) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int r = i * 4 + (lane >> 3);
+      if (grow0 + r < m) {
+        const uint4 val = *reinterpret_cast<const uint4*>(s + r * kStageLd + piece * 16);
+        *reinterpret_cast<uint4*>(gout + (grow0 + r) * ld + col0 + piece * 8) = val;
+      }
+    }
+  }
+  __syncwarp();
+}
+
+// coalesced global read of a bf16 16 x 64 block (issued early, it hides behind the epilogue math)
+__device__ __forceinline__ void aux_load(uint4 (&ax)[4], const __nv_bfloat16* aux, long long ld,
+                                         long long grow0, int m, int col0, int n, int lane) {
+  const int piece = lane & 7;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int r = i * 4 + (lane >> 3);
+    ax[i] = (grow0 + r < m && col0 + piece * 8 < n)
+                ? *reinterpret_cast<const uint4*>(aux + (grow0 + r) * ld + col0 + piece * 8)
+                : make_uint4(0, 0, 0, 0);
+  }
+}
+// ... -> staging -> fragment pairs: a[2j] = row fr, a[2j+1] = row fr + 8 (bf16x2 each)
+__device__ __forceinline__ void aux_to_frag(const uint4 (&ax)[4], uint8_t* s, int lane,
+                                            uint32_t (&a)[16]) {
+  const int piece = lane & 7;
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    *reinterpret_cast<uint4*>(s + (i * 4 + (lane >> 3)) * kStageLd + piece * 16) = ax[i];
+  __syncwarp();
+  const uint8_t* mine = s + (lane >> 2) * kStageLd + (lane & 3) * 4;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    a[2 * j] = *reinterpret_cast<const uint32_t*>(mine + j * 16);
+    a[2 * j + 1] = *reinterpret_cast<const uint32_t*>(mine + 8 * kStageLd + j * 16);
+  }
+  __syncwarp();
+}
+
+// dropout on fragments with the element-wise mask dropout_keep4(seed, (row * n + col) >> 2).
+// A 4-column group belongs to lanes l and l ^ 1: the even lane hashes it for row fr, the odd lane
+// for row fr + 8, and they swap results.
+__device__ __forceinline__ void frag_dropout(float (&f)[32], uint64_t seed, uint32_t thr16,
+                                             float scale, long long row_a, int col0, int n,
+                                             int lane) {
+  const int odd = lane & 1;
+  const uint64_t row = static_cast<uint64_t>(row_a + (odd ? 8 : 0));
+  const int c4 = col0 + (lane & 2) * 2;  // first column of my 4-column group in block 0
+  const uint32_t sh = odd * 2;           // my column pair's bits in the group's mask
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const uint32_t h =
+        dropout_keep4(seed, (row * static_cast<uint64_t>(n) + c4 + j * 8) >> 2, thr16);
+    const uint32_t o = __shfl_xor_sync(0xffffffffu, h, 1);
+    const uint32_t ma = (odd ? o : h) >> sh;
+    const uint32_t mb = (odd ? h : o) >> sh;
+    f[4 * j] = (ma & 1u) ? f[4 * j] * scale : 0.f;
+    f[4 * j + 1] = (ma & 2u) ? f[4 * j + 1] * scale : 0.f;
+    f[4 * j + 2] = (mb & 1u) ? f[4 * j + 2] * scale : 0.f;
+    f[4 * j + 3] = (mb & 2u) ? f[4 * j + 3] * scale : 0.f;
+  }
+}
 
 struct GemmDev {
   int M, N, K;
@@ -225,7 +321,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   uint64_t* empty_bar = bars + kStages;  // [kStages]
   uint32_t* s_ticket = reinterpret_cast<uint32_t*>(bars + 2 * kStages);
   float* s_bias = reinterpret_cast<float*>(smem + C::kOffBias);
-  float* s_acc = reinterpret_cast<float*>(smem + C::kOffAcc);
 
   const int warp_idx = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
@@ -356,20 +451,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   } else {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     // ============================ consumers: wgmma main loop + epilogue ============================
-    // Main loop: warpgroup wg owns rows 64 wg .. 64 wg + 63 of the tile.  Epilogue: warp e handles
-    // rows 32 (e & 3) .. + 31 and, of every 64-column group, columns 32 (e >> 2) .. + 31; a lane
-    // owns one ROW of those.  Latency hiding: bias for the tile is staged once in shared memory,
-    // aux (residual / pre-activation) chunks are loaded before the staging barriers, fp32 gradient
-    // accumulation uses red.global.add.v4.f32 (no read-modify-write).
+    // Warpgroup wg owns rows 64 wg .. 64 wg + 63 of the tile, warp q of it rows 16 q .. 16 q + 15.
+    // The epilogue runs on the accumulator fragments in registers, 64 columns at a time; bias for
+    // the tile is staged once in shared memory, aux (residual / pre-activation) blocks are loaded
+    // before the epilogue math, fp32 gradient accumulation uses red.global.add (no
+    // read-modify-write).
     const int e = warp_idx - kEpiWarp0;
     const int q = e & 3;
-    const int half = e >> 2;
     const int wg = e >> 2;  // consumer warpgroup 0 / 1
     const int epi_tid = threadIdx.x - kEpiWarp0 * 32;  // 0..255
     const int wg_tid = epi_tid & 127;
     const bool elected = wg_tid == 0;
-    uint8_t* s_stage = smem + C::kOffOut + e * (32 * 80);
-    const int row_in_tile = q * 32 + lane;
+    uint8_t* s_stage = smem + C::kOffOut + e * kWarpStageBytes;
+    const int fr = lane >> 2;        // fragment rows fr and fr + 8 of the warp's 16
+    const int fc = (lane & 3) * 2;   // fragment column pair inside every 8-column block
+    const int warp_row_in_tile = wg * 64 + q * 16;
     const bool has_dropout = p.dropout_p > 0.f;
     const bool has_aux = p.aux != nullptr;
     uint64_t seed = 0;
@@ -396,8 +492,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       const int tile = w.tile;
       const int m_blk = (tile % num_m_units) * (PAIR ? 2 : 1) + static_cast<int>(cta_rank);
       const int n_blk = (tile / num_m_units) * (MC ? 2 : 1) + (MC ? static_cast<int>(pair_idx) : 0);
-      const long long row = static_cast<long long>(m_blk) * BLOCK_M + row_in_tile;
-      const bool row_ok = row < p.M;
+      const long long warp_row0 = static_cast<long long>(m_blk) * BLOCK_M + warp_row_in_tile;
+      const long long row_a = warp_row0 + fr;  // and row_a + 8
       // ---- stage bias (overlaps the main loop of the other warpgroup) ----
       float* sb = s_bias + (it & 1) * BLOCK_N;
       if (epi_tid < BLOCK_N) {
@@ -446,162 +542,112 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
           asm volatile("bar.sync 1, 256;" ::: "memory");
         }
       }
-      // workspace layout of one 128 x BLOCK_N tile: [column / 4][row][4] floats, so that the 32
-      // lanes (= 32 rows) of a warp touch 512 contiguous bytes per float4 access
-      auto ws_ptr = [&](float* base, int ct) {
-        return reinterpret_cast<float4*>(base) + (ct >> 2) * BLOCK_M + row_in_tile;
+      // workspace layout of one 128 x BLOCK_N tile: [8-column block][consumer thread][4] floats,
+      // the fragment registers as they are, so that a warp's float4 accesses are contiguous
+      auto ws_ptr = [&](float* base, int j) {
+        return reinterpret_cast<float4*>(base) + j * 256 + epi_tid;
       };
+      // every consumer thread has staged its share of this tile's bias (and, through the barrier of
+      // the previous tile, nobody still reads the buffer that was overwritten)
+      asm volatile("bar.sync 1, 256;" ::: "memory");
 
-      // bf16 stores go through a per-warp smem transpose: a lane owns one accumulator ROW, so
-      // storing straight from registers makes every STG.128 touch 32 different rows (32 partial
-      // sectors per request).  Staged, a warp store covers 8 rows x 64 contiguous bytes.
-      // Row stride 80 B keeps both the row-wise writes and the 4-lanes-per-row reads (nearly)
-      // bank-conflict free.
-      const long long warp_row0 = static_cast<long long>(m_blk) * BLOCK_M + q * 32;
-      auto store_bf16_chunk = [&](const float (&f)[32], __nv_bfloat16* gout, long long ld,
-                                  int col0) {
-        uint8_t* mine = s_stage + lane * 80;
 #pragma unroll
-        for (int j = 0; j < 32; j += 8) {
-          uint4 pk;
-          pk.x = pack_bf16x2(f[j], f[j + 1]);
-          pk.y = pack_bf16x2(f[j + 2], f[j + 3]);
-          pk.z = pack_bf16x2(f[j + 4], f[j + 5]);
-          pk.w = pack_bf16x2(f[j + 6], f[j + 7]);
-          *reinterpret_cast<uint4*>(mine + j * 2) = pk;
-        }
-        __syncwarp();
-        const int piece = lane & 3;
-        if (col0 + piece * 8 < p.N) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int r = i * 8 + (lane >> 2);
-            if (warp_row0 + r < p.M) {
-              const uint4 val = *reinterpret_cast<const uint4*>(s_stage + r * 80 + piece * 16);
-              *reinterpret_cast<uint4*>(gout + (warp_row0 + r) * ld + col0 + piece * 8) = val;
-            }
-          }
-        }
-        __syncwarp();
-      };
-
-      // ct = first of my 32 columns inside the tile
-      auto process = [&](uint32_t (&v)[32], const uint4 (&ax)[4], int ct) {
+      for (int g = 0; g < BLOCK_N / 64; ++g) {
+        const int ct = g * 64;  // first column of the group inside the tile
         const int col0 = n_blk * BLOCK_N + ct;
-        if (col0 >= p.N || p.debug == 1 || p.debug >= 3) return;  // warp-uniform
+        if (col0 >= p.N || p.debug == 1 || p.debug >= 3) continue;  // uniform across the CTA
+        uint4 ax[4];
+        if (has_aux) aux_load(ax, p.aux, p.ldaux, warp_row0, p.M, col0, p.N, lane);
+        float f[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) f[i] = acc[g * 32 + i];
         if (partial) {
           if (!finisher) {
-            float4* wp = ws_ptr(ws_mine, ct);
 #pragma unroll
             for (int j = 0; j < 8; ++j)
-              wp[j * BLOCK_M] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                            __uint_as_float(v[4 * j + 2]),
-                                            __uint_as_float(v[4 * j + 3]));
-            return;
+              *ws_ptr(ws_mine, g * 8 + j) =
+                  make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
+            continue;
           }
           for (int u = u_first; u < u_first + n_contrib; ++u) {
             if (u == unit_id) continue;
             const int which_u = (tile == sched.first_tile(u)) ? 0 : 1;
-            const float4* rp = ws_ptr(
-                p.ws + static_cast<size_t>((2 * u + which_u) * kCtasPerUnit + cl_rank) * kTileElems,
-                ct);
+            float* base =
+                p.ws + static_cast<size_t>((2 * u + which_u) * kCtasPerUnit + cl_rank) * kTileElems;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-              const float4 x = __ldcg(rp + j * BLOCK_M);
-              v[4 * j] = __float_as_uint(__uint_as_float(v[4 * j]) + x.x);
-              v[4 * j + 1] = __float_as_uint(__uint_as_float(v[4 * j + 1]) + x.y);
-              v[4 * j + 2] = __float_as_uint(__uint_as_float(v[4 * j + 2]) + x.z);
-              v[4 * j + 3] = __float_as_uint(__uint_as_float(v[4 * j + 3]) + x.w);
+              const float4 x = __ldcg(ws_ptr(base, g * 8 + j));
+              f[4 * j] = f[4 * j] + x.x;
+              f[4 * j + 1] = f[4 * j + 1] + x.y;
+              f[4 * j + 2] = f[4 * j + 2] + x.z;
+              f[4 * j + 3] = f[4 * j + 3] + x.w;
             }
           }
         }
-        float f[32];
-        const float4* sb4 = reinterpret_cast<const float4*>(sb + ct);
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          const float4 bb = sb4[j >> 2];  // smem broadcast
-          f[j] = __uint_as_float(v[j]) + bb.x;
-          f[j + 1] = __uint_as_float(v[j + 1]) + bb.y;
-          f[j + 2] = __uint_as_float(v[j + 2]) + bb.z;
-          f[j + 3] = __uint_as_float(v[j + 3]) + bb.w;
+        for (int j = 0; j < 8; ++j) {
+          const float2 bb = *reinterpret_cast<const float2*>(sb + ct + j * 8 + fc);  // broadcast
+          f[4 * j] = f[4 * j] + bb.x;
+          f[4 * j + 1] = f[4 * j + 1] + bb.y;
+          f[4 * j + 2] = f[4 * j + 2] + bb.x;
+          f[4 * j + 3] = f[4 * j + 3] + bb.y;
         }
         if (p.act == ACT_GELU) {
           if (p.out2 != nullptr && p.debug != 2)
-            store_bf16_chunk(f, reinterpret_cast<__nv_bfloat16*>(p.out2), p.ldo2, col0);
+            frag_store_bf16(f, s_stage, lane, reinterpret_cast<__nv_bfloat16*>(p.out2), p.ldo2,
+                            warp_row0, p.M, col0, p.N);
 #pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = gelu_fast(f[j]);
+          for (int i = 0; i < 32; ++i) f[i] = gelu_fast(f[i]);
         } else if (p.act == ACT_TANH) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = tanh_fast(f[j]);
+          for (int i = 0; i < 32; ++i) f[i] = tanh_fast(f[i]);
         }
-        if (has_dropout) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const uint64_t idx4 = (static_cast<uint64_t>(row) * p.N + col0 + j) >> 2;
-            const uint32_t m = dropout_keep4(seed, idx4, thr16);
-            f[j] = (m & 1u) ? f[j] * drop_scale : 0.f;
-            f[j + 1] = (m & 2u) ? f[j + 1] * drop_scale : 0.f;
-            f[j + 2] = (m & 4u) ? f[j + 2] * drop_scale : 0.f;
-            f[j + 3] = (m & 8u) ? f[j + 3] * drop_scale : 0.f;
-          }
-        }
+        if (has_dropout) frag_dropout(f, seed, thr16, drop_scale, row_a, col0, p.N, lane);
         if (has_aux) {
+          uint32_t aw[16];
+          aux_to_frag(ax, s_stage, lane, aw);
 #pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            const uint32_t aw[4] = {ax[t].x, ax[t].y, ax[t].z, ax[t].w};
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              const float2 x = unpack_bf16x2(aw[u]);
-              const int j = t * 8 + u * 2;
-              if (p.act == ACT_DGELU_MUL_AUX) {
-                f[j] *= dgelu_fast(x.x);
-                f[j + 1] *= dgelu_fast(x.y);
-              } else if (p.add_aux) {
-                f[j] += x.x;
-                f[j + 1] += x.y;
-              }
+          for (int j = 0; j < 8; ++j) {
+            const float2 xa = unpack_bf16x2(aw[2 * j]);
+            const float2 xb = unpack_bf16x2(aw[2 * j + 1]);
+            if (p.act == ACT_DGELU_MUL_AUX) {
+              f[4 * j] *= dgelu_fast(xa.x);
+              f[4 * j + 1] *= dgelu_fast(xa.y);
+              f[4 * j + 2] *= dgelu_fast(xb.x);
+              f[4 * j + 3] *= dgelu_fast(xb.y);
+            } else if (p.add_aux) {
+              f[4 * j] += xa.x;
+              f[4 * j + 1] += xa.y;
+              f[4 * j + 2] += xb.x;
+              f[4 * j + 3] += xb.y;
             }
           }
         }
         if (p.debug != 2) {
           if constexpr (OUT_F32) {
-            if (row_ok) {
-              float* o = reinterpret_cast<float*>(p.out) + row * p.ldo + col0;
 #pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                if (col0 + j < p.N) {
-                  if (p.accumulate)
-                    red_add_v4_f32(o + j, f[j], f[j + 1], f[j + 2], f[j + 3]);
-                  else
-                    *reinterpret_cast<float4*>(o + j) =
-                        make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
+            for (int h = 0; h < 2; ++h) {
+              const long long row = row_a + 8 * h;
+              if (row < p.M) {
+                float* o = reinterpret_cast<float*>(p.out) + row * p.ldo + col0 + fc;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                  // covers columns fc, fc + 1 only because N % 8 == 0 (launch_gemm checks it)
+                  if (col0 + j * 8 < p.N) {
+                    if (p.accumulate)
+                      red_add_v2_f32(o + j * 8, f[4 * j + 2 * h], f[4 * j + 2 * h + 1]);
+                    else
+                      *reinterpret_cast<float2*>(o + j * 8) =
+                          make_float2(f[4 * j + 2 * h], f[4 * j + 2 * h + 1]);
+                  }
                 }
               }
             }
           } else {
-            store_bf16_chunk(f, reinterpret_cast<__nv_bfloat16*>(p.out), p.ldo, col0);
+            frag_store_bf16(f, s_stage, lane, reinterpret_cast<__nv_bfloat16*>(p.out), p.ldo,
+                            warp_row0, p.M, col0, p.N);
           }
         }
-      };
-
-#pragma unroll
-      for (int g = 0; g < BLOCK_N / 64; ++g) {
-        const int ct = g * 64 + half * 32;
-        uint4 ax[4];
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const int col = n_blk * BLOCK_N + ct + t * 8;
-          ax[t] = (has_aux && row_ok && col < p.N)
-                      ? *reinterpret_cast<const uint4*>(p.aux + row * p.ldaux + col)
-                      : make_uint4(0, 0, 0, 0);
-        }
-        // every reader of the previous group is done (g == 0: and this tile's bias is staged)
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        acc_store_smem<64>(acc, g * 64, s_acc, kAccLd, wg * 64, 0, wg_tid);
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        uint32_t v[32];
-        row_load32(s_acc + row_in_tile * kAccLd + half * 32, v);
-        process(v, ax, ct);
       }
       if (partial && !finisher) {
         // publish the parked partial: all stores -> fence -> barrier -> one counter bump
@@ -635,12 +681,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
 // CTAs that own the column tiles of one 128-row panel form a THREAD-BLOCK CLUSTER (2..8 CTAs) and
 // exchange per-row partial sums through distributed shared memory:
 //
-//   pass 1  accumulators -> row owners (through the fp32 staging tile): + bias, dropout,
-//           + residual; store z (bf16, saved for backward); accumulate row sum / sum of squares;
-//           the fp32 sums go BACK into the accumulator registers the same way
-//   DSMEM   every row-owner thread stores its (sum, sumsq) into ALL CTAs of the cluster
+//   pass 1  on the accumulator fragments: + bias, dropout, + residual; store z (bf16, saved for
+//           backward); accumulate row sum / sum of squares (the quad that holds a row combines
+//           them with two shuffles); the fp32 sums stay in the accumulator registers
+//   DSMEM   one thread per row stores the row's (sum, sumsq) into ALL CTAs of the cluster
 //           (st.shared::cluster) and arrives on their mbarriers (release.cluster)
-//   pass 2  accumulators -> row owners again: normalise with the cluster-wide statistics,
+//   pass 2  on the fragments again: normalise with the cluster-wide statistics,
 //           gamma / beta, store y - straight into the NEXT PIPELINE STAGE's HBM when y is a peer
 //           pointer, then one red.release.sys per CTA on the panel flag.
 //
@@ -683,8 +729,8 @@ struct LnCfg {
   static constexpr int kOffVec = kOffBars + 256;
   static constexpr int kOffOut = kOffVec + kVecBytes;
   static constexpr int kOffStats = kOffOut + C::kOutStageBytes;
-  static constexpr int kOffAcc = kOffStats + kStatsBytes;
-  static constexpr int kSmemBytes = kOffAcc + C::kAccStageBytes + 1024 /*align slack*/;
+  static constexpr int kSmemBytes = kOffStats + kStatsBytes + 1024 /*align slack*/;
+  static_assert(kSmemBytes <= kMaxSmemBytes, "GEMM + LayerNorm shared memory over the per-block limit");
 };
 
 template <int BLOCK_N>
@@ -711,7 +757,6 @@ gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   float* s_gamma = s_bias + BLOCK_N;
   float* s_beta = s_gamma + BLOCK_N;
   float2* s_stats = reinterpret_cast<float2*>(smem + L::kOffStats);   // [cln][128]
-  float* s_acc = reinterpret_cast<float*>(smem + L::kOffAcc);
 
   const int warp_idx = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
@@ -769,17 +814,20 @@ gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   } else {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     // ============================ consumers: wgmma main loop + epilogue ============================
+    // warpgroup wg owns rows 64 wg .. + 63 of the panel, warp q of it rows 16 q .. + 15; the whole
+    // epilogue runs on the accumulator fragments (rows fr and fr + 8 of the warp, see
+    // frag_store_bf16)
     const int e = warp_idx - kEpiWarp0;
     const int q = e & 3;
-    const int half = e >> 2;
     const int wg = e >> 2;
     const int epi_tid = threadIdx.x - kEpiWarp0 * 32;
     const int wg_tid = epi_tid & 127;
-    uint8_t* s_out = smem + L::kOffOut;
-    uint8_t* s_stage = s_out + e * (32 * 80);
-    const int row_in_tile = q * 32 + lane;
-    const long long row = static_cast<long long>(m_blk) * BLOCK_M + row_in_tile;
-    const bool row_ok = row < p.M;
+    uint8_t* s_stage = smem + L::kOffOut + e * kWarpStageBytes;
+    const int fr = lane >> 2;
+    const int fc = (lane & 3) * 2;
+    const int warp_row_in_tile = wg * 64 + q * 16;
+    const long long warp_row0 = static_cast<long long>(m_blk) * BLOCK_M + warp_row_in_tile;
+    const long long row_a = warp_row0 + fr;  // and row_a + 8
     const bool has_dropout = p.dropout_p > 0.f;
     const bool has_aux = p.aux != nullptr;
     uint64_t seed = 0;
@@ -805,150 +853,115 @@ gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
           acc, 0, num_k_blks, smem_u32(smem_a) + wg * 8192, smem_u32(smem_b), C::kABytes,
           C::kBBytes, full_bar, empty_bar, stage, phase, wg_tid == 0, false);
     }
-
-    const long long warp_row0 = static_cast<long long>(m_blk) * BLOCK_M + q * 32;
-    auto store_bf16_chunk = [&](const float (&f)[32], __nv_bfloat16* gout, long long ld, int col0) {
-      uint8_t* mine = s_stage + lane * 80;
-#pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        uint4 pk;
-        pk.x = pack_bf16x2(f[j], f[j + 1]);
-        pk.y = pack_bf16x2(f[j + 2], f[j + 3]);
-        pk.z = pack_bf16x2(f[j + 4], f[j + 5]);
-        pk.w = pack_bf16x2(f[j + 6], f[j + 7]);
-        *reinterpret_cast<uint4*>(mine + j * 2) = pk;
-      }
-      __syncwarp();
-      const int piece = lane & 3;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = i * 8 + (lane >> 2);
-        if (warp_row0 + r < p.M) {
-          const uint4 val = *reinterpret_cast<const uint4*>(s_stage + r * 80 + piece * 16);
-          *reinterpret_cast<uint4*>(gout + (warp_row0 + r) * ld + col0 + piece * 8) = val;
-        }
-      }
-      __syncwarp();
-    };
+    asm volatile("bar.sync 1, 256;" ::: "memory");   // bias / gamma / beta staged
 
     // ---------------- pass 1: z = dropout(acc + bias) + residual; row statistics ----------------
-    float s1 = 0.f, s2 = 0.f;
-    float* my_row = s_acc + row_in_tile * kAccLd + half * 32;
+    // the fp32 sums stay in the accumulator registers for pass 2
+    float s1a = 0.f, s2a = 0.f, s1b = 0.f, s2b = 0.f;   // rows fr / fr + 8
 #pragma unroll
     for (int g = 0; g < BLOCK_N / 64; ++g) {
-      const int ct = g * 64 + half * 32;
+      const int ct = g * 64;
       const int col0 = static_cast<int>(n_blk) * BLOCK_N + ct;
       uint4 ax[4];
-#pragma unroll
-      for (int t = 0; t < 4; ++t)
-        ax[t] = (has_aux && row_ok)
-                    ? *reinterpret_cast<const uint4*>(p.aux + row * p.ldaux + col0 + t * 8)
-                    : make_uint4(0, 0, 0, 0);
-      asm volatile("bar.sync 1, 256;" ::: "memory");   // g == 0: bias / gamma / beta staged
-      acc_store_smem<64>(acc, g * 64, s_acc, kAccLd, wg * 64, 0, wg_tid);
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      uint32_t v[32];
-      row_load32(my_row, v);
+      if (has_aux) aux_load(ax, p.aux, p.ldaux, warp_row0, p.M, col0, p.N, lane);
       float f[32];
-      const float4* sb4 = reinterpret_cast<const float4*>(s_bias + ct);
 #pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const float4 bb = sb4[j >> 2];
-        f[j] = __uint_as_float(v[j]) + bb.x;
-        f[j + 1] = __uint_as_float(v[j + 1]) + bb.y;
-        f[j + 2] = __uint_as_float(v[j + 2]) + bb.z;
-        f[j + 3] = __uint_as_float(v[j + 3]) + bb.w;
+      for (int j = 0; j < 8; ++j) {
+        const float2 bb = *reinterpret_cast<const float2*>(s_bias + ct + j * 8 + fc);
+        f[4 * j] = acc[g * 32 + 4 * j] + bb.x;
+        f[4 * j + 1] = acc[g * 32 + 4 * j + 1] + bb.y;
+        f[4 * j + 2] = acc[g * 32 + 4 * j + 2] + bb.x;
+        f[4 * j + 3] = acc[g * 32 + 4 * j + 3] + bb.y;
       }
-      if (has_dropout) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          const uint64_t idx4 = (static_cast<uint64_t>(row) * p.N + col0 + j) >> 2;
-          const uint32_t m = dropout_keep4(seed, idx4, thr16);
-          f[j] = (m & 1u) ? f[j] * drop_scale : 0.f;
-          f[j + 1] = (m & 2u) ? f[j + 1] * drop_scale : 0.f;
-          f[j + 2] = (m & 4u) ? f[j + 2] * drop_scale : 0.f;
-          f[j + 3] = (m & 8u) ? f[j + 3] * drop_scale : 0.f;
-        }
-      }
+      if (has_dropout) frag_dropout(f, seed, thr16, drop_scale, row_a, col0, p.N, lane);
       if (has_aux) {
+        uint32_t aw[16];
+        aux_to_frag(ax, s_stage, lane, aw);
 #pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const uint32_t aw[4] = {ax[t].x, ax[t].y, ax[t].z, ax[t].w};
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const float2 x = unpack_bf16x2(aw[u]);
-            f[t * 8 + u * 2] += x.x;
-            f[t * 8 + u * 2 + 1] += x.y;
-          }
+        for (int j = 0; j < 8; ++j) {
+          const float2 xa = unpack_bf16x2(aw[2 * j]);
+          const float2 xb = unpack_bf16x2(aw[2 * j + 1]);
+          f[4 * j] += xa.x;
+          f[4 * j + 1] += xa.y;
+          f[4 * j + 2] += xb.x;
+          f[4 * j + 3] += xb.y;
         }
       }
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        s1 += f[j];
-        s2 = fmaf(f[j], f[j], s2);
-        v[j] = __float_as_uint(f[j]);
+      for (int j = 0; j < 8; ++j) {
+        s1a += f[4 * j] + f[4 * j + 1];
+        s2a = fmaf(f[4 * j], f[4 * j], fmaf(f[4 * j + 1], f[4 * j + 1], s2a));
+        s1b += f[4 * j + 2] + f[4 * j + 3];
+        s2b = fmaf(f[4 * j + 2], f[4 * j + 2], fmaf(f[4 * j + 3], f[4 * j + 3], s2b));
       }
-      row_store32(my_row, v);   // the fp32 sum returns to the accumulator registers
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[g * 32 + i] = f[i];
       if (p.z != nullptr)
-        store_bf16_chunk(f, reinterpret_cast<__nv_bfloat16*>(p.z), p.ldz, col0);
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      acc_load_smem<64>(acc, g * 64, s_acc, kAccLd, wg * 64, 0, wg_tid);
+        frag_store_bf16(f, s_stage, lane, reinterpret_cast<__nv_bfloat16*>(p.z), p.ldz, warp_row0,
+                        p.M, col0, p.N);
     }
     // ---------------- cluster-wide row statistics through distributed shared memory ----------------
-    // the two column halves of a row live in warps e and e + 4: combine them through the (now
-    // idle) output staging area, then the half-0 thread of each row publishes to every CTA
-    float2* s_half = reinterpret_cast<float2*>(s_out);
-    asm volatile("bar.sync 1, 256;" ::: "memory");   // every warp is done with its staging slice
-    if (half == 1) s_half[row_in_tile] = make_float2(s1, s2);
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    if (half == 0) {
-      const float2 o = s_half[row_in_tile];
-      s1 += o.x;
-      s2 += o.y;
-      const uint32_t slot = smem_u32(&s_stats[n_blk * BLOCK_M + row_in_tile]);
+    // a row of this CTA's BLOCK_N columns lives in one quad: two shuffles give its sums, then lane
+    // 0 (row fr) and lane 1 (row fr + 8) of the quad publish them to every CTA of the cluster
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      s1a += __shfl_xor_sync(0xffffffffu, s1a, o);
+      s2a += __shfl_xor_sync(0xffffffffu, s2a, o);
+      s1b += __shfl_xor_sync(0xffffffffu, s1b, o);
+      s2b += __shfl_xor_sync(0xffffffffu, s2b, o);
+    }
+    const int row_a_in_tile = warp_row_in_tile + fr;
+    if ((lane & 3) < 2) {
+      const int hb = lane & 1;
+      const uint32_t slot = smem_u32(&s_stats[n_blk * BLOCK_M + row_a_in_tile + 8 * hb]);
       const uint32_t bar = smem_u32(stats_bar);
+      const float v1 = hb ? s1b : s1a;
+      const float v2 = hb ? s2b : s2a;
       for (uint32_t r = 0; r < cln; ++r) {
-        st_cluster_v2_f32(mapa_shared(slot, r), s1, s2);
+        st_cluster_v2_f32(mapa_shared(slot, r), v1, v2);
         mbar_arrive_cluster(mapa_shared(bar, r));
       }
     }
     mbar_wait_cluster(stats_bar, 0);
-    float t1 = 0.f, t2 = 0.f;
+    float t1a = 0.f, t2a = 0.f, t1b = 0.f, t2b = 0.f;
     for (uint32_t r = 0; r < cln; ++r) {
-      const float2 o = s_stats[r * BLOCK_M + row_in_tile];
-      t1 += o.x;
-      t2 += o.y;
+      const float2 oa = s_stats[r * BLOCK_M + row_a_in_tile];
+      const float2 ob = s_stats[r * BLOCK_M + row_a_in_tile + 8];
+      t1a += oa.x;
+      t2a += oa.y;
+      t1b += ob.x;
+      t2b += ob.y;
     }
     const float inv_n = 1.f / static_cast<float>(p.N);
-    const float mean = t1 * inv_n;
-    const float var = fmaxf(fmaf(-mean, mean, t2 * inv_n), 0.f);
-    const float rstd = rsqrtf(var + p.eps);
-    if (n_blk == 0 && half == 0 && row_ok) {
-      p.mean[row] = mean;
-      p.rstd[row] = rstd;
+    const float mean_a = t1a * inv_n;
+    const float rstd_a = rsqrtf(fmaxf(fmaf(-mean_a, mean_a, t2a * inv_n), 0.f) + p.eps);
+    const float mean_b = t1b * inv_n;
+    const float rstd_b = rsqrtf(fmaxf(fmaf(-mean_b, mean_b, t2b * inv_n), 0.f) + p.eps);
+    if (n_blk == 0 && (lane & 3) < 2) {
+      const int hb = lane & 1;
+      const long long row = row_a + 8 * hb;
+      if (row < p.M) {
+        p.mean[row] = hb ? mean_b : mean_a;
+        p.rstd[row] = hb ? rstd_b : rstd_a;
+      }
     }
     // ---------------- pass 2: normalise, gamma / beta, store y (possibly into a peer GPU) ----------------
 #pragma unroll
     for (int g = 0; g < BLOCK_N / 64; ++g) {
-      const int ct = g * 64 + half * 32;
+      const int ct = g * 64;
       const int col0 = static_cast<int>(n_blk) * BLOCK_N + ct;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      acc_store_smem<64>(acc, g * 64, s_acc, kAccLd, wg * 64, 0, wg_tid);
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      uint32_t v[32];
-      row_load32(my_row, v);
       float f[32];
-      const float4* g4 = reinterpret_cast<const float4*>(s_gamma + ct);
-      const float4* b4 = reinterpret_cast<const float4*>(s_beta + ct);
 #pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const float4 gm = g4[j >> 2], b = b4[j >> 2];
-        f[j] = fmaf((__uint_as_float(v[j]) - mean) * rstd, gm.x, b.x);
-        f[j + 1] = fmaf((__uint_as_float(v[j + 1]) - mean) * rstd, gm.y, b.y);
-        f[j + 2] = fmaf((__uint_as_float(v[j + 2]) - mean) * rstd, gm.z, b.z);
-        f[j + 3] = fmaf((__uint_as_float(v[j + 3]) - mean) * rstd, gm.w, b.w);
+      for (int j = 0; j < 8; ++j) {
+        const float2 gm = *reinterpret_cast<const float2*>(s_gamma + ct + j * 8 + fc);
+        const float2 bt = *reinterpret_cast<const float2*>(s_beta + ct + j * 8 + fc);
+        f[4 * j] = fmaf((acc[g * 32 + 4 * j] - mean_a) * rstd_a, gm.x, bt.x);
+        f[4 * j + 1] = fmaf((acc[g * 32 + 4 * j + 1] - mean_a) * rstd_a, gm.y, bt.y);
+        f[4 * j + 2] = fmaf((acc[g * 32 + 4 * j + 2] - mean_b) * rstd_b, gm.x, bt.x);
+        f[4 * j + 3] = fmaf((acc[g * 32 + 4 * j + 3] - mean_b) * rstd_b, gm.y, bt.y);
       }
-      store_bf16_chunk(f, reinterpret_cast<__nv_bfloat16*>(p.y), p.ldy, col0);
+      frag_store_bf16(f, s_stage, lane, reinterpret_cast<__nv_bfloat16*>(p.y), p.ldy, warp_row0,
+                      p.M, col0, p.N);
     }
     if (p.signal_flags != nullptr) {
       // publish this CTA's 128 x BLOCK_N tile of the panel: stores -> fence -> barrier -> one

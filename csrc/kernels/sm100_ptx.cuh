@@ -304,21 +304,6 @@ __device__ __forceinline__ void acc_store_smem(const float (&d)[NREG], int C0, f
         make_float2(d[(C0 / 8 + j) * 4 + 2], d[(C0 / 8 + j) * 4 + 3]);
   }
 }
-template <int NC, int NREG>
-__device__ __forceinline__ void acc_load_smem(float (&d)[NREG], int C0, const float* src, int ld,
-                                              int row0, int col0, int wg_tid) {
-  const int r = row0 + (wg_tid >> 5) * 16 + ((wg_tid & 31) >> 2);
-  const float* p0 = src + r * ld + col0 + (wg_tid & 3) * 2;
-#pragma unroll
-  for (int j = 0; j < NC / 8; ++j) {
-    const float2 a = *reinterpret_cast<const float2*>(p0 + j * 8);
-    const float2 b = *reinterpret_cast<const float2*>(p0 + 8 * ld + j * 8);
-    d[(C0 / 8 + j) * 4] = a.x;
-    d[(C0 / 8 + j) * 4 + 1] = a.y;
-    d[(C0 / 8 + j) * 4 + 2] = b.x;
-    d[(C0 / 8 + j) * 4 + 3] = b.y;
-  }
-}
 // 32 consecutive floats of one staged row -> registers
 __device__ __forceinline__ void row_load32(const float* src, uint32_t (&v)[32]) {
 #pragma unroll
@@ -339,11 +324,6 @@ __device__ __forceinline__ void row_load16(const float* src, uint32_t (&v)[16]) 
     v[j + 2] = x.z;
     v[j + 3] = x.w;
   }
-}
-__device__ __forceinline__ void row_store32(float* dst, const uint32_t (&v)[32]) {
-#pragma unroll
-  for (int j = 0; j < 32; j += 4)
-    *reinterpret_cast<uint4*>(dst + j) = make_uint4(v[j], v[j + 1], v[j + 2], v[j + 3]);
 }
 // TMA load delivered to every CTA of `mask` at the same CTA-relative offsets (data and barrier)
 __device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar,
@@ -440,10 +420,8 @@ __device__ __forceinline__ float tanh_fast(float x) {
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void red_add_v4_f32(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c),
-               "f"(d)
-               : "memory");
+__device__ __forceinline__ void red_add_v2_f32(float* addr, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
 // Counter-based RNG for dropout: splitmix64 of (seed, element-group index) -> 4 x 16-bit lanes.
