@@ -264,6 +264,12 @@ void softmax_ce(uintptr_t logits, uintptr_t labels, uintptr_t loss, uintptr_t dl
                                P<float>(dlogits), M, C, grad_scale, P<float>(loss_acc), S(stream)),
         "softmax_ce");
 }
+void classify_eval(uintptr_t logits, int ldl, uintptr_t labels, int M, int C,
+                   long long ignore_index, uintptr_t acc, uintptr_t stream) {
+  check(sky::launch_classify_eval(P<const float>(logits), ldl, P<const int64_t>(labels), M, C,
+                                  ignore_index, P<sky::EvalAccum>(acc), S(stream)),
+        "classify_eval");
+}
 
 // descriptors: list of (p, g, mom, p_bf16, numel) -> packed host bytes to upload once
 py::bytes pack_sgd_descriptors(
@@ -474,6 +480,10 @@ PYBIND11_MODULE(_cuda, m) {
   m.def("softmax_ce", &softmax_ce, py::arg("logits"), py::arg("labels"), py::arg("loss"),
         py::arg("dlogits"), py::arg("M"), py::arg("C"), py::arg("grad_scale") = 1.f,
         py::arg("loss_acc") = 0, py::arg("stream") = 0);
+  m.def("classify_eval", &classify_eval, py::arg("logits"), py::arg("ldl"), py::arg("labels"),
+        py::arg("M"), py::arg("C"), py::arg("ignore_index"), py::arg("acc"),
+        py::arg("stream") = 0);
+  m.def("eval_max_classes", []() { return sky::kEvalMaxClasses; });
   m.def("pack_sgd_descriptors", &pack_sgd_descriptors);
   m.def("sgd_multi", &sgd_multi, py::arg("d_tensors"), py::arg("n"), py::arg("max_numel"),
         py::arg("lr"), py::arg("momentum") = 0.f, py::arg("weight_decay") = 0.f,

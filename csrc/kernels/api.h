@@ -219,6 +219,20 @@ int launch_small_linear_bwd(const void* x, bool x_bf16, int ldx, const float* w,
 // loss = mean_m CE(logits[m,:], labels[m]);  dlogits = (softmax - onehot) / M * grad_scale
 int launch_softmax_ce(const float* logits, const int64_t* labels, float* loss, float* dlogits,
                       int M, int C, float grad_scale, float* loss_acc, cudaStream_t stream);
+// Evaluation accumulator: the header is followed by C x C confusion counters [label * C + pred].
+struct EvalAccum {
+  double loss_sum;                  // sum of the per-row cross entropies (fp32 rows, fp64 sum)
+  unsigned long long count;         // rows with a label in [0, C)
+  unsigned long long invalid;       // rows whose label is neither ignore_index nor in [0, C)
+  unsigned long long confusion[];   // C * C
+};
+constexpr int kEvalMaxClasses = 1024;
+// Adds one batch of fp32 logits [M, C] (row stride ldl) into *acc: per row lse - logit[label] and
+// pred = argmax (first maximum, NaN counts as the maximum).  Rows with label == ignore_index are
+// skipped.  One CTA, fixed reduction order: deterministic, no host sync, graph-capturable.
+// C > kEvalMaxClasses returns 940.
+int launch_classify_eval(const float* logits, int ldl, const int64_t* labels, int M, int C,
+                         long long ignore_index, EvalAccum* acc, cudaStream_t stream);
 
 // ---------------------------------------------------------------------------------------------
 // Optimizer / parameter maintenance

@@ -720,6 +720,87 @@ softmax_ce_kernel(const float* __restrict__ logits, const int64_t* __restrict__ 
   }
 }
 
+// Evaluation: per-row cross entropy + argmax of one batch of logits, added into an EvalAccum.
+// One CTA of 16 warps; warp w owns rows w, w + 16, ... of each 512-row chunk, its lanes stride
+// over the classes.  The row max / argmax and the exp-sum are reduced with one fixed xor pattern,
+// the chunk's row losses are summed in a fixed fp64 tree and the chunk sums are added in chunk
+// order by thread 0, so the result does not depend on scheduling (graph replays are bit-equal).
+constexpr int kEvalWarps = 16;
+constexpr int kEvalChunk = 512;
+
+// (a, ia) is a better argmax candidate than (b, ib): NaN beats everything, then larger, then the
+// smaller index (torch.argmax: the first maximum wins, a NaN counts as the maximum)
+__device__ __forceinline__ bool eval_better(float a, int ia, float b, int ib) {
+  const bool na = a != a, nb = b != b;
+  if (na || nb) return na && (!nb || ia < ib);
+  return a > b || (a == b && ia < ib);
+}
+
+__global__ void __launch_bounds__(kEvalWarps * 32)
+classify_eval_kernel(const float* __restrict__ logits, long long ldl,
+                     const int64_t* __restrict__ labels, int M, int C, long long ignore_index,
+                     EvalAccum* __restrict__ acc) {
+  __shared__ double row_loss[kEvalChunk];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned long long counted = 0, invalid = 0;
+  double total = 0.0;
+  for (int base = 0; base < M; base += kEvalChunk) {
+    for (int r = warp; r < kEvalChunk; r += kEvalWarps) {
+      const int m = base + r;
+      double contrib = 0.0;
+      if (m < M) {
+        const float* l = logits + static_cast<long long>(m) * ldl;
+        float mx = -INFINITY;
+        int arg = C;  // no candidate yet (C > 0: every row has one after the reduction)
+        for (int c = lane; c < C; c += 32) {
+          const float v = l[c];
+          if (arg == C || eval_better(v, c, mx, arg)) {
+            mx = v;
+            arg = c;
+          }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          const float omx = __shfl_xor_sync(0xffffffffu, mx, o);
+          const int oarg = __shfl_xor_sync(0xffffffffu, arg, o);
+          if (oarg < C && (arg == C || eval_better(omx, oarg, mx, arg))) {
+            mx = omx;
+            arg = oarg;
+          }
+        }
+        // lse = mx + log(sum exp(l - mx)), as in softmax_ce_kernel
+        float se = 0.f;
+        for (int c = lane; c < C; c += 32) se += expf(l[c] - mx);
+        se = warp_sum(se);
+        const long long lab = labels[m];
+        if (lab != ignore_index) {
+          if (lab < 0 || lab >= C) {
+            ++invalid;
+          } else {
+            const float loss = (mx + logf(se)) - l[lab];
+            contrib = static_cast<double>(loss);
+            ++counted;
+            if (lane == 0) atomicAdd(&acc->confusion[lab * C + arg], 1ull);
+          }
+        }
+      }
+      if (lane == 0) row_loss[r] = contrib;
+    }
+    __syncthreads();
+    for (int s = kEvalChunk / 2; s > 0; s >>= 1) {
+      for (int i = threadIdx.x; i < s; i += blockDim.x) row_loss[i] += row_loss[i + s];
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) total += row_loss[0];
+    __syncthreads();
+  }
+  if (lane == 0) {
+    if (counted) atomicAdd(&acc->count, counted);
+    if (invalid) atomicAdd(&acc->invalid, invalid);
+  }
+  if (threadIdx.x == 0) acc->loss_sum += total;
+}
+
 // ------------------------------------------------------------------------------------------
 // Optimizer
 // ------------------------------------------------------------------------------------------
@@ -1232,6 +1313,16 @@ int launch_softmax_ce(const float* logits, const int64_t* labels, float* loss, f
                       int M, int C, float grad_scale, float* loss_acc, cudaStream_t stream) {
   softmax_ce_kernel<<<1, 256, 0, stream>>>(logits, labels, loss, dlogits, M, C, grad_scale,
                                            loss_acc);
+  SKY_LAUNCH_CHECK();
+}
+
+int launch_classify_eval(const float* logits, int ldl, const int64_t* labels, int M, int C,
+                         long long ignore_index, EvalAccum* acc, cudaStream_t stream) {
+  if (C < 1 || C > kEvalMaxClasses) return 940;
+  if (acc == nullptr || ldl < C) return 941;
+  if (M <= 0) return 0;
+  classify_eval_kernel<<<1, kEvalWarps * 32, 0, stream>>>(logits, ldl, labels, M, C, ignore_index,
+                                                          acc);
   SKY_LAUNCH_CHECK();
 }
 

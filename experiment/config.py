@@ -33,6 +33,11 @@ LR_SCHEDULE = os.getenv("LR_SCHEDULE")
 WARMUP_STEPS = int(os.getenv("WARMUP_STEPS", "0"))
 TOTAL_STEPS = int(os.getenv("TOTAL_STEPS", str(MAX_ITERS)))
 MAX_GRAD_NORM = float(os.getenv("MAX_GRAD_NORM")) if os.getenv("MAX_GRAD_NORM") else None
+# EVAL_EVERY=N: train on the learnable synthetic task (label_rule="token") and evaluate on a
+# held-out split of it (EVAL_SAMPLES samples of another seed) every N iterations and after the
+# run; unset = random labels, no evaluation
+EVAL_EVERY = int(os.getenv("EVAL_EVERY")) if os.getenv("EVAL_EVERY") else None
+EVAL_SAMPLES = int(os.getenv("EVAL_SAMPLES", "256"))
 TINY = os.getenv("TINY", "0") == "1"                          # shrink the geometry for CPU smoke runs
 
 _config = BertConfig.bert_large()                              # wwm_uncased_L-24_H-1024_A-16 geometry
@@ -88,6 +93,13 @@ data_config = dict(
                      max_seq_length=_SEQ, vocab_size=_config.vocab_size, num_classes=3, seed=0),
     dataloader_cfg=dict(batch_size=BATCH_SIZE, shuffle=True, num_workers=0, drop_last=True),
 )
+if EVAL_EVERY is not None:
+    # a learnable task (label = first token after [CLS] mod 3) for training and the held-out split,
+    # so that the dev accuracy measures something; random labels stay at chance
+    data_config["dataset_cfg"]["label_rule"] = "token"
+    data_config["eval_datasets"] = dict(
+        dev=dict(type="SynthMNLIDataset", num_samples=EVAL_SAMPLES, max_seq_length=_SEQ,
+                 vocab_size=_config.vocab_size, num_classes=3, seed=1, label_rule="token"))
 
 allocator_config = dict(
     type=ALLOCATE_TYPE,
@@ -132,3 +144,5 @@ train_config = dict(
        if os.getenv("REALLOCATE_EVERY") else []),
     timer_config=dict(root=_LOG_ROOT),
 )
+if EVAL_EVERY is not None:
+    train_config["eval_cfg"] = dict(interval=EVAL_EVERY, at_end=True)

@@ -16,6 +16,7 @@ backward time log lines, ``detect_mem`` - re-designed for one-process-per-GPU ex
 """
 from __future__ import annotations
 
+import contextlib
 import subprocess
 import time
 from typing import List, Optional
@@ -149,6 +150,7 @@ class ModuleWrapper(nn.Module):
         self._logger = Logger(**logging_config) if logging_config else None
         self._timer = DistributedTimer(**(timer_config or {}))
         self._record_forward_time = record_forward_time
+        self._probes_suspended = False  # suspend_forward_probes(): forwards are not timed / logged
         self._fuse_spans = fuse_spans
         self._fwd_events: list = []     # (start_event, end_event) pairs, resolved lazily
         self._bwd_events: list = []
@@ -357,6 +359,17 @@ class ModuleWrapper(nn.Module):
         """Resolve pending device timings into the log file (one sync)."""
         self._resolve_events()
 
+    @contextlib.contextmanager
+    def suspend_forward_probes(self):
+        """Forward calls inside the block (evaluation passes) are neither timed nor logged and
+        leave ``forward_time`` as it was; a simulated slowdown still applies."""
+        saved = self._probes_suspended
+        self._probes_suspended = True
+        try:
+            yield
+        finally:
+            self._probes_suspended = saved
+
     def reset_timers(self) -> None:
         self._resolve_events()
         self._forward_time_resolved, self._backward_time_resolved = [], []
@@ -388,12 +401,14 @@ class ModuleWrapper(nn.Module):
     def forward(self, *args):
         args = [self._move_in(a) for a in args]
         need_probe = self._record_forward_time or self._slowdown > 0 or self._logger is not None
+        timed = not self._probes_suspended
         cuda = self._on_cuda()
         if need_probe:
             args = [self._probe(a, True) for a in args]
             if cuda:
-                s_evt = torch.cuda.Event(enable_timing=True)
-                s_evt.record()
+                if timed:
+                    s_evt = torch.cuda.Event(enable_timing=True)
+                    s_evt.record()
                 if self._slowdown > 0:
                     self._device_throttle_begin()
             else:
@@ -403,19 +418,21 @@ class ModuleWrapper(nn.Module):
             if cuda:
                 if self._slowdown > 0:
                     self._device_throttle_end()
-                e_evt = torch.cuda.Event(enable_timing=True)
-                e_evt.record()
-                self._fwd_events.append((s_evt, e_evt))
-                if len(self._fwd_events) > 4096:
-                    self._resolve_events()
+                if timed:
+                    e_evt = torch.cuda.Event(enable_timing=True)
+                    e_evt.record()
+                    self._fwd_events.append((s_evt, e_evt))
+                    if len(self._fwd_events) > 4096:
+                        self._resolve_events()
             else:
                 comp = time.time() - t0
                 if self._slowdown > 0:
                     time.sleep(comp * self._slowdown)
                 total = time.time() - t0
-                if self._logger:
-                    self._logger.info("forward time on rank {}: {}".format(self._rank, total))
-                self._forward_time_resolved.append(total)
+                if timed:
+                    if self._logger:
+                        self._logger.info("forward time on rank {}: {}".format(self._rank, total))
+                    self._forward_time_resolved.append(total)
         single = not isinstance(out, (tuple, list))
         outs = (out,) if single else tuple(out)
         if need_probe:

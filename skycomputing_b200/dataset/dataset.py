@@ -18,6 +18,9 @@ from ..registry import DATASET
 class SynthMNLIDataset(Dataset):
     """Random token ids with MNLI-like structure: ``[CLS] a [SEP] b [SEP] pad...``.
 
+    ``label_rule="random"`` (default) draws labels independently of the tokens; ``"token"`` sets
+    ``label = input_ids[:, 1] % num_classes``, a task a model can learn and be evaluated on.
+
     Items are ``((input_ids, token_type_ids, attention_mask), label)`` - the order
     ``BertEmbeddings.forward`` consumes.  ``reference_order=True`` yields the reference
     ``GlueDataset`` order ``(input_ids, input_mask, segment_ids)`` instead
@@ -26,7 +29,7 @@ class SynthMNLIDataset(Dataset):
 
     def __init__(self, num_samples: int = 1024, max_seq_length: int = 128, vocab_size: int = 30522,
                  num_classes: int = 3, seed: int = 0, full_length: bool = True,
-                 reference_order: bool = False):
+                 reference_order: bool = False, label_rule: str = "random"):
         g = torch.Generator().manual_seed(seed)
         S = max_seq_length
         low = 1000 if vocab_size > 2000 else max(1, vocab_size // 10)
@@ -42,6 +45,12 @@ class SynthMNLIDataset(Dataset):
         self.input_ids = self.input_ids * self.input_mask
         self.input_ids[:, 0] = min(101, vocab_size - 1)  # [CLS]
         self.labels = torch.randint(0, num_classes, (num_samples,), generator=g)
+        if label_rule == "token":
+            # a learnable task: the label is a function of the first token after [CLS]; another
+            # seed draws another sample of the same task (a held-out split)
+            self.labels = self.input_ids[:, 1] % num_classes
+        elif label_rule != "random":
+            raise ValueError("label_rule must be 'random' or 'token', got {!r}".format(label_rule))
         self.reference_order = reference_order
 
     def __len__(self):

@@ -5,7 +5,7 @@ from __future__ import annotations
 
 import csv
 import os
-from typing import List, Optional
+from typing import Dict, List, Optional
 
 
 class InputExample:
@@ -39,6 +39,7 @@ class _ColumnProcessor(DataProcessor):
     labels: List[str] = []
     col_a, col_b, col_label, skip_header = 0, None, -1, True
     dev_file = "dev.tsv"
+    extra_splits: Dict[str, str] = {}
 
     def _create(self, lines, set_type):
         out = []
@@ -56,6 +57,18 @@ class _ColumnProcessor(DataProcessor):
     def get_dev_examples(self, data_dir):
         return self._create(self._read_tsv(os.path.join(data_dir, self.dev_file)), "dev")
 
+    def get_split_examples(self, data_dir, split: str):
+        """``train``, ``dev`` or one of ``extra_splits`` (file name by split name)."""
+        if split == "train":
+            return self.get_train_examples(data_dir)
+        if split == "dev":
+            return self.get_dev_examples(data_dir)
+        if split in self.extra_splits:
+            return self._create(self._read_tsv(os.path.join(data_dir, self.extra_splits[split])),
+                                split)
+        raise ValueError("unknown split {!r} (known: {})".format(
+            split, ["train", "dev"] + sorted(self.extra_splits)))
+
     def get_labels(self):
         return list(self.labels)
 
@@ -69,6 +82,7 @@ class MnliProcessor(_ColumnProcessor):
     labels = ["contradiction", "entailment", "neutral"]
     col_a, col_b, col_label = 8, 9, -1
     dev_file = "dev_matched.tsv"
+    extra_splits = {"dev_mismatched": "dev_mismatched.tsv"}
 
 
 class ColaProcessor(_ColumnProcessor):

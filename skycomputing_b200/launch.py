@@ -62,6 +62,19 @@ def _seeded_loader(data_config: dict, seed: int):
     return build_dataloader_from_cfg(dataset_cfg=dataset_cfg, dataloader_cfg=dataloader_cfg)
 
 
+def _eval_loaders(data_config: dict) -> dict:
+    """``data_config["eval_datasets"] = {name: dataset_cfg}`` -> {name: DataLoader}, in order.
+    ``eval_dataloader_cfg`` (optional) defaults to the training loader's batch size; shuffle is
+    always off and the short final batch is kept (Runner.evaluate pads it)."""
+    sets = data_config.get("eval_datasets") or {}
+    base = dict(batch_size=data_config["dataloader_cfg"].get("batch_size", 1), num_workers=0)
+    base.update(data_config.get("eval_dataloader_cfg") or {})
+    base.update(shuffle=False, drop_last=False)
+    base.pop("generator", None)
+    return {name: build_dataloader_from_cfg(dataset_cfg=dict(cfg), dataloader_cfg=dict(base))
+            for name, cfg in sets.items()}
+
+
 def run_process(rank: int, world_size: int, rpc_config: dict, model_config: list = None,
                 data_config: dict = None, logging_config: dict = None,
                 allocator_config: dict = None, train_config: dict = None,
@@ -212,6 +225,11 @@ def run_process(rank: int, world_size: int, rpc_config: dict, model_config: list
                 cfg.setdefault("grad_clip", step_cfg["grad_clip"])
                 cfg.setdefault("allocate_type", alloc_type)
             runner.register_hook(build_hook(cfg.pop("type"), **cfg))
+        eval_loaders = _eval_loaders(data_config)
+        if eval_loaders:
+            # periodic evaluation on held-out data (train_config["eval_cfg"]: EvalHook arguments)
+            runner.register_hook(build_hook("EvalHook", datasets=eval_loaders,
+                                            **dict(train_config.get("eval_cfg") or {})))
         info("register hooks")
         runner.train(data_loader)
         runner.engine.close()

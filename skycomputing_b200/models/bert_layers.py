@@ -352,8 +352,12 @@ class BertSpan:
         inputs = tuple(t.to(torch.bfloat16) if (torch.is_tensor(t) and t.is_floating_point()
                                                 and t.dim() == 3 and t.dtype != torch.bfloat16)
                        else t for t in inputs)
-        out = BertSpanFn.apply(sp, training, self.in_channel, self.out_channel, self.microbatch,
-                               len(inputs), *inputs, *sp.all_params())
+        if not training and not torch.is_grad_enabled():
+            # inference: nothing is kept for a backward pass that cannot happen
+            out = BertSpanFn.infer(sp, self.in_channel, self.out_channel, self.microbatch, inputs)
+        else:
+            out = BertSpanFn.apply(sp, training, self.in_channel, self.out_channel,
+                                   self.microbatch, len(inputs), *inputs, *sp.all_params())
         mask = inputs[-1]
         if self.tail is not None:
             return out, mask

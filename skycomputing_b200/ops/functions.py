@@ -192,7 +192,24 @@ class BertSpanFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, sp: SpanParams, training: bool, in_ch, out_ch, mb: int, n_in: int, *tensors):
-        inputs = tensors[:n_in]
+        out, saved, shape3 = BertSpanFn._run(sp, training, in_ch, out_ch, mb, tensors[:n_in], True)
+        ctx.sp, ctx.saved, ctx.training = sp, saved, training
+        ctx.in_ch, ctx.out_ch, ctx.mb, ctx.n_in = in_ch, out_ch, mb, n_in
+        ctx.n_tensors = len(tensors)
+        ctx.shape3 = shape3
+        return out
+
+    @staticmethod
+    def infer(sp: SpanParams, in_ch, out_ch, mb: int, inputs):
+        """Inference forward (eval mode, no autograd): the same kernels and outputs as
+        ``forward(training=False)``, without what only backward reads - no FFN1 pre-activation
+        copy, no pre-LayerNorm sums, no attention LSE - and without an autograd node."""
+        return BertSpanFn._run(sp, False, in_ch, out_ch, mb, inputs, False)[0]
+
+    @staticmethod
+    def _run(sp: SpanParams, training: bool, in_ch, out_ch, mb, inputs, keep: bool):
+        """Returns (outputs, tensors saved for backward, (B, S, H)); ``keep`` = False skips every
+        buffer that only backward needs."""
         # slot index on the inbound link / on the outbound link: the same number in a plain
         # pipeline (micro-batch j), different ones on the wrap-around link of a looped pipeline
         mb_in, mb_out = mb if isinstance(mb, tuple) else (mb, mb)
@@ -210,14 +227,15 @@ class BertSpanFn(torch.autograd.Function):
             wait = _ch_kwargs_wait(in_ch, mb_in) if in_ch is not None else {}
             qkv = nat.gemm(x, sp.wqkv.shadow(), bias=sp.bqkv.master(), **wait)
             ctxt, lse = nat.attention_fwd(qkv, mask2, B, S, sp.heads, dropout_p=p_attn, rng=rng,
-                                          rng_stream=sp.rng_base + 1)
+                                          rng_stream=sp.rng_base + 1, save_lse=keep)
             ln_out = {}
             if out_ch is not None and not sp.has_body:
                 ln_out = dict(y_ptr=out_ch.peer_act_ptr(mb_out), signal_flags=out_ch.peer_act_flags_ptr(mb_out))
             y1, z1, mean1, rstd1 = _gemm_ln(ctxt, sp.wo, sp.bo, x, sp.g1, sp.b1n, sp.eps, p_hid, rng,
-                                            sp.rng_base + 2, ln_out)
-            saved.update(x=x, mask2=mask2, qkv=qkv, ctxt=ctxt, lse=lse, z1=z1, mean1=mean1,
-                         rstd1=rstd1)
+                                            sp.rng_base + 2, ln_out, save_z=keep)
+            if keep:
+                saved.update(x=x, mask2=mask2, qkv=qkv, ctxt=ctxt, lse=lse, z1=z1, mean1=mean1,
+                             rstd1=rstd1)
             a = y1
             shape3 = (B, S, H)
         else:
@@ -234,9 +252,10 @@ class BertSpanFn(torch.autograd.Function):
         if sp.has_body:
             wait = _ch_kwargs_wait(in_ch, mb_in) if (in_ch is not None and not sp.has_head) else {}
             I = sp.w1.master().shape[0]
-            h1 = torch.empty((a.shape[0], I), dtype=torch.bfloat16, device=a.device)
+            h1 = torch.empty((a.shape[0], I), dtype=torch.bfloat16, device=a.device) if keep else None
             inter = nat.gemm(a, sp.w1.shadow(), bias=sp.b1.master(), act=nat.ACT_GELU, out2=h1, **wait)
-            saved.update(h1=h1)
+            if keep:
+                saved.update(h1=h1)
         elif sp.has_tail:
             inter = _flat2d(inputs[0])
         if sp.has_tail:
@@ -245,25 +264,21 @@ class BertSpanFn(torch.autograd.Function):
             if out_ch is not None:
                 ln_out = dict(y_ptr=out_ch.peer_act_ptr(mb_out), signal_flags=out_ch.peer_act_flags_ptr(mb_out))
             y2, z2, mean2, rstd2 = _gemm_ln(inter, sp.w2, sp.b2, a, sp.g2, sp.b2n, sp.eps, p_hid, rng,
-                                            sp.rng_base + 3, ln_out, **wait)
-            saved.update(z2=z2, mean2=mean2, rstd2=rstd2)
-        if sp.has_body or sp.has_tail:
+                                            sp.rng_base + 3, ln_out, save_z=keep, **wait)
+            if keep:
+                saved.update(z2=z2, mean2=mean2, rstd2=rstd2)
+        if keep and (sp.has_body or sp.has_tail):
             saved.update(a=a, inter=inter)
-        ctx.sp, ctx.saved, ctx.training = sp, saved, training
-        ctx.in_ch, ctx.out_ch, ctx.mb, ctx.n_in = in_ch, out_ch, mb, n_in
-        ctx.n_tensors = len(tensors)
-        ctx.shape3 = shape3
         B, S, H = shape3
         if sp.has_tail:
             out = y2.view(B, S, H) if y2 is not None else _dummy_out(a)
-            return out
-        if sp.has_body:
+        elif sp.has_body:
             # the pass-through attention output is only returned when this span produced it;
             # a span that starts at Body lets the caller forward its own input tensor
-            if sp.has_head:
-                return inter.view(B, S, -1), a.view(B, S, H)
-            return inter.view(B, S, -1)
-        return y1.view(B, S, H) if y1 is not None else _dummy_out(x)
+            out = (inter.view(B, S, -1), a.view(B, S, H)) if sp.has_head else inter.view(B, S, -1)
+        else:
+            out = y1.view(B, S, H) if y1 is not None else _dummy_out(x)
+        return out, saved, shape3
 
     @staticmethod
     def backward(ctx, *grads):
@@ -446,19 +461,20 @@ def _dummy_out(like: torch.Tensor) -> torch.Tensor:
 
 
 def _gemm_ln(a, wbank, bbank, residual, gbank, betabank, eps, p_drop, rng, rng_stream,
-             ln_out: dict, **wait):
+             ln_out: dict, save_z: bool = True, **wait):
     """Dense + bias + dropout + residual + LayerNorm (the reference's BertSelfOutput / BertOutput,
     scaelum/model/bert_layers.py:285-289,323-327).  ONE wgmma kernel with the LayerNorm in the
     GEMM epilogue whenever the row fits a thread-block cluster; with ``ln_out`` (peer pointer + panel
     flags of a fused stage boundary) that kernel stores y straight into the next stage's HBM.  Otherwise GEMM, then the standalone LayerNorm.
-    Returns (y | None, z, mean, rstd)."""
+    Returns (y | None, z, mean, rstd); ``z`` is None when ``save_z`` is False and the fused kernel
+    runs (the unfused path needs z as the LayerNorm input anyway)."""
     M, N = a.shape[0], wbank.master().shape[0]
     # both ends of a fused boundary evaluate the same predicate on the same (rows, cols): the
     # consumer's expected signal count per panel follows from it (parallel/p2p.py)
     if nat.gemm_ln_supported(M, N):
         return nat.gemm_ln(a, wbank.shadow(), gbank.master(), betabank.master(), eps=eps,
                            bias=bbank.master(), residual=residual, dropout_p=p_drop, rng=rng,
-                           rng_stream=rng_stream, y_ld=N, **ln_out, **wait)
+                           rng_stream=rng_stream, save_z=save_z, y_ld=N, **ln_out, **wait)
     z = nat.gemm(a, wbank.shadow(), bias=bbank.master(), aux=residual, add_aux=True,
                  dropout_p=p_drop, rng=rng, rng_stream=rng_stream, **wait)
     y, mean, rstd = _ln_fwd(z, gbank.master(), betabank.master(), eps, **ln_out)

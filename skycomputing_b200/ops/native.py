@@ -36,7 +36,8 @@ def available() -> bool:
 _KERNELS_PER_CALL = {
     "gemm": 1, "layernorm_fwd": 1, "layernorm_bwd": 1, "ln_param_grad": 1, "colsum": 1, "dgelu_mul": 1,
     "attention_fwd": 1, "attention_bwd": 1, "embed_fwd": 1, "embed_bwd": 1,
-    "small_linear_fwd": 1, "small_linear_bwd": 2, "softmax_ce": 1, "sgd_multi": 1, "adam_multi": 1,
+    "small_linear_fwd": 1, "small_linear_bwd": 2, "softmax_ce": 1, "classify_eval": 1,
+    "sgd_multi": 1, "adam_multi": 1,
     "grad_sumsq_multi": 1, "optim_finalize": 1,
     "cast_f32_to_bf16": 1, "cast_bf16_to_f32": 1, "advance_counter": 1, "advance_epoch": 1,
     "signal_flags": 1, "wait_flags": 1, "spin_ns": 1, "record_time": 1, "spin_factor": 1,
@@ -333,14 +334,15 @@ def colsum_(x: torch.Tensor, out: torch.Tensor) -> None:
 
 
 def attention_fwd(qkv, mask, B: int, S: int, heads: int, *, dropout_p: float = 0.0,
-                  rng: Optional[RngState] = None, rng_stream: int = 0):
+                  rng: Optional[RngState] = None, rng_stream: int = 0, save_lse: bool = True):
+    """Returns ``(ctx, lse)``; ``lse`` (kept for backward) is None when ``save_lse`` is False."""
     _check(qkv, torch.bfloat16, "qkv")
     H = qkv.shape[1] // 3
     d = H // heads
     ctx = torch.empty((B * S, H), dtype=torch.bfloat16, device=qkv.device)
-    lse = torch.empty((B * heads * S,), dtype=torch.float32, device=qkv.device)
+    lse = torch.empty((B * heads * S,), dtype=torch.float32, device=qkv.device) if save_lse else None
     ext().attention_fwd(qkv=qkv.data_ptr(), mask=_ptr(mask), ctx=ctx.data_ptr(),
-                        lse=lse.data_ptr(), B=B, S=S, heads=heads, head_dim=d,
+                        lse=_ptr(lse), B=B, S=S, heads=heads, head_dim=d,
                         scale=1.0 / (d ** 0.5), dropout_p=float(dropout_p),
                         rng_state=0 if rng is None else rng.ptr, rng_stream=rng_stream,
                         stream=_stream())
@@ -379,3 +381,54 @@ def softmax_ce(logits: torch.Tensor, labels: torch.Tensor, grad_scale: float = 1
                      dlogits=dlogits.data_ptr(), M=M, C=C, grad_scale=grad_scale,
                      loss_acc=_ptr(loss_acc), stream=_stream())
     return loss, dlogits
+
+
+def classify_eval(logits: torch.Tensor, labels: torch.Tensor, accum: torch.Tensor,
+                  ignore_index: int = -100) -> None:
+    """Adds one batch of fp32 logits [M, C] into the device accumulator ``accum`` (the int64
+    buffer of an ``EvalAccumulator``): per-row cross entropy, argmax and confusion counts.  One
+    launch, no host synchronisation, deterministic."""
+    _check(logits, torch.float32, "logits")
+    if logits.dim() != 2:
+        raise ValueError("logits must be 2-D [M, C]")
+    M, C = logits.shape
+    if not labels.is_cuda or labels.dtype != torch.int64 or labels.numel() != M:
+        raise ValueError("labels must be a CUDA int64 tensor with one entry per logits row")
+    if accum.dtype != torch.int64 or accum.numel() < 3 + C * C:
+        raise ValueError("accum is not an EvalAccumulator buffer for {} classes".format(C))
+    ext().classify_eval(logits=logits.data_ptr(), ldl=logits.stride(0),
+                        labels=labels.contiguous().data_ptr(), M=M, C=C,
+                        ignore_index=int(ignore_index), acc=accum.data_ptr(), stream=_stream())
+
+
+class EvalAccumulator:
+    """Device-side classification accumulator of one evaluation pass: ``{loss_sum (fp64), count,
+    invalid, confusion[C, C]}`` in one int64 buffer (the layout of ``sky::EvalAccum``).
+
+    ``reset()`` is one memset and ``add()`` one ``classify_eval`` launch, both capturable into a
+    CUDA graph; ``read()`` is the single device-to-host copy of the pass."""
+
+    def __init__(self, C: int, device=None):
+        if C < 1 or C > ext().eval_max_classes():
+            raise ValueError("EvalAccumulator supports 1 <= C <= {} classes, got {}".format(
+                ext().eval_max_classes(), C))
+        self.C = int(C)
+        self.buffer = torch.zeros(3 + self.C * self.C, dtype=torch.int64,
+                                  device=device if device is not None else "cuda")
+
+    def reset(self) -> None:
+        self.buffer.zero_()
+
+    def add(self, logits: torch.Tensor, labels: torch.Tensor, ignore_index: int = -100) -> None:
+        logits = logits.detach().reshape(-1, logits.shape[-1])
+        if logits.dtype != torch.float32:
+            logits = logits.float()
+        if logits.shape[1] != self.C:
+            raise ValueError("logits have {} classes, the accumulator {}".format(
+                logits.shape[1], self.C))
+        classify_eval(logits, labels.reshape(-1), self.buffer, ignore_index)
+
+    def read(self) -> dict:
+        host = self.buffer.cpu()
+        return dict(loss_sum=float(host[0:1].view(torch.float64)[0]), count=int(host[1]),
+                    invalid=int(host[2]), confusion=host[3:].view(self.C, self.C).clone())

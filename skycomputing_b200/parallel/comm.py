@@ -142,6 +142,13 @@ class TorchDistComm:
         reqs = dist.batch_isend_irecv(ops) if ops else []
         return outs, reqs
 
+    def forget(self, direction: str) -> None:
+        """Drop the cached metadata of ``direction`` (both ends of a link call this at the same
+        point, e.g. at the start of every forward-only pass, whose batch shape may change)."""
+        for cache in (self._meta_sent, self._meta_recv):
+            for key in [k for k in cache if k[1] == direction]:
+                del cache[key]
+
     def cached_meta(self, src: int, direction: str) -> Optional[list]:
         return self._meta_recv.get((src, direction))
 

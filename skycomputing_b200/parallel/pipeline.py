@@ -85,6 +85,8 @@ class PipelineEngine(EngineBase):
         self._eager_steps = 0
         self._advance_rng = advance_rng
         self._pending_sends: list = []
+        self._eval_comm_obj = None      # forward-only transport when training needs none
+        self._eval: Optional[dict] = None   # the evaluation CUDA graph and its static buffers
         self.stage.engine_managed_backward = True
         self.launches_per_step = 0
         self._init_common()
@@ -402,31 +404,105 @@ class PipelineEngine(EngineBase):
         self._graph.replay()
         return self._loss_acc if self.is_last else None
 
-    # ------------------------------------------------------------------ plain forward (eval)
-    @torch.no_grad()
-    def forward_only(self, inputs: Optional[Sequence[torch.Tensor]] = None):
-        """Sequential forward through the pipeline without gradients (logits on the last stage)."""
-        if self.P == 1:
-            return self.stage(*inputs)
-        from .comm import TorchDistComm
+    # ------------------------------------------------------------------ forward only (eval)
+    def _eval_comm(self):
+        """The p2p transport of forward-only passes: the training one when this rank has it,
+        otherwise one of its own (fused boundaries carry training steps only)."""
+        if self.comm is not None:
+            return self.comm
+        if self._eval_comm_obj is None:
+            from .comm import TorchDistComm
 
-        comm = self.comm or TorchDistComm(self.device, group=self.group)
-        if self.is_first:
-            args = tuple(inputs)
-        else:
-            args, reqs = comm.recv(self.prev_rank, "eval")
-            comm.wait(reqs)
+            self._eval_comm_obj = TorchDistComm(self.device, group=self.group)
+        return self._eval_comm_obj
+
+    @torch.no_grad()
+    def forward_only(self, inputs: Optional[Sequence[torch.Tensor]] = None, micro_batches: int = 1):
+        """Forward through the pipeline without gradients.  The batch is split into
+        ``micro_batches`` chunks; sends are asynchronous and waited for at the end of the pass, so
+        stage s runs chunk j + 1 while stage s + 1 runs chunk j.  Returns on the last stage the
+        stage outputs (``micro_batches == 1``) or the list of per-chunk outputs, None elsewhere."""
+        m = int(micro_batches)
         st = self.stage
         st.in_channel = st.out_channel = None
-        outs = st(*args)
+        chunks = [t.chunk(m, dim=0) for t in inputs] if self.is_first else None
+        if self.P == 1:
+            results = [st(*(c[j] for c in chunks)) for j in range(m)]
+            return results[0] if m == 1 else results
+        comm = self._eval_comm()
+        comm.forget("eval")   # every pass announces its own shapes
+        results, pending, keep = [], [], []
+        for j in range(m):
+            st.microbatch = j
+            if self.is_first:
+                args = tuple(c[j] for c in chunks)
+            else:
+                args, reqs = comm.recv(self.prev_rank, "eval")
+                comm.wait(reqs)
+            outs = st(*args)
+            if self.is_last:
+                results.append(outs)
+            else:
+                keep.append(outs)
+                pending += comm.send(list(outs), self.next_rank, "eval")
+        comm.wait(pending)
         if not self.is_last:
-            comm.wait(comm.send(list(outs), self.next_rank, "eval"))
             return None
-        return outs
+        return results[0] if m == 1 else results
+
+    def eval_step(self, inputs: Optional[Sequence[torch.Tensor]], labels: Optional[torch.Tensor],
+                  accum, micro_batches: Optional[int] = None) -> None:
+        """One evaluation batch: ``forward_only`` and, on the last stage, ``accum.add(logits,
+        labels)`` per micro-batch.  On one GPU with the native kernels and ``use_cuda_graph`` the
+        whole batch (forward + accumulation) is captured into its own CUDA graph after one eager
+        pass and replayed; it touches neither the dropout RNG, the boundary epochs, the training
+        loss nor the optimizer."""
+        m = int(micro_batches or self.m)
+        if self.is_first and inputs[0].shape[0] % m:
+            raise ValueError("an evaluation batch of {} samples cannot be split into {} equal "
+                             "micro-batches".format(inputs[0].shape[0], m))
+        with self.stage.suspend_forward_probes():
+            # the graph reads the bf16 weight copies in place: only an optimizer that refreshes
+            # them on the device (graph_safe) keeps a captured evaluation current
+            if self.P == 1 and self._want_graph and self._native_active() and \
+                    bool(getattr(self.optimizer, "graph_safe", False)):
+                self._eval_graph_step(inputs, labels, accum, m)
+            else:
+                self._eval_body(inputs, labels, accum, m)
+
+    def _eval_body(self, inputs, labels, accum, m: int) -> None:
+        res = self.forward_only(inputs, micro_batches=m)
+        if self.is_last:
+            res = [res] if m == 1 else res
+            for outs, lab in zip(res, labels.chunk(m, dim=0)):
+                accum.add(outs[0], lab)
+
+    def _eval_graph_step(self, inputs, labels, accum, m: int) -> None:
+        key = (tuple((tuple(t.shape), t.dtype) for t in inputs), tuple(labels.shape), m, id(accum))
+        ev = self._eval
+        if ev is None or ev["key"] != key:
+            # one evaluation graph per engine: a new shape / accumulator replaces the old one
+            ev = self._eval = dict(key=key, inputs=[t.clone() for t in inputs],
+                                   labels=labels.clone(), graph=None, eager=0, accum=accum)
+        for s_, t in zip(ev["inputs"], inputs):
+            s_.copy_(t, non_blocking=True)
+        ev["labels"].copy_(labels, non_blocking=True)
+        if ev["graph"] is None and ev["eager"] < 1:
+            self._eval_body(ev["inputs"], ev["labels"], accum, m)   # warm-up: allocations, attrs
+            ev["eager"] += 1
+            return
+        if ev["graph"] is None:
+            torch.cuda.synchronize(self.device)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._eval_body(ev["inputs"], ev["labels"], accum, m)
+            ev["graph"] = g
+        ev["graph"].replay()
 
     def close(self) -> None:
         if self.device.type == "cuda":
             torch.cuda.synchronize(self.device)  # nothing of ours may still touch a peer region
+        self._eval = None   # the evaluation graph is rebuilt by the next engine
         self._close_grad_norm()
         if self.fused is not None:
             self.fused.close()

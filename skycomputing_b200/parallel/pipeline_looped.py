@@ -25,6 +25,7 @@ which is why it is opt-in.
 """
 from __future__ import annotations
 
+import contextlib
 from typing import Callable, List, Optional, Sequence
 
 import torch
@@ -94,8 +95,11 @@ class LoopedPipelineEngine(EngineBase):
     # ------------------------------------------------------------------ helpers
     @property
     def comm(self) -> TorchDistComm:
+        """torch.distributed p2p transport.  Forward-only passes use it even when training runs
+        on the fused ring; one communicator per direction, as on the training path (collective
+        on first use)."""
         if self._comm is None:
-            self._comm = TorchDistComm(self.device, group=self.group)   # eval-only use
+            self._comm = TorchDistComm(self.device, group=self.group, directional=True)
         return self._comm
 
     @staticmethod
@@ -346,21 +350,51 @@ class LoopedPipelineEngine(EngineBase):
 
     # ------------------------------------------------------------------ plain forward (eval)
     @torch.no_grad()
-    def forward_only(self, inputs: Optional[Sequence[torch.Tensor]] = None):
-        outs = None
+    def forward_only(self, inputs: Optional[Sequence[torch.Tensor]] = None, micro_batches: int = 1):
+        """Breadth-first forward of every (chunk, micro-batch) without gradients; sends are
+        asynchronous and waited for at the end of the pass.  Returns on the rank that owns the last
+        virtual stage its outputs (``micro_batches == 1``) or the list of per-chunk outputs."""
+        m = int(micro_batches)
+        comm = self.comm
+        chunks_in = [t.chunk(m, dim=0) for t in inputs] if self.is_first else None
+        results, pending, keep = [], [], []
         for c, st in enumerate(self.stages):
+            comm.forget(f"eval{c}")
             k = self.vidx[c]
-            if k == 0:
-                args = tuple(inputs)
-            else:
-                args, reqs = self.comm.recv(self.prev_rank, f"eval{c}")
-                self.comm.wait(reqs)
             st.in_channel = st.out_channel = None
-            outs = st(*args)
-            if k != self.total - 1:
-                self.comm.wait(self.comm.send(list(outs), self.next_rank, f"eval{c}"))
-                outs = None
-        return outs
+            for j in range(m):
+                st.microbatch = c * m + j
+                if k == 0:
+                    args = tuple(t[j] for t in chunks_in)
+                else:
+                    args, reqs = comm.recv(self.prev_rank, f"eval{c}")
+                    comm.wait(reqs)
+                outs = st(*args)
+                if k == self.total - 1:
+                    results.append(outs)
+                else:
+                    keep.append(outs)
+                    pending += comm.send(list(outs), self.next_rank, f"eval{c}")
+        comm.wait(pending)
+        if not results:
+            return None
+        return results[0] if m == 1 else results
+
+    def eval_step(self, inputs: Optional[Sequence[torch.Tensor]], labels: Optional[torch.Tensor],
+                  accum, micro_batches: Optional[int] = None) -> None:
+        """``forward_only`` + ``accum.add(logits, labels)`` per micro-batch on the last stage."""
+        m = int(micro_batches or self.m)
+        if self.is_first and inputs[0].shape[0] % m:
+            raise ValueError("an evaluation batch of {} samples cannot be split into {} equal "
+                             "micro-batches".format(inputs[0].shape[0], m))
+        with contextlib.ExitStack() as stack:
+            for st in self.stages:
+                stack.enter_context(st.suspend_forward_probes())
+            res = self.forward_only(inputs, micro_batches=m)
+        if self.is_last:
+            res = [res] if m == 1 else res
+            for outs, lab in zip(res, labels.chunk(m, dim=0)):
+                accum.add(outs[0], lab)
 
     def close(self) -> None:
         if self.device.type == "cuda":

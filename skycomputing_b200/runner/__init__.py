@@ -1,7 +1,9 @@
 from .hooks import Hook
-from .hooks_collection import (CheckpointHook, DistributedTimerHelperHook, ReallocateHook,
-                               StopHook)
+from .hooks_collection import (CheckpointHook, DistributedTimerHelperHook, EvalHook,
+                               ReallocateHook, StopHook)
+from .metrics import TorchEvalAccumulator, classification_metrics
 from .runner import Runner, build_loss
 
-__all__ = ["Hook", "CheckpointHook", "DistributedTimerHelperHook", "StopHook", "ReallocateHook",
-           "Runner", "build_loss"]
+__all__ = ["Hook", "CheckpointHook", "DistributedTimerHelperHook", "EvalHook", "StopHook",
+           "ReallocateHook", "Runner", "build_loss", "TorchEvalAccumulator",
+           "classification_metrics"]

@@ -94,6 +94,10 @@ class CheckpointHook(Hook):
             return
         self.save(runner, osp.join(self._save_path, "epoch_{}.pth".format(runner.epoch)))
 
+    def after_val_epoch(self, runner):
+        # an evaluation pass is not a training epoch: no checkpoint
+        return None
+
     def save(self, runner, file_name: str) -> None:
         if runner.is_rank0:
             os.makedirs(osp.dirname(osp.abspath(file_name)), exist_ok=True)

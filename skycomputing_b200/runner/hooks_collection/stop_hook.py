@@ -51,6 +51,10 @@ class StopHook(Hook):
         if flag == "1":
             runner.request_stop()
 
+    def after_val_iter(self, runner):
+        # the flag is checked between training iterations only
+        return None
+
     def after_run(self, runner):
         if self._is_rank0() and osp.exists(self.file_path):
             os.remove(self.file_path)

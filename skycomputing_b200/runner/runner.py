@@ -109,6 +109,9 @@ class Runner:
         self.last_step_seconds: Optional[float] = None
         self._boundary = boundary
         self._use_cuda_graph = use_cuda_graph
+        self._eval_accum = None       # kept across passes: a captured eval graph adds into it
+        self.val_iter = 0             # batch index of the current evaluation pass
+        self.last_eval: Optional[dict] = None
         self.engine = None
         self._build_engine()
 
@@ -289,6 +292,83 @@ class Runner:
             self._epoch += 1
             self._call_hook("after_train_epoch")
         self._call_hook("after_run")
+
+    # ------------------------------------------------------------------ evaluation
+    def evaluate(self, data_loader, name: str = "val", micro_batches: Optional[int] = None,
+                 ignore_index: int = -100) -> dict:
+        """Classification metrics of the model on ``data_loader`` (collective: every rank calls
+        it and every rank gets the same dict, broadcast by the last stage).
+
+        The model runs in eval mode (the previous mode is restored) through the engine's
+        forward-only pass with ``micro_batches`` chunks per batch (default: the training value;
+        it must divide the batch size).  The first batch fixes the evaluation batch size; a
+        shorter last batch is padded to it with zero ids / mask and ``ignore_index`` labels, so
+        every example is counted exactly once.  Fires ``before/after_val_epoch`` once and
+        ``before/after_val_iter`` per batch; ``val_iter`` counts the batches of the pass and
+        ``iter`` does not move.  Neither the training RNG streams nor the optimizer are touched.
+        """
+        import torch.distributed as dist
+
+        from .metrics import LazyEvalAccumulator, classification_metrics, format_metrics
+
+        eng = self.engine
+        m = int(micro_batches or self.micro_batches)
+        if self._eval_accum is None or self._eval_accum.ignore_index != ignore_index:
+            self._eval_accum = LazyEvalAccumulator(ignore_index)
+        acc = self._eval_accum
+        was_training = self.model.training
+        cpu_rng = torch.random.get_rng_state()   # iterating a DataLoader draws a base seed
+        self.model.train(False)
+        self.val_iter = 0
+        try:
+            acc.reset()
+            self._call_hook("before_val_epoch")
+            batch = None
+            for data, labels in data_loader:
+                data = list(data) if isinstance(data, (list, tuple)) else [data]
+                n = int(data[0].shape[0])
+                if batch is None:
+                    batch = n
+                    if batch % m:
+                        raise ValueError("evaluation batches of {} samples cannot be split into {} "
+                                         "equal micro-batches".format(batch, m))
+                if n > batch:
+                    raise ValueError("evaluation batch of {} samples after batches of {}".format(
+                        n, batch))
+                if n < batch:
+                    data = [torch.cat([t, t.new_zeros((batch - n,) + tuple(t.shape[1:]))])
+                            for t in data]
+                    labels = torch.cat([labels, labels.new_full((batch - n,), ignore_index)])
+                self._call_hook("before_val_iter")
+                inputs = [self._to_device(t) for t in data] if eng.is_first else None
+                lab = self._to_device(labels) if eng.is_last else None
+                eng.eval_step(inputs, lab, acc, micro_batches=m)
+                self.val_iter += 1
+                self._call_hook("after_val_iter")
+            totals = acc.read() if eng.is_last else None
+            payload = None
+            if totals is not None:
+                payload = dict(classification_metrics(totals["confusion"], totals["loss_sum"],
+                                                      totals["count"]),
+                               invalid=totals["invalid"])
+            if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+                box = [payload]
+                dist.broadcast_object_list(box, src=self.model.stage_to_rank[-1])
+                payload = box[0]
+        finally:
+            self.model.train(was_training)
+            torch.random.set_rng_state(cpu_rng)
+        invalid = payload.pop("invalid")
+        if invalid:
+            raise ValueError("evaluation {}: {} labels are outside [0, {}) and not ignore_index "
+                             "({})".format(name, invalid, len(payload["confusion"]), ignore_index))
+        self._call_hook("after_val_epoch")
+        self._log("eval {}: {}".format(name, format_metrics(payload)))
+        if self._metrics_path is not None:
+            with open(self._metrics_path, "a") as f:
+                f.write(json.dumps(dict(mode="val", name=name, iter=self._iter, **payload)) + "\n")
+        self.last_eval = dict(payload, name=name)
+        return payload
 
     def _batch_shape_ok(self, data) -> bool:
         """The engine fixes the micro-batch shape on the first step (static CUDA-graph buffers,
