@@ -512,7 +512,8 @@ LoopedScore looped_score(const std::vector<double>& pre_f, const std::vector<dou
 }
 }  // namespace
 
-std::vector<int> refine_looped_partition(const AllocProblem& p, std::vector<int> b) {
+std::vector<int> refine_looped_partition(const AllocProblem& p, std::vector<int> b,
+                                         double max_chunk) {
   const int D = static_cast<int>(p.dev_time.size());
   const int VP = static_cast<int>(b.size()) - 1;
   const int L = static_cast<int>(p.layer_flops.size());
@@ -524,6 +525,8 @@ std::vector<int> refine_looped_partition(const AllocProblem& p, std::vector<int>
     pre_m[i + 1] = pre_m[i] + p.layer_mem[i];
   }
   LoopedScore cur = looped_score(pre_f, pre_m, p, b);
+  // a start that is already over the cap may keep its worst chunk, but no move may raise it
+  const double cap = std::max(max_chunk, cur.worst_chunk);
   for (int iter = 0; iter < 20 * VP; ++iter) {
     int busiest = 0;
     for (int d = 1; d < D; ++d)
@@ -542,7 +545,8 @@ std::vector<int> refine_looped_partition(const AllocProblem& p, std::vector<int>
         else
           continue;
         LoopedScore sc = looped_score(pre_f, pre_m, p, nb);
-        if (sc.feasible && sc.better_than(cur) && (!found || sc.better_than(best))) {
+        if (sc.feasible && sc.worst_chunk <= cap && sc.better_than(cur) &&
+            (!found || sc.better_than(best))) {
           best = sc;
           best_b = nb;
           found = true;

@@ -51,8 +51,11 @@ double partition_bottleneck(const AllocProblem& p, const std::vector<int>& order
 // Looped pipelines (v chunks per device, chunk k belongs to device k % D): hill-climb on the chunk
 // boundaries of a partition into v * D chunks until the descending-sorted vector of per-DEVICE
 // loads dev_time[d] * sum(flops of d's chunks) cannot be lowered any more (ties: the smaller most
-// expensive chunk).  Every chunk keeps >= 1 unit, per-device memory caps are respected.
+// expensive chunk).  Every chunk keeps >= 1 unit, per-device memory caps are respected, and no
+// move makes a chunk cost more than `max_chunk` (dev_time * flops; +inf: no cap) unless the
+// starting partition already did.
 // `p.dev_time / p.dev_mem` are per DEVICE (D entries), `boundaries` has v * D + 1 entries.
-std::vector<int> refine_looped_partition(const AllocProblem& p, std::vector<int> boundaries);
+std::vector<int> refine_looped_partition(const AllocProblem& p, std::vector<int> boundaries,
+                                         double max_chunk);
 
 }  // namespace sky

@@ -3,6 +3,8 @@
 #include <pybind11/pybind11.h>
 #include <pybind11/stl.h>
 
+#include <limits>
+
 #include "alloc/allocator.h"
 #include "alloc/stimulator.h"
 
@@ -72,11 +74,11 @@ PYBIND11_MODULE(_core, m) {
       "refine_looped_partition",
       [](const std::vector<double>& lf, const std::vector<double>& lm,
          const std::vector<double>& dt, const std::vector<double>& dm,
-         const std::vector<int>& boundaries) {
-        return refine_looped_partition(make_problem(lf, lm, dt, dm, {}), boundaries);
+         const std::vector<int>& boundaries, double max_chunk) {
+        return refine_looped_partition(make_problem(lf, lm, dt, dm, {}), boundaries, max_chunk);
       },
       py::arg("layer_flops"), py::arg("layer_mem"), py::arg("dev_time"), py::arg("dev_mem"),
-      py::arg("boundaries"),
+      py::arg("boundaries"), py::arg("max_chunk") = std::numeric_limits<double>::infinity(),
       "looped pipelines: refine a v * D chunk partition towards balanced per-device loads");
   m.def("numpy_default_rng_random", &numpy_default_rng_random, py::arg("seed"), py::arg("n"));
   py::class_<Stimulator>(m, "Stimulator")

@@ -1,18 +1,20 @@
 // Fused self-attention for BERT geometry (S = 128 keys per sequence, head_dim = 64) on wgmma.
 //
-// One CTA (one warpgroup) per (batch, head).  With S = 128 a whole score matrix is one 128x128
-// tile, so no online-softmax tiling is needed:
+// One CTA of two warpgroups per (batch, head).  With S = 128 a whole score matrix is one 128x128
+// tile, so no online-softmax tiling is needed.  Warpgroup w owns query rows 64w .. 64w + 63, and
+// every MMA result stays in the wgmma accumulator registers:
 //
-//   forward : S = Q K^T (wgmma 2 x m64n128, K = 64) -> fp32 staging tile in shared memory ->
-//             per-row softmax (+mask, +dropout) with one thread per query row -> P (bf16) into
-//             swizzled smem -> O = P V (wgmma 2 x m64n64, K = 128) -> ctx
-//   backward: S = Q K^T, dP = dO V^T (64 keys at a time) -> P = exp2(s - lse),
-//             dS = P (dP*keep - delta) -> smem (one copy serves as K-major AND MN-major operand) ->
-//             dV = P^T dO, dK = dS^T Q, dQ = dS K
+//   forward : S = Q K^T (wgmma m64n128, K = 64) -> softmax (+mask, +dropout) on the fragments,
+//             row max / row sum over the thread's columns and then its quad -> bf16 P as the
+//             register A operand of O = P V (wgmma m64n64, K = 128) -> ctx through per-warp
+//             staging buffers (128-byte rows)
+//   backward: per 64-key half, S = Q K^T and dP = dO V^T (m64n64) -> P = exp2(s - lse),
+//             dS = P (dP*keep - delta) on the fragments -> bf16 P / dS into swizzled smem (one copy
+//             serves as K-major AND MN-major operand) -> dV = P^T dO, dK = dS^T Q (each warpgroup
+//             64 keys), dQ = dS K (each warpgroup its 64 query rows) -> dqkv through the staging
+//             buffers
 //
-// The accumulator fragments of a warpgroup are spread over its threads; the softmax needs whole
-// rows, so every MMA result goes through an fp32 staging tile ([128][N + 4] floats).
-//
+// Fragment layout, staging buffer and the register-A wgmma are described in sm100_ptx.cuh.
 // Q/K/V/dO tiles come straight out of the fused [tokens, 3H] QKV activation via 2D TMA boxes
 // (no head split/merge copies), outputs are written head-merged.
 //
@@ -23,6 +25,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <climits>
 #include <cstdlib>
 
 #include "api.h"
@@ -39,8 +42,7 @@ namespace {
 constexpr int kS = 128;   // sequence length handled by this kernel
 constexpr int kD = 64;    // head dim
 constexpr int kTile = kS * kD * 2;  // 16 KB: one [128 x 64] bf16 tile
-constexpr int kLdS = kS + 4;        // floats per row of a staged [128 x 128] fp32 tile
-constexpr int kLdO = kD + 4;        // floats per row of a staged [128 x 64] fp32 tile
+constexpr int kThreads = 256;       // two warpgroups
 constexpr float kLog2e = 1.4426950408889634f;
 
 // byte offset of element (row, col) inside a [128 x 64]-bf16 SWIZZLE_128B tile (16B granularity)
@@ -66,11 +68,12 @@ struct AttnDev {
 // ----------------------------------------------------------------------------------------------
 // forward
 // ----------------------------------------------------------------------------------------------
-// Q, K, V, P (2 blocks), mask, barrier, the fp32 staging tile (S, later O)
-constexpr int kFwdOffStage = 5 * kTile + 512 + 64;
-constexpr int kFwdSmem = kFwdOffStage + kS * kLdS * 4 + 1024 /*align*/;
+// Q, K, V, mask, barrier, 8 per-warp staging buffers: 68.6 KB with the alignment slack, so the
+// 128-register budget of __launch_bounds__(256, 2) decides the occupancy (2 CTAs per SM)
+constexpr int kFwdOffStage = 3 * kTile + 512 + 64;
+constexpr int kFwdSmem = kFwdOffStage + 8 * kWarpStageBytes + 1024 /*align*/;
 
-__global__ void __launch_bounds__(128, 1)
+__global__ void __launch_bounds__(kThreads, 2)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnDev p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -78,16 +81,21 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnDev
   uint8_t* sQ = smem;
   uint8_t* sK = smem + kTile;
   uint8_t* sV = smem + 2 * kTile;
-  uint8_t* sP = smem + 3 * kTile;  // two [128 x 64] K-blocks
-  float* sMask = reinterpret_cast<float*>(smem + 5 * kTile);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 5 * kTile + 512);
-  float* sAcc = reinterpret_cast<float*>(smem + kFwdOffStage);
+  float* sMask = reinterpret_cast<float*>(smem + 3 * kTile);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 3 * kTile + 512);
 
   const int tid = threadIdx.x;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+  const int lane = tid & 31;
+  const int wg = warp >> 2;
   const int bh = blockIdx.x;
   const int b = bh / p.heads;
   const int h = bh % p.heads;
+  uint8_t* s_stage = smem + kFwdOffStage + warp * kWarpStageBytes;
+  // my fragment rows are query rows q0 and q0 + 8; my columns in every 8-column block 8j + fc + {0,1}
+  const int wrow0 = wg * 64 + (warp & 3) * 16;
+  const int q0 = wrow0 + (lane >> 2);
+  const int fc = (lane & 3) * 2;
 
   if (tid == 0) {
     tma_prefetch_desc(&tmap_qkv);
@@ -96,7 +104,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnDev
   }
   pdl_wait();
   pdl_launch_dependents();
-  sMask[tid] = p.mask ? p.mask[b * kS + tid] * kLog2e : 0.f;
+  if (tid < kS) sMask[tid] = p.mask ? p.mask[b * kS + tid] * kLog2e : 0.f;
   __syncthreads();
 
   if (warp == 0 && elect_one_sync()) {
@@ -106,105 +114,118 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnDev
     tma_load_2d(sV, &tmap_qkv, &bars[0], 2 * p.H + h * kD, b * kS);
   }
   mbar_wait(&bars[0], 0);
+
+  // S[my 64 rows, 128 keys] = Q K^T
+  float s[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) s[i] = 0.f;
   {
     const uint32_t aq = smem_u32(sQ), ak = smem_u32(sK);
-    wg_mma_to_smem<128, 0, 0, kD / 16>(
-        sAcc, kLdS, [&](int k, int mh) { return desc_kmajor(aq, k, kTile, mh * 64); },
-        [&](int k) { return desc_kmajor(ak, k, kTile, 0); }, tid);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kD / 16; ++k)
+      wgmma_k16<128, 0, 0>(s, desc_kmajor(aq, k, kTile, wg * 64), desc_kmajor(ak, k, kTile, 0), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
   }
-  __syncthreads();
 
-  // ---- softmax over my row (query index = tid) ----
-  const float* srow = sAcc + tid * kLdS;
+  // ---- softmax on the fragments: row max / row sum over my 32 columns, then over the quad ----
   const float sc = p.scale * kLog2e;
-  float mx = -INFINITY;
-#pragma unroll 1
-  for (int c = 0; c < 4; ++c) {
-    uint32_t v[32];
-    row_load32(srow + c * 32, v);
+  float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
-    for (int j = 0; j < 32; ++j) mx = fmaxf(mx, __uint_as_float(v[j]) * sc + sMask[c * 32 + j]);
+  for (int j = 0; j < 16; ++j) {
+    const float m0 = sMask[8 * j + fc], m1 = sMask[8 * j + fc + 1];
+    s[4 * j] = s[4 * j] * sc + m0;
+    s[4 * j + 1] = s[4 * j + 1] * sc + m1;
+    s[4 * j + 2] = s[4 * j + 2] * sc + m0;
+    s[4 * j + 3] = s[4 * j + 3] * sc + m1;
+    mx0 = fmaxf(mx0, fmaxf(s[4 * j], s[4 * j + 1]));
+    mx1 = fmaxf(mx1, fmaxf(s[4 * j + 2], s[4 * j + 3]));
   }
+  mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+  mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+  mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+  mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+  float sum0 = 0.f, sum1 = 0.f;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    s[4 * j] = exp2f(s[4 * j] - mx0);
+    s[4 * j + 1] = exp2f(s[4 * j + 1] - mx0);
+    s[4 * j + 2] = exp2f(s[4 * j + 2] - mx1);
+    s[4 * j + 3] = exp2f(s[4 * j + 3] - mx1);
+    sum0 += s[4 * j];
+    sum0 += s[4 * j + 1];
+    sum1 += s[4 * j + 2];
+    sum1 += s[4 * j + 3];
+  }
+  // the row sum is taken before dropout: it normalises the un-dropped probabilities
+  sum0 += __shfl_xor_sync(0xffffffffu, sum0, 1);
+  sum1 += __shfl_xor_sync(0xffffffffu, sum1, 1);
+  sum0 += __shfl_xor_sync(0xffffffffu, sum0, 2);
+  sum1 += __shfl_xor_sync(0xffffffffu, sum1, 2);
   const bool has_dropout = p.dropout_p > 0.f;
-  uint64_t seed = 0;
-  uint32_t thr16 = 0;
   if (has_dropout) {
-    seed = dropout_seed(p.rng_state, p.rng_stream);
-    thr16 = static_cast<uint32_t>(p.dropout_p * 65536.f);
-  }
-  const uint64_t drop_row = (static_cast<uint64_t>(bh) * kS + tid) * kS;
-  float sum = 0.f;
-#pragma unroll 1
-  for (int c = 0; c < 4; ++c) {
-    uint32_t v[32];
-    row_load32(srow + c * 32, v);
-    float e[32];
+    // element index ((b * heads + h) * S + q) * S + key, as in the host replica (dropout_ref.py)
+    const uint64_t seed = dropout_seed(p.rng_state, p.rng_stream);
+    const uint32_t thr16 = static_cast<uint32_t>(p.dropout_p * 65536.f);
+    const long long row_a = static_cast<long long>(bh) * kS + q0;
 #pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      e[j] = exp2f(__uint_as_float(v[j]) * sc + sMask[c * 32 + j] - mx);
-      sum += e[j];
-    }
-    if (has_dropout) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const uint32_t m = dropout_keep4(seed, (drop_row + c * 32 + j) >> 2, thr16);
-        e[j] = (m & 1u) ? e[j] : 0.f;
-        e[j + 1] = (m & 2u) ? e[j + 1] : 0.f;
-        e[j + 2] = (m & 4u) ? e[j + 2] : 0.f;
-        e[j + 3] = (m & 8u) ? e[j + 3] : 0.f;
-      }
-    }
-    uint8_t* blk = sP + (c >> 1) * kTile;
-#pragma unroll
-    for (int j = 0; j < 32; j += 8) {
-      uint4 pk;
-      pk.x = pack_bf16x2(e[j], e[j + 1]);
-      pk.y = pack_bf16x2(e[j + 2], e[j + 3]);
-      pk.z = pack_bf16x2(e[j + 4], e[j + 5]);
-      pk.w = pack_bf16x2(e[j + 6], e[j + 7]);
-      *reinterpret_cast<uint4*>(blk + sw128_offset(tid, (c & 1) * 32 + j)) = pk;
+    for (int j = 0; j < 16; ++j) {
+      const uint32_t m = frag_keep_bits(seed, thr16, row_a, (j >> 3) * 64, kS, lane, j & 7);
+      s[4 * j] = (m & 1u) ? s[4 * j] : 0.f;
+      s[4 * j + 1] = (m & 2u) ? s[4 * j + 1] : 0.f;
+      s[4 * j + 2] = (m & 4u) ? s[4 * j + 2] : 0.f;
+      s[4 * j + 3] = (m & 8u) ? s[4 * j + 3] : 0.f;
     }
   }
-  if (p.lse != nullptr) p.lse[static_cast<long long>(bh) * kS + tid] = mx + log2f(sum);
-  fence_proxy_async_smem();   // P (generic-proxy stores) -> wgmma (async-proxy reads)
-  __syncthreads();            // also: every row of S has been read, the staging tile is free
+  if (p.lse != nullptr && (lane & 3) == 0) {
+    float* l = p.lse + static_cast<long long>(bh) * kS;
+    l[q0] = mx0 + log2f(sum0);
+    l[q0 + 8] = mx1 + log2f(sum1);
+  }
 
+  // O[my rows, d] = P V: A = bf16 P straight from the score fragments (8 K steps of 16 keys),
+  // B = V (MN-major)
+  uint32_t pa[kS / 16][4];
+#pragma unroll
+  for (int k = 0; k < kS / 16; ++k) frag_to_a(s, k, pa[k]);
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
   {
-    // O[q, d] = sum_key P[q, key] V[key, d]: A = P (K-major, 2 K-blocks), B = V (MN-major)
-    const uint32_t ap = smem_u32(sP), av = smem_u32(sV);
-    wg_mma_to_smem<64, 0, 1, kS / 16>(
-        sAcc, kLdO, [&](int k, int mh) { return desc_kmajor(ap, k, kTile, mh * 64); },
-        [&](int k) { return desc_mnmajor(av, k, kTile, 0); }, tid);
-  }
-  __syncthreads();
-
-  const float inv = (has_dropout ? 1.f / (1.f - p.dropout_p) : 1.f) / sum;
-  __nv_bfloat16* orow = p.ctx + (static_cast<long long>(b) * kS + tid) * p.H + h * kD;
-#pragma unroll 1
-  for (int c = 0; c < 2; ++c) {
-    uint32_t v[32];
-    row_load32(sAcc + tid * kLdO + c * 32, v);
+    const uint32_t av = smem_u32(sV);
+    wgmma_fence();
 #pragma unroll
-    for (int j = 0; j < 32; j += 8) {
-      uint4 pk;
-      pk.x = pack_bf16x2(__uint_as_float(v[j]) * inv, __uint_as_float(v[j + 1]) * inv);
-      pk.y = pack_bf16x2(__uint_as_float(v[j + 2]) * inv, __uint_as_float(v[j + 3]) * inv);
-      pk.z = pack_bf16x2(__uint_as_float(v[j + 4]) * inv, __uint_as_float(v[j + 5]) * inv);
-      pk.w = pack_bf16x2(__uint_as_float(v[j + 6]) * inv, __uint_as_float(v[j + 7]) * inv);
-      *reinterpret_cast<uint4*>(orow + c * 32 + j) = pk;
-    }
+    for (int k = 0; k < kS / 16; ++k)
+      wgmma_rs_k16<64, 1>(o, pa[k], desc_mnmajor(av, k, kTile, 0), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
   }
+
+  const float keep_scale = has_dropout ? 1.f / (1.f - p.dropout_p) : 1.f;
+  const float inv0 = keep_scale / sum0, inv1 = keep_scale / sum1;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    o[4 * j] *= inv0;
+    o[4 * j + 1] *= inv0;
+    o[4 * j + 2] *= inv1;
+    o[4 * j + 3] *= inv1;
+  }
+  frag_store_bf16(o, s_stage, lane, p.ctx, p.H, static_cast<long long>(b) * kS + wrow0, INT_MAX,
+                  h * kD, p.H);
 }
 
 // ----------------------------------------------------------------------------------------------
 // backward
 // ----------------------------------------------------------------------------------------------
-// 8 bf16 tiles (Q, K, V, dO, P0, P1, dS0, dS1) + mask + barrier + two [128 x 64] fp32 staging tiles
-constexpr int kBwdOffStage = 8 * kTile + 512 + 64;
-constexpr int kBwdStage = kS * kLdO * 4;
-constexpr int kBwdSmem = kBwdOffStage + 2 * kBwdStage + 1024 /*align*/;
+// 8 bf16 tiles (Q, K, V, dO, P0, P1, dS0, dS1) + mask, lse, delta + barrier + 8 per-warp staging
+// buffers: 152.6 KB, one CTA per SM
+constexpr int kBwdOffVec = 8 * kTile;  // sMask | sLse | sDelta, 128 floats each
+constexpr int kBwdOffBar = kBwdOffVec + 3 * kS * 4;
+constexpr int kBwdOffStage = kBwdOffBar + 64;
+constexpr int kBwdSmem = kBwdOffStage + 8 * kWarpStageBytes + 1024 /*align*/;
 
-__global__ void __launch_bounds__(128, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
                      const __grid_constant__ CUtensorMap tmap_do, const AttnDev p) {
   extern __shared__ uint8_t smem_raw[];
@@ -217,16 +238,22 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
   uint8_t* sdO = smem + 3 * kTile;
   uint8_t* sP = smem + 4 * kTile;   // 2 blocks: keys 0..63 | 64..127
   uint8_t* sdS = smem + 6 * kTile;  // 2 blocks
-  float* sMask = reinterpret_cast<float*>(smem + 8 * kTile);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 8 * kTile + 512);
-  float* stA = reinterpret_cast<float*>(smem + kBwdOffStage);
-  float* stB = reinterpret_cast<float*>(smem + kBwdOffStage + kBwdStage);
+  float* sMask = reinterpret_cast<float*>(smem + kBwdOffVec);
+  float* sLse = sMask + kS;
+  float* sDelta = sLse + kS;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kBwdOffBar);
 
   const int tid = threadIdx.x;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+  const int lane = tid & 31;
+  const int wg = warp >> 2;
   const int bh = blockIdx.x;
   const int b = bh / p.heads;
   const int h = bh % p.heads;
+  uint8_t* s_stage = smem + kBwdOffStage + warp * kWarpStageBytes;
+  const int wrow0 = wg * 64 + (warp & 3) * 16;
+  const int q0 = wrow0 + (lane >> 2);
+  const int fc = (lane & 3) * 2;
 
   if (tid == 0) {
     tma_prefetch_desc(&tmap_qkv);
@@ -236,7 +263,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
   }
   pdl_wait();
   pdl_launch_dependents();
-  sMask[tid] = p.mask ? p.mask[b * kS + tid] * kLog2e : 0.f;
+  if (tid < kS) sMask[tid] = p.mask ? p.mask[b * kS + tid] * kLog2e : 0.f;
   __syncthreads();
 
   if (warp == 0 && elect_one_sync()) {
@@ -247,9 +274,9 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
     tma_load_2d(sdO, &tmap_do, &bars[0], h * kD, b * kS);
   }
 
-  // delta = rowsum(dO * O) while the loads run (query row = tid)
-  float delta = 0.f;
-  {
+  // delta = rowsum(dO * O) and lse, one thread per query row while the loads run
+  if (tid < kS) {
+    float delta = 0.f;
     const long long off = (static_cast<long long>(b) * kS + tid) * p.H + h * kD;
     const uint4* o4 = reinterpret_cast<const uint4*>(p.ctx_in + off);
     // dO row read from global (also in smem, but swizzled; global read is simpler and cached)
@@ -268,8 +295,12 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
         delta += x.x * y.x + x.y * y.y;
       }
     }
+    sDelta[tid] = delta;
+    sLse[tid] = p.lse[static_cast<long long>(bh) * kS + tid];
   }
-  const float lse = p.lse[static_cast<long long>(bh) * kS + tid];
+  __syncthreads();
+  const float lse0 = sLse[q0], lse1 = sLse[q0 + 8];
+  const float delta0 = sDelta[q0], delta1 = sDelta[q0 + 8];
 
   mbar_wait(&bars[0], 0);
   const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK), aV = smem_u32(sV), adO = smem_u32(sdO);
@@ -285,102 +316,99 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
     thr16 = static_cast<uint32_t>(p.dropout_p * 65536.f);
     dscale = 1.f / (1.f - p.dropout_p);
   }
-  const uint64_t drop_row = (static_cast<uint64_t>(bh) * kS + tid) * kS;
+  const long long row_a = static_cast<long long>(bh) * kS + q0;
 #pragma unroll 1
-  for (int kh = 0; kh < 2; ++kh) {  // 64 keys at a time: S and dP of those keys, all 128 queries
-    wg_mma_to_smem<64, 0, 0, kD / 16>(
-        stA, kLdO, [&](int k, int mh) { return desc_kmajor(aQ, k, kTile, mh * 64); },
-        [&](int k) { return desc_kmajor(aK, k, kTile, kh * 64); }, tid);
-    wg_mma_to_smem<64, 0, 0, kD / 16>(
-        stB, kLdO, [&](int k, int mh) { return desc_kmajor(adO, k, kTile, mh * 64); },
-        [&](int k) { return desc_kmajor(aV, k, kTile, kh * 64); }, tid);
-    __syncthreads();
-#pragma unroll 1
-    for (int cc = 0; cc < 4; ++cc) {  // 16 keys per step
-      const int c = kh * 4 + cc;
-      uint32_t vs[16], vd[16];
-      row_load16(stA + tid * kLdO + cc * 16, vs);
-      row_load16(stB + tid * kLdO + cc * 16, vd);
-      float pd[16], ds[16];
+  for (int kh = 0; kh < 2; ++kh) {  // 64 keys at a time: S and dP of those keys, my 64 queries
+    float s[32], dp[32];
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        pd[j] = exp2f(__uint_as_float(vs[j]) * sc + sMask[c * 16 + j] - lse);
-        ds[j] = __uint_as_float(vd[j]);
-      }
+    for (int i = 0; i < 32; ++i) {
+      s[i] = 0.f;
+      dp[i] = 0.f;
+    }
+    acc_fence(s);
+    acc_fence(dp);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kD / 16; ++k)
+      wgmma_k16<64, 0, 0>(s, desc_kmajor(aQ, k, kTile, wg * 64), desc_kmajor(aK, k, kTile, kh * 64),
+                          1u);
+#pragma unroll
+    for (int k = 0; k < kD / 16; ++k)
+      wgmma_k16<64, 0, 0>(dp, desc_kmajor(adO, k, kTile, wg * 64),
+                          desc_kmajor(aV, k, kTile, kh * 64), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    uint8_t* bp = sP + kh * kTile;
+    uint8_t* bd = sdS + kh * kTile;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int col = 8 * j + fc;  // key kh * 64 + col
+      const float m0 = sMask[kh * 64 + col], m1 = sMask[kh * 64 + col + 1];
+      float pr[4], ds[4];
+      pr[0] = exp2f(s[4 * j] * sc + m0 - lse0);
+      pr[1] = exp2f(s[4 * j + 1] * sc + m1 - lse0);
+      pr[2] = exp2f(s[4 * j + 2] * sc + m0 - lse1);
+      pr[3] = exp2f(s[4 * j + 3] * sc + m1 - lse1);
       if (has_dropout) {
+        const uint32_t m = frag_keep_bits(seed, thr16, row_a, kh * 64, kS, lane, j);
 #pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          const uint32_t m = dropout_keep4(seed, (drop_row + c * 16 + j) >> 2, thr16);
-#pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            const bool keep = (m >> t) & 1u;
-            const float pj = pd[j + t];
-            // dS uses the un-dropped P; the dropped/scaled P feeds dV
-            ds[j + t] = pj * ((keep ? ds[j + t] * dscale : 0.f) - delta) * p.scale;
-            pd[j + t] = keep ? pj * dscale : 0.f;
-          }
+        for (int t = 0; t < 4; ++t) {
+          const bool keep = (m >> t) & 1u;
+          const float pj = pr[t];
+          // dS uses the un-dropped P; the dropped/scaled P feeds dV
+          ds[t] = pj * ((keep ? dp[4 * j + t] * dscale : 0.f) - (t < 2 ? delta0 : delta1)) *
+                  p.scale;
+          pr[t] = keep ? pj * dscale : 0.f;
         }
       } else {
 #pragma unroll
-        for (int j = 0; j < 16; ++j) ds[j] = pd[j] * (ds[j] - delta) * p.scale;
+        for (int t = 0; t < 4; ++t)
+          ds[t] = pr[t] * (dp[4 * j + t] - (t < 2 ? delta0 : delta1)) * p.scale;
       }
-      uint8_t* bp = sP + kh * kTile;
-      uint8_t* bd = sdS + kh * kTile;
-#pragma unroll
-      for (int j = 0; j < 16; j += 8) {
-        const uint32_t off = sw128_offset(tid, cc * 16 + j);
-        uint4 pk;
-        pk.x = pack_bf16x2(pd[j], pd[j + 1]);
-        pk.y = pack_bf16x2(pd[j + 2], pd[j + 3]);
-        pk.z = pack_bf16x2(pd[j + 4], pd[j + 5]);
-        pk.w = pack_bf16x2(pd[j + 6], pd[j + 7]);
-        *reinterpret_cast<uint4*>(bp + off) = pk;
-        pk.x = pack_bf16x2(ds[j], ds[j + 1]);
-        pk.y = pack_bf16x2(ds[j + 2], ds[j + 3]);
-        pk.z = pack_bf16x2(ds[j + 4], ds[j + 5]);
-        pk.w = pack_bf16x2(ds[j + 6], ds[j + 7]);
-        *reinterpret_cast<uint4*>(bd + off) = pk;
-      }
+      const uint32_t off0 = sw128_offset(q0, col), off1 = sw128_offset(q0 + 8, col);
+      *reinterpret_cast<uint32_t*>(bp + off0) = pack_bf16x2(pr[0], pr[1]);
+      *reinterpret_cast<uint32_t*>(bp + off1) = pack_bf16x2(pr[2], pr[3]);
+      *reinterpret_cast<uint32_t*>(bd + off0) = pack_bf16x2(ds[0], ds[1]);
+      *reinterpret_cast<uint32_t*>(bd + off1) = pack_bf16x2(ds[2], ds[3]);
     }
-    fence_proxy_async_smem();
-    __syncthreads();   // staging tiles are free again; P / dS of these keys are visible
   }
+  fence_proxy_async_smem();   // P / dS (generic-proxy stores) -> wgmma (async-proxy reads)
+  __syncthreads();            // dV / dK need the P / dS rows of both warpgroups
 
-  __nv_bfloat16* grow = p.dqkv + (static_cast<long long>(b) * kS + tid) * (3 * p.H) + h * kD;
-  auto store_row = [&](const float* src, __nv_bfloat16* o) {
-#pragma unroll 1
-    for (int c = 0; c < 2; ++c) {
-      uint32_t v[32];
-      row_load32(src + tid * kLdO + c * 32, v);
-#pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        uint4 pk;
-        pk.x = pack_bf16x2(__uint_as_float(v[j]), __uint_as_float(v[j + 1]));
-        pk.y = pack_bf16x2(__uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-        pk.z = pack_bf16x2(__uint_as_float(v[j + 4]), __uint_as_float(v[j + 5]));
-        pk.w = pack_bf16x2(__uint_as_float(v[j + 6]), __uint_as_float(v[j + 7]));
-        *reinterpret_cast<uint4*>(o + c * 32 + j) = pk;
-      }
-    }
-  };
   // dV[key, d] = sum_q P[q,key] dO[q,d] : A = P (MN-major, one key-chunk per block), B = dO (MN)
   // dK[key, d] = sum_q dS[q,key] Q[q,d] : A = dS (MN-major),                         B = Q  (MN)
-  wg_mma_to_smem<64, 1, 1, kS / 16>(
-      stA, kLdO, [&](int k, int mh) { return desc_mnmajor(aP, k, kTile, mh); },
-      [&](int k) { return desc_mnmajor(adO, k, kTile, 0); }, tid);
-  wg_mma_to_smem<64, 1, 1, kS / 16>(
-      stB, kLdO, [&](int k, int mh) { return desc_mnmajor(adS, k, kTile, mh); },
-      [&](int k) { return desc_mnmajor(aQ, k, kTile, 0); }, tid);
-  __syncthreads();
-  store_row(stA, grow + 2 * p.H);
-  store_row(stB, grow + p.H);
-  __syncthreads();
+  // warpgroup w: keys 64w .. 64w + 63 of dV / dK; query rows 64w .. 64w + 63 of
   // dQ[q, d] = sum_key dS[q,key] K[key,d] : A = dS (K-major, 2 K-blocks), B = K (MN-major)
-  wg_mma_to_smem<64, 0, 1, kS / 16>(
-      stA, kLdO, [&](int k, int mh) { return desc_kmajor(adS, k, kTile, mh * 64); },
-      [&](int k) { return desc_mnmajor(aK, k, kTile, 0); }, tid);
-  __syncthreads();
-  store_row(stA, grow);
+  float dv[32], dk[32], dq[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    dv[i] = 0.f;
+    dk[i] = 0.f;
+    dq[i] = 0.f;
+  }
+  acc_fence(dv);
+  acc_fence(dk);
+  acc_fence(dq);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < kS / 16; ++k)
+    wgmma_k16<64, 1, 1>(dv, desc_mnmajor(aP, k, kTile, wg), desc_mnmajor(adO, k, kTile, 0), 1u);
+#pragma unroll
+  for (int k = 0; k < kS / 16; ++k)
+    wgmma_k16<64, 1, 1>(dk, desc_mnmajor(adS, k, kTile, wg), desc_mnmajor(aQ, k, kTile, 0), 1u);
+  wgmma_commit();
+#pragma unroll
+  for (int k = 0; k < kS / 16; ++k)
+    wgmma_k16<64, 0, 1>(dq, desc_kmajor(adS, k, kTile, wg * 64), desc_mnmajor(aK, k, kTile, 0), 1u);
+  wgmma_commit();
+
+  const long long grow0 = static_cast<long long>(b) * kS + wrow0;  // my warp's keys / queries
+  const int ld = 3 * p.H;
+  wgmma_wait<1>();  // dV and dK leave while dQ is still in flight
+  frag_store_bf16(dv, s_stage, lane, p.dqkv, ld, grow0, INT_MAX, 2 * p.H + h * kD, ld);
+  frag_store_bf16(dk, s_stage, lane, p.dqkv, ld, grow0, INT_MAX, p.H + h * kD, ld);
+  wgmma_wait<0>();
+  frag_store_bf16(dq, s_stage, lane, p.dqkv, ld, grow0, INT_MAX, h * kD, ld);
 }
 
 }  // namespace
@@ -424,7 +452,7 @@ int launch_attention_fwd(const AttnArgs& a, cudaStream_t stream) {
   d.dropout_p = a.dropout_p;
   d.rng_state = a.rng_state;
   d.rng_stream = a.rng_stream;
-  cudaError_t le = launch_pdl(attention_fwd_kernel, dim3(a.B * a.heads), dim3(128), kFwdSmem, stream, tm, d);
+  cudaError_t le = launch_pdl(attention_fwd_kernel, dim3(a.B * a.heads), dim3(kThreads), kFwdSmem, stream, tm, d);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
 }
@@ -463,7 +491,7 @@ int launch_attention_bwd(const AttnArgs& a, cudaStream_t stream) {
   d.dropout_p = a.dropout_p;
   d.rng_state = a.rng_state;
   d.rng_stream = a.rng_stream;
-  cudaError_t le = launch_pdl(attention_bwd_kernel, dim3(a.B * a.heads), dim3(128), kBwdSmem, stream, tm, tdo, d);
+  cudaError_t le = launch_pdl(attention_bwd_kernel, dim3(a.B * a.heads), dim3(kThreads), kBwdSmem, stream, tm, tdo, d);
   if (le != cudaSuccess) return static_cast<int>(le);
   return static_cast<int>(cudaGetLastError());
 }

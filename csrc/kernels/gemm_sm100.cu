@@ -49,12 +49,8 @@ constexpr int kNumThreads = 384;
 constexpr int kEpiWarp0 = 4;
 constexpr uint64_t kFlagTimeoutNs = 4000000000ull;  // 4 s
 constexpr int kMaxSmemBytes = 227 * 1024;           // opt-in dynamic shared memory per block (H100)
-
-// Per-warp bf16 staging buffer of the epilogues: the warp's 16 fragment rows x 64 columns, rows
-// 144 B apart (128 B + 16 B pad).  With that stride both the fragment side (4-byte column pairs,
-// 8 rows x 4 lanes) and the global side (16-byte pieces, 8 lanes per row) are bank-conflict free.
-constexpr int kStageLd = 144;
-constexpr int kWarpStageBytes = 16 * kStageLd;
+// the per-warp bf16 staging buffer of the epilogues (kStageLd, kWarpStageBytes) is defined next
+// to frag_store_bf16 in sm100_ptx.cuh
 
 template <int BLOCK_N>
 struct Cfg {
@@ -72,42 +68,13 @@ struct Cfg {
 };
 
 // ---- epilogue on accumulator fragments ----
-// A consumer thread holds, of each 64-column group of its warpgroup's 64 x BLOCK_N accumulator,
-// f[4j], f[4j+1] = (row fr, columns 8j + fc + {0,1}) and f[4j+2], f[4j+3] = (row fr + 8, the same
-// columns), j = 0..7, with fr = lane / 4 and fc = 2 (lane % 4) (see acc_store_smem in
-// sm100_ptx.cuh).  Global memory is reached through the warp's staging buffer `s` for bf16 tiles
-// (coalesced 128-byte rows) and straight from the fragments for fp32 (a quad covers 32 contiguous
-// bytes of a row).  Column bounds are checked per 8-column block (one 16-byte bf16 piece, or the
-// block's column pairs in the fp32 stores); that is exact only because the launchers require
-// N % 8 == 0.  Relaxing that host check needs per-pair checks here first, or ragged tiles would
-// write past column N.
-
-// f (16 rows x 64 columns, bf16) -> gout rows grow0 .. grow0 + 15, columns col0 .. col0 + 63;
-// rows >= m and 8-column pieces >= n are skipped
-__device__ __forceinline__ void frag_store_bf16(const float (&f)[32], uint8_t* s, int lane,
-                                                __nv_bfloat16* gout, long long ld, long long grow0,
-                                                int m, int col0, int n) {
-  uint8_t* mine = s + (lane >> 2) * kStageLd + (lane & 3) * 4;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    *reinterpret_cast<uint32_t*>(mine + j * 16) = pack_bf16x2(f[4 * j], f[4 * j + 1]);
-    *reinterpret_cast<uint32_t*>(mine + 8 * kStageLd + j * 16) =
-        pack_bf16x2(f[4 * j + 2], f[4 * j + 3]);
-  }
-  __syncwarp();
-  const int piece = lane & 7;
-  if (col0 + piece * 8 < n) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int r = i * 4 + (lane >> 3);
-      if (grow0 + r < m) {
-        const uint4 val = *reinterpret_cast<const uint4*>(s + r * kStageLd + piece * 16);
-        *reinterpret_cast<uint4*>(gout + (grow0 + r) * ld + col0 + piece * 8) = val;
-      }
-    }
-  }
-  __syncwarp();
-}
+// The fragment layout, the per-warp staging buffer, frag_store_bf16 and frag_dropout are in
+// sm100_ptx.cuh (the attention kernels use them too).  Global memory is reached through the warp's
+// staging buffer `s` for bf16 tiles (coalesced 128-byte rows) and straight from the fragments for
+// fp32 (a quad covers 32 contiguous bytes of a row).  Column bounds are checked per 8-column block
+// (one 16-byte bf16 piece, or the block's column pairs in the fp32 stores); that is exact only
+// because the launchers require N % 8 == 0.  Relaxing that host check needs per-pair checks here
+// first, or ragged tiles would write past column N.
 
 // coalesced global read of a bf16 16 x 64 block (issued early, it hides behind the epilogue math)
 __device__ __forceinline__ void aux_load(uint4 (&ax)[4], const __nv_bfloat16* aux, long long ld,
@@ -136,30 +103,6 @@ __device__ __forceinline__ void aux_to_frag(const uint4 (&ax)[4], uint8_t* s, in
     a[2 * j + 1] = *reinterpret_cast<const uint32_t*>(mine + 8 * kStageLd + j * 16);
   }
   __syncwarp();
-}
-
-// dropout on fragments with the element-wise mask dropout_keep4(seed, (row * n + col) >> 2).
-// A 4-column group belongs to lanes l and l ^ 1: the even lane hashes it for row fr, the odd lane
-// for row fr + 8, and they swap results.
-__device__ __forceinline__ void frag_dropout(float (&f)[32], uint64_t seed, uint32_t thr16,
-                                             float scale, long long row_a, int col0, int n,
-                                             int lane) {
-  const int odd = lane & 1;
-  const uint64_t row = static_cast<uint64_t>(row_a + (odd ? 8 : 0));
-  const int c4 = col0 + (lane & 2) * 2;  // first column of my 4-column group in block 0
-  const uint32_t sh = odd * 2;           // my column pair's bits in the group's mask
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const uint32_t h =
-        dropout_keep4(seed, (row * static_cast<uint64_t>(n) + c4 + j * 8) >> 2, thr16);
-    const uint32_t o = __shfl_xor_sync(0xffffffffu, h, 1);
-    const uint32_t ma = (odd ? o : h) >> sh;
-    const uint32_t mb = (odd ? h : o) >> sh;
-    f[4 * j] = (ma & 1u) ? f[4 * j] * scale : 0.f;
-    f[4 * j + 1] = (ma & 2u) ? f[4 * j + 1] * scale : 0.f;
-    f[4 * j + 2] = (mb & 1u) ? f[4 * j + 2] * scale : 0.f;
-    f[4 * j + 3] = (mb & 2u) ? f[4 * j + 3] * scale : 0.f;
-  }
 }
 
 struct GemmDev {

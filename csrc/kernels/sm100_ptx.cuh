@@ -287,6 +287,78 @@ __device__ __forceinline__ void wgmma_k16(float (&d)[N / 2], uint64_t desc_a, ui
   if constexpr (N == 128) wgmma_m64n128k16<TA, TB>(d, desc_a, desc_b, scale_d);
   if constexpr (N == 256) wgmma_m64n256k16<TA, TB>(d, desc_a, desc_b, scale_d);
 }
+
+// Register-A wgmma: D[64 x N] (+)= A[64 x 16] (registers) * B (shared memory).  Only B takes a
+// transpose bit in this form (TB = 1: B is MN-major).  A thread's A fragment is four bf16x2 words:
+//   a[0] = (row fr, k 2(l%4) + {0,1}),     a[1] = (row fr + 8, the same k),
+//   a[2] = (row fr, k 8 + 2(l%4) + {0,1}), a[3] = (row fr + 8, the same k),
+// with fr = 16 (warp % 4) + l / 4.  That is the accumulator layout of acc_store_smem restricted to
+// 16 columns, so the accumulator d of columns 16k .. 16k + 15 IS the A fragment of K step k:
+//   a[0] = pack(d[8k], d[8k+1]), a[1] = pack(d[8k+2], d[8k+3]),
+//   a[2] = pack(d[8k+4], d[8k+5]), a[3] = pack(d[8k+6], d[8k+7])
+// (frag_to_a below), and a bf16 probability tile goes from one MMA into the next with no shuffle.
+template <int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_t (&a)[4],
+                                                    uint64_t desc_b, uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1, %38;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]),
+        "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+        "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]),
+        "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]),
+        "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d), "n"(TB));
+}
+template <int TB>
+__device__ __forceinline__ void wgmma_m64n128k16_rs(float (&d)[64], const uint32_t (&a)[4],
+                                                     uint64_t desc_b, uint32_t scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %69, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1, %70;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]),
+        "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+        "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]),
+        "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]),
+        "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+        "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]),
+        "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]),
+        "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
+        "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d), "n"(TB));
+}
+// Pins an accumulator's registers at this point of the instruction stream.  Zero-initialising an
+// accumulator is plain register moves, which the compiler may otherwise sink past an earlier
+// wgmma that is still in flight; ptxas then serialises the two MMAs with an injected wait.
+template <int NREG>
+__device__ __forceinline__ void acc_fence(float (&d)[NREG]) {
+#pragma unroll
+  for (int i = 0; i < NREG; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int N, int TB>
+__device__ __forceinline__ void wgmma_rs_k16(float (&d)[N / 2], const uint32_t (&a)[4],
+                                             uint64_t desc_b, uint32_t scale_d) {
+  static_assert(N == 64 || N == 128, "unsupported register-A wgmma width");
+  if constexpr (N == 64) wgmma_m64n64k16_rs<TB>(d, a, desc_b, scale_d);
+  if constexpr (N == 128) wgmma_m64n128k16_rs<TB>(d, a, desc_b, scale_d);
+}
 // Accumulator fragment of one warpgroup thread: warp w of the group owns rows 16w .. 16w+15; lane l
 // holds, for every 8-column block j, d[4j], d[4j+1] = (row 16w + l/4, columns 8j + 2(l%4) + {0,1})
 // and d[4j+2], d[4j+3] = the same columns of row + 8.  Stores columns [C0, C0 + NC) of the
@@ -445,6 +517,89 @@ __device__ __forceinline__ uint32_t dropout_keep4(uint64_t seed, uint64_t idx4, 
   m |= (static_cast<uint32_t>((r >> 32) & 0xFFFF) >= thr16) ? 4u : 0u;
   m |= (static_cast<uint32_t>((r >> 48) & 0xFFFF) >= thr16) ? 8u : 0u;
   return m;
+}
+
+// ----------------------------------------------------------------------------------------------
+// epilogues on accumulator fragments (GEMM and attention)
+// ----------------------------------------------------------------------------------------------
+// A thread holds, of each 64-column group of its warpgroup's 64 x N accumulator, f[4j], f[4j+1] =
+// (row fr, columns 8j + fc + {0,1}) and f[4j+2], f[4j+3] = (row fr + 8, the same columns), j =
+// 0..7, with fr = lane / 4 and fc = 2 (lane % 4) (see acc_store_smem).
+//
+// Per-warp bf16 staging buffer: the warp's 16 fragment rows x 64 columns, rows 144 B apart (128 B +
+// 16 B pad).  With that stride both the fragment side (4-byte column pairs, 8 rows x 4 lanes) and
+// the global side (16-byte pieces, 8 lanes per row) are bank-conflict free.
+constexpr int kStageLd = 144;
+constexpr int kWarpStageBytes = 16 * kStageLd;
+
+// f (16 rows x 64 columns, bf16) -> gout rows grow0 .. grow0 + 15, columns col0 .. col0 + 63,
+// through the warp's staging buffer `s` so that every global store is a whole 16-byte piece of a
+// 128-byte row; rows >= m and 8-column pieces >= n are skipped
+__device__ __forceinline__ void frag_store_bf16(const float (&f)[32], uint8_t* s, int lane,
+                                                __nv_bfloat16* gout, long long ld, long long grow0,
+                                                int m, int col0, int n) {
+  uint8_t* mine = s + (lane >> 2) * kStageLd + (lane & 3) * 4;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    *reinterpret_cast<uint32_t*>(mine + j * 16) = pack_bf16x2(f[4 * j], f[4 * j + 1]);
+    *reinterpret_cast<uint32_t*>(mine + 8 * kStageLd + j * 16) =
+        pack_bf16x2(f[4 * j + 2], f[4 * j + 3]);
+  }
+  __syncwarp();
+  const int piece = lane & 7;
+  if (col0 + piece * 8 < n) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int r = i * 4 + (lane >> 3);
+      if (grow0 + r < m) {
+        const uint4 val = *reinterpret_cast<const uint4*>(s + r * kStageLd + piece * 16);
+        *reinterpret_cast<uint4*>(gout + (grow0 + r) * ld + col0 + piece * 8) = val;
+      }
+    }
+  }
+  __syncwarp();
+}
+
+// Dropout keep bits of 8-column block j of a fragment group, for the element-wise mask
+// dropout_keep4(seed, (row * n + col) >> 2) with row_a = the global row of fragment row fr and
+// col0 = the group's first column: bits 0, 1 = (row fr, my two columns), bits 2, 3 = (row fr + 8,
+// the same columns).  A 4-column group belongs to lanes l and l ^ 1: the even lane hashes it for
+// row fr, the odd lane for row fr + 8, and they swap results.
+__device__ __forceinline__ uint32_t frag_keep_bits(uint64_t seed, uint32_t thr16, long long row_a,
+                                                   int col0, int n, int lane, int j) {
+  const int odd = lane & 1;
+  const uint64_t row = static_cast<uint64_t>(row_a + (odd ? 8 : 0));
+  const int c4 = col0 + (lane & 2) * 2;  // first column of my 4-column group in block 0
+  const uint32_t sh = odd * 2;           // my column pair's bits in the group's mask
+  const uint32_t h =
+      dropout_keep4(seed, (row * static_cast<uint64_t>(n) + c4 + j * 8) >> 2, thr16);
+  const uint32_t o = __shfl_xor_sync(0xffffffffu, h, 1);
+  const uint32_t ma = (odd ? o : h) >> sh;
+  const uint32_t mb = (odd ? h : o) >> sh;
+  return (ma & 3u) | ((mb & 3u) << 2);
+}
+// dropout on a 64-column fragment group: kept elements are multiplied by `scale`, dropped ones
+// become 0
+__device__ __forceinline__ void frag_dropout(float (&f)[32], uint64_t seed, uint32_t thr16,
+                                             float scale, long long row_a, int col0, int n,
+                                             int lane) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const uint32_t m = frag_keep_bits(seed, thr16, row_a, col0, n, lane, j);
+    f[4 * j] = (m & 1u) ? f[4 * j] * scale : 0.f;
+    f[4 * j + 1] = (m & 2u) ? f[4 * j + 1] * scale : 0.f;
+    f[4 * j + 2] = (m & 4u) ? f[4 * j + 2] * scale : 0.f;
+    f[4 * j + 3] = (m & 8u) ? f[4 * j + 3] * scale : 0.f;
+  }
+}
+
+// accumulator columns 16k .. 16k + 15 -> register A fragment of K step k (see wgmma_m64n64k16_rs)
+template <int NREG>
+__device__ __forceinline__ void frag_to_a(const float (&d)[NREG], int k, uint32_t (&a)[4]) {
+  a[0] = pack_bf16x2(d[8 * k], d[8 * k + 1]);
+  a[1] = pack_bf16x2(d[8 * k + 2], d[8 * k + 3]);
+  a[2] = pack_bf16x2(d[8 * k + 4], d[8 * k + 5]);
+  a[3] = pack_bf16x2(d[8 * k + 6], d[8 * k + 7]);
 }
 
 // One warpgroup (128 threads): dst[128 x N] (fp32 tile in shared memory, leading dimension `ld`

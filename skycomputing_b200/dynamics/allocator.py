@@ -208,8 +208,13 @@ class Allocator:
             res = _core.optimal_partition(uf, um, vdt, vdm, permute=False, min_layers=1,
                                           cut_penalty=self._cut_penalty(units, vdt, uf))
             # the exact solver balanced the most expensive CHUNK (pipeline latency); throughput
-            # is set by the busiest DEVICE (sum of its v chunks): refine towards that
-            bounds = self._refine_device_loads(list(res["boundaries"]), uf, um, dt, dm, D)
+            # is set by the busiest DEVICE (sum of its v chunks): refine towards that, but never
+            # past the most expensive chunk of the even split, so that the result is no worse than
+            # ``even`` on either measure
+            even = _core.even_partition(len(units), VP)
+            even_worst = max(sum(uf[even[k]:even[k + 1]]) * dt[k % D] for k in range(VP))
+            bounds = self._refine_device_loads(list(res["boundaries"]), uf, um, dt, dm, D,
+                                               max_chunk=even_worst * (1.0 + 1e-12))
             self.last_result = dict(res, boundaries=bounds, virtual_stages=v)
         else:
             bounds = _core.even_partition(len(units), VP)
@@ -232,17 +237,19 @@ class Allocator:
         return self._worker_manager
 
     @staticmethod
-    def _refine_device_loads(bounds: List[int], uf, um, dt, dm, D: int) -> List[int]:
+    def _refine_device_loads(bounds: List[int], uf, um, dt, dm, D: int,
+                             max_chunk: float = float("inf")) -> List[int]:
         """Hill-climb on the chunk boundaries of a looped partition (C++ core,
         csrc/alloc/allocator.cc: refine_looped_partition): repeatedly shrink a chunk of the busiest
         device by one unit (handing the unit to the neighbouring chunk, which belongs to another
         device) while that lowers the descending-sorted vector of device loads
         dt[d] x sum(flops of d's chunks); ties are broken towards the smaller most-expensive
-        chunk.  Every chunk keeps >= 1 unit, device memory caps are respected."""
+        chunk.  Every chunk keeps >= 1 unit, device memory caps are respected, and no move makes
+        a chunk cost more than ``max_chunk`` (dt x flops)."""
         assert len(dt) == D and len(dm) == D
         return list(_core.refine_looped_partition([float(x) for x in uf], [float(x) for x in um],
                                                   [float(x) for x in dt], [float(x) for x in dm],
-                                                  [int(x) for x in bounds]))
+                                                  [int(x) for x in bounds], float(max_chunk)))
 
     def allocate(self, alloc_type: str, virtual_stages: int = 1, **kwargs) -> WorkerManager:
         """Dispatch on ``allocator_config['type']`` (experiment/launch.py:119-138 semantics)."""
