@@ -1,8 +1,15 @@
-"""What the pipeline engines share: weight-gradient placement, the device timeline, batch checks.
+"""What the pipeline engines share.
 
-Both ``PipelineEngine`` (one span per rank, sequential / 1F1B) and ``LoopedPipelineEngine`` (v
-chunks per rank on a ring) keep the input-gradient chain of a stage on the critical path and move
-everything that only feeds the optimizer (weight / bias / LayerNorm-parameter gradients) off it:
+``PipelineEngine`` (one span per rank, sequential / 1F1B) and ``LoopedPipelineEngine`` (v chunks
+per rank on a ring) differ in their micro-batch orders and transports.  The base owns the rest:
+construction and ``close()``; ``train_step`` with the whole-step CUDA graph (``_run_graphed``,
+which the single-GPU evaluation graph uses too); the step's preamble, last-stage loss, backward
+and optimizer step; the fused-boundary input and the torch.distributed p2p helpers; ``eval_step``;
+the global gradient norm; the device timeline; batch checks; and the placement of weight
+gradients.
+
+Both engines keep the input-gradient chain of a stage on the critical path and move everything
+that only feeds the optimizer (weight / bias / LayerNorm-parameter gradients) off it:
 
 * ``lazy_stream`` (multi-GPU default): backward only queues those gradients; the queue is launched
   on a SIDE STREAM in front of the next backward, i.e. in front of the kernel that will wait for
@@ -18,17 +25,49 @@ records as parallel branches.  Reference context: scaelum/runner/runner.py:137 r
 """
 from __future__ import annotations
 
+import contextlib
 import os
-from typing import Optional
+from typing import List, Optional, Sequence
 
 import torch
+import torch.distributed as dist
+
+
+def graph_state(warmup: int, key=None) -> dict:
+    """Static buffers and CUDA graph of one captured body (see ``EngineBase._run_graphed``):
+    ``warmup`` eager calls before the capture, ``key`` what the graph was captured for, and the
+    native kernel launches the capture recorded."""
+    return dict(warmup=warmup, key=key, inputs=None, labels=None, graph=None, eager=0, launches=0)
 
 
 class EngineBase:
-    """Mixin state + helpers; concrete engines set ``device``, ``m``, ``is_first``, ``is_last``,
-    ``mb_batch`` and call ``_init_common()`` from their constructor."""
+    """State + helpers of both engines.  A concrete engine sets ``is_first``, ``is_last``, ``P``
+    and ``schedule``, calls ``EngineBase.__init__`` from its constructor and provides ``_setup``,
+    ``_step_body`` and ``forward_only``."""
 
-    def _init_common(self) -> None:
+    def __init__(self, stages: Sequence, device: torch.device, optimizer, loss_fn,
+                 micro_batches: int, boundary: str, use_cuda_graph: bool, group,
+                 advance_rng: bool) -> None:
+        self.stages = list(stages)
+        for st in self.stages:
+            st.engine_managed_backward = True
+        self.device = device
+        self.optimizer = optimizer
+        self.loss_fn = loss_fn
+        self.m = micro_batches
+        self.boundary = boundary
+        self.group = group
+        self._advance_rng = advance_rng
+        self._want_graph = use_cuda_graph and device.type == "cuda"
+        self.graphable = False
+        self._setup_done = False
+        self.mb_batch = self.seq = 0
+        self.fused = None
+        self.in_fused = self.out_fused = False
+        self._loss_acc: Optional[torch.Tensor] = None
+        self._pending_sends: list = []
+        self._step = graph_state(warmup=3)     # the whole training step
+        self._eval: Optional[dict] = None      # the evaluation graph (PipelineEngine, 1 GPU)
         self._defer_wgrad = False
         self._wgrad_stream = None
         self._wgrad_forked = False
@@ -47,6 +86,228 @@ class EngineBase:
         self._trace_tags: list = []
         self._trace_capacity = 0
         self._norm_exchange = None
+
+    # the captured training step (None until it is captured), the native kernel launches of one
+    # replay, and its static input / label buffers
+    @property
+    def _graph(self) -> Optional[torch.cuda.CUDAGraph]:
+        return self._step["graph"]
+
+    @property
+    def launches_per_step(self) -> int:
+        return self._step["launches"]
+
+    @property
+    def _static_inputs(self) -> Optional[list]:
+        return self._step["inputs"]
+
+    @property
+    def _static_labels(self) -> Optional[torch.Tensor]:
+        return self._step["labels"]
+
+    def close(self) -> None:
+        if self.device.type == "cuda":
+            torch.cuda.synchronize(self.device)  # nothing of ours may still touch a peer region
+        self._eval = None   # the evaluation graph is rebuilt by the next engine
+        self._close_grad_norm()
+        if self.fused is not None:
+            self.fused.close()
+            self.fused = None
+        self._release_wgrad_switches()
+
+    # ------------------------------------------------------------------ setup
+    def _setup_batch_shape(self, inputs, src: Optional[int]) -> None:
+        """``mb_batch`` and ``seq`` of the first stage's micro-batches, broadcast from rank ``src``
+        (None: a single rank).  Collective."""
+        shape = [0, 0]
+        if self.is_first and inputs is not None:
+            x = inputs[0]
+            shape = [x.shape[0] // self.m, int(x.shape[1]) if x.dim() > 1 else 0]
+        if src is not None:
+            box = [shape]
+            dist.broadcast_object_list(box, src=src, group=self.group)
+            shape = box[0]
+        self.mb_batch, self.seq = shape
+
+    def _setup_graphable(self, capturable: bool) -> None:
+        """``capturable``: the step runs native kernels only and every link of this rank is fused
+        (or absent), i.e. nothing but the optimizer can keep the step out of a CUDA graph."""
+        # only an optimizer whose step() is pure device work may be captured (a torch.optim class
+        # behind TorchOptimizerAdapter keeps host-side state and refreshes the bf16 shadows through
+        # a host-side version check: replaying it would train on stale weights)
+        self.graphable = self._want_graph and capturable and \
+            bool(getattr(self.optimizer, "graph_safe", False))
+        if self.graphable:
+            # device timers cannot be recorded inside a captured graph
+            for st in self.stages:
+                st._record_forward_time = False
+                st._logger = None
+
+    # ------------------------------------------------------------------ one optimisation step
+    def train_step(self, inputs: Optional[Sequence[torch.Tensor]] = None,
+                   labels: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
+        """Run one optimisation step; returns the (mean) loss tensor on the last stage."""
+        if not self._setup_done:
+            self._setup(inputs)
+            self._loss_acc = torch.zeros((), dtype=torch.float32, device=self.device)
+        self._check_batch(inputs, labels)
+        if self.graphable:
+            self._run_graphed(self._step, self._step_body,
+                              inputs if self.is_first else None, labels if self.is_last else None)
+        else:
+            self._step_body(inputs, labels)
+        return self._loss_acc if self.is_last else None
+
+    def _run_graphed(self, state: dict, body, inputs, labels) -> None:
+        """``body(inputs, labels)`` through the CUDA graph of ``state`` (``graph_state``): the
+        arguments are copied into static buffers, the first ``warmup`` calls run eagerly on them
+        (allocations, lazily created attributes), the next one captures and, since capture only
+        records, replays right away so that its batch is processed; every later call replays."""
+        if state["inputs"] is None:
+            state["inputs"] = [t.clone() for t in inputs] if inputs is not None else []
+            state["labels"] = labels.clone() if labels is not None else None
+        for s, t in zip(state["inputs"], inputs or ()):
+            s.copy_(t, non_blocking=True)
+        if state["labels"] is not None and labels is not None:
+            state["labels"].copy_(labels, non_blocking=True)
+        if state["graph"] is None and state["eager"] < state["warmup"]:
+            body(state["inputs"], state["labels"])
+            state["eager"] += 1
+            return
+        if state["graph"] is None:
+            from ..ops import native as nat
+
+            torch.cuda.synchronize(self.device)
+            g = torch.cuda.CUDAGraph()
+            before = nat.launch_count()
+            with torch.cuda.graph(g):
+                body(state["inputs"], state["labels"])
+            state["launches"] = nat.launch_count() - before
+            state["graph"] = g
+        state["graph"].replay()
+
+    def _begin_step(self, inputs, labels):
+        """Start of a step body: boundary epoch, dropout RNG, loss accumulator, timeline; returns
+        the per-micro-batch input chunks (first stage) and label chunks (last stage)."""
+        from ..models.bert_layers import advance_rng
+
+        if self.fused is not None:
+            self.fused.begin_step()
+        if self._advance_rng and self._native_active():
+            advance_rng()
+        self._loss_acc.zero_()
+        self._trace_tags = []
+        self._mark(("STEP", 0, "begin"))
+        chunks = [t.chunk(self.m, dim=0) for t in inputs] if self.is_first else None
+        label_chunks = labels.chunk(self.m, dim=0) if (self.is_last and labels is not None) else None
+        return chunks, label_chunks
+
+    def _last_stage_loss(self, logits, labels):
+        """The loss of one micro-batch on the last stage, added into ``_loss_acc``."""
+        if hasattr(self.loss_fn, "fused") and logits.is_cuda and self._loss_acc.dtype == torch.float32:
+            # (dlogits,) instead of a scalar loss: see _NativeCrossEntropy.fused
+            return (self.loss_fn.fused(logits, labels, 1.0 / self.m, self._loss_acc.view(1)),)
+        loss = self.loss_fn(logits, labels) / self.m
+        self._loss_acc += loss.detach().float()
+        return loss
+
+    @staticmethod
+    def _backward_from_loss(outs, loss) -> None:
+        if isinstance(loss, tuple):
+            torch.autograd.backward([outs[0]], [loss[0].to(outs[0].dtype)])
+        else:
+            loss.backward()
+
+    @staticmethod
+    def _backward_from_grads(outs, grads) -> None:
+        """Backward from the received gradients of the outputs that require grad."""
+        ts, gs = [], []
+        for o, g in zip(outs, grads):
+            if g is not None and torch.is_tensor(o) and o.requires_grad:
+                ts.append(o)
+                gs.append(g.to(o.dtype))
+        torch.autograd.backward(ts, gs)
+
+    def _optimizer_step(self, pending: list) -> None:
+        """The optimizer step at the end of a step; ``pending`` (outstanding p2p sends) is waited
+        for and emptied."""
+        self._mark(("OPT", 0, "begin"))
+        if pending and self._sends_before_optimizer():
+            self.comm.wait(pending)
+            pending.clear()
+        self.optimizer.step()
+        self._mark(("OPT", 0, "end"))
+        if pending:
+            self.comm.wait(pending)
+            pending.clear()
+
+    # ------------------------------------------------------------------ boundaries
+    def _fused_inputs(self, slot: int):
+        """(activation, additive mask) of inbound fused-boundary slot ``slot``."""
+        from ..ops import native as nat
+
+        ch = self.fused.prev
+        rows = self.mb_batch * self.seq
+        # the additive mask rides next to the activation slot under its own flag
+        nat.ext().wait_flags(ch.local.mask_flag_ptr(slot), 1, ch.epoch_ptr, 1, ch.error_ptr,
+                             torch.cuda.current_stream().cuda_stream)
+        x = ch.act_view(slot, rows, ch.cols).view(self.mb_batch, self.seq, ch.cols)
+        x.requires_grad_(True)
+        mask = ch.mask_view(slot, rows).view(self.mb_batch, 1, 1, self.seq)
+        return (x, mask)
+
+    @staticmethod
+    def _diff_flags(tensors) -> List[bool]:
+        """Which boundary tensors carry gradients: floating tensors, except a trailing additive
+        mask when several tensors cross the boundary.  Both sides of a link apply this rule, so
+        gradient messages need no metadata handshake."""
+        n = len(tensors)
+        return [torch.is_tensor(t) and t.is_floating_point() and (i < n - 1 or n == 1)
+                for i, t in enumerate(tensors)]
+
+    def _prep_inputs(self, tensors):
+        for t, d in zip(tensors, self._diff_flags(tensors)):
+            if d:
+                t.requires_grad_(True)
+        return tuple(tensors)
+
+    def _grad_metas(self, outs):
+        return [(o.dtype, tuple(o.shape)) if d else None
+                for o, d in zip(outs, self._diff_flags(outs))]
+
+    def _in_grads(self, args):
+        out = []
+        for a, d in zip(args, self._diff_flags(args)):
+            if not d:
+                out.append(None)
+            else:
+                out.append(a.grad if a.grad is not None else torch.zeros_like(a))
+        return out
+
+    # ------------------------------------------------------------------ evaluation
+    def eval_step(self, inputs: Optional[Sequence[torch.Tensor]], labels: Optional[torch.Tensor],
+                  accum, micro_batches: Optional[int] = None) -> None:
+        """One evaluation batch: ``forward_only`` and, on the last stage, ``accum.add(logits,
+        labels)`` per micro-batch, with the forward-time probes of every local stage suspended."""
+        m = int(micro_batches or self.m)
+        if self.is_first and inputs[0].shape[0] % m:
+            raise ValueError("an evaluation batch of {} samples cannot be split into {} equal "
+                             "micro-batches".format(inputs[0].shape[0], m))
+        with contextlib.ExitStack() as stack:
+            for st in self.stages:
+                stack.enter_context(st.suspend_forward_probes())
+            self._eval_pass(inputs, labels, accum, m)
+
+    def _eval_pass(self, inputs, labels, accum, m: int) -> None:
+        """The evaluation batch of ``eval_step``; PipelineEngine may replay it from a graph."""
+        self._eval_body(inputs, labels, accum, m)
+
+    def _eval_body(self, inputs, labels, accum, m: int) -> None:
+        res = self.forward_only(inputs, micro_batches=m)
+        if self.is_last:
+            res = [res] if m == 1 else res
+            for outs, lab in zip(res, labels.chunk(m, dim=0)):
+                accum.add(outs[0], lab)
 
     # ------------------------------------------------------------------ global gradient norm
     def _norm_info(self) -> tuple:
@@ -114,7 +375,7 @@ class EngineBase:
             set_wgrad_stream(self._wgrad_stream)
 
     def _slowdown_factor(self) -> float:
-        return 0.0
+        return max(float(getattr(st, "_slowdown", 0) or 0) for st in self.stages)
 
     def _flush_wgrads(self) -> None:
         if not self._defer_wgrad:
@@ -179,7 +440,7 @@ class EngineBase:
         self._trace = True
 
     def _trace_slots(self) -> int:
-        return 8 * (2 * self.m + 4) + 64
+        return 8 * (2 * len(self.stages) * self.m + 4) + 64
 
     def _mark(self, tag) -> None:
         if self._nvtx and self.device.type == "cuda":

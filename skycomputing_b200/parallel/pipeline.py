@@ -25,7 +25,7 @@ import torch
 import torch.distributed as dist
 
 from ..builder.module_wrapper import ModuleWrapper
-from .engine_base import EngineBase
+from .engine_base import EngineBase, graph_state
 
 
 def one_f_one_b_order(stage: int, num_stages: int, micro_batches: int) -> List[tuple]:
@@ -60,51 +60,22 @@ class PipelineEngine(EngineBase):
                  group=None, advance_rng: bool = True):
         assert schedule in ("1f1b", "sequential"), schedule
         assert boundary in ("auto", "fused", "nccl", "gloo", "dist"), boundary
+        super().__init__([stage], device, optimizer, loss_fn, micro_batches, boundary,
+                         use_cuda_graph, group, advance_rng)
         self.stage = stage
         self.s, self.P = stage_index, num_stages
         self.stage_to_rank = list(stage_to_rank)
-        self.device = device
-        self.optimizer = optimizer
-        self.loss_fn = loss_fn
-        self.m = micro_batches
         self.schedule = schedule
-        self.boundary = boundary
-        self.group = group
         self.is_first, self.is_last = stage_index == 0, stage_index == num_stages - 1
         self.prev_rank = None if self.is_first else self.stage_to_rank[stage_index - 1]
         self.next_rank = None if self.is_last else self.stage_to_rank[stage_index + 1]
         self.comm = None
-        self.fused = None
-        self.in_fused = self.out_fused = False
-        self._setup_done = False
-        self._want_graph = use_cuda_graph and device.type == "cuda"
-        self._graph = None
-        self._static_inputs: Optional[list] = None
-        self._static_labels: Optional[torch.Tensor] = None
-        self._loss_acc: Optional[torch.Tensor] = None
-        self._eager_steps = 0
-        self._advance_rng = advance_rng
-        self._pending_sends: list = []
         self._eval_comm_obj = None      # forward-only transport when training needs none
-        self._eval: Optional[dict] = None   # the evaluation CUDA graph and its static buffers
-        self.stage.engine_managed_backward = True
-        self.launches_per_step = 0
-        self._init_common()
 
     # ------------------------------------------------------------------ setup
     def _setup(self, inputs: Optional[Sequence[torch.Tensor]]) -> None:
         multi = self.P > 1
-        shape = [0, 0]
-        if multi:
-            if self.is_first:
-                b = inputs[0].shape[0]
-                shape = [b // self.m, int(inputs[0].shape[1]) if inputs[0].dim() > 1 else 0]
-            obj = [shape]
-            dist.broadcast_object_list(obj, src=self.stage_to_rank[0], group=self.group)
-            shape = obj[0]
-        elif inputs is not None:
-            shape = [inputs[0].shape[0] // self.m, int(inputs[0].shape[1]) if inputs[0].dim() > 1 else 0]
-        self.mb_batch, self.seq = shape
+        self._setup_batch_shape(inputs, self.stage_to_rank[0] if multi else None)
         want_fused = self.boundary in ("auto", "fused") and self._native_active() and multi
         in_ok = out_ok = False
         hidden = 0
@@ -141,16 +112,8 @@ class PipelineEngine(EngineBase):
 
                 self.comm = TorchDistComm(self.device, group=self.group)
             self._setup_grad_norm(self.s, self.P, self.stage_to_rank, [f[4] for f in flags])
-        # only an optimizer whose step() is pure device work may be captured (a torch.optim class
-        # behind TorchOptimizerAdapter keeps host-side state and refreshes the bf16 shadows through
-        # a host-side version check: replaying it would train on stale weights)
-        self.graphable = self._want_graph and self._native_active() and \
-            (self.is_first or self.in_fused) and (self.is_last or self.out_fused) and \
-            bool(getattr(self.optimizer, "graph_safe", False))
-        if self.graphable:
-            # device timers cannot be recorded inside a captured graph
-            self.stage._record_forward_time = False
-            self.stage._logger = None
+        self._setup_graphable(self._native_active() and (self.is_first or self.in_fused) and
+                              (self.is_last or self.out_fused))
         self._configure_wgrad(multi)
         self._order = (one_f_one_b_order if self.schedule == "1f1b" else sequential_order)(
             self.s, self.P, self.m)
@@ -169,17 +132,7 @@ class PipelineEngine(EngineBase):
         if self.is_first:
             return tuple(c[j] for c in chunks)
         if self.in_fused:
-            ch = self.fused.prev
-            from ..ops import native as nat
-
-            rows = self.mb_batch * self.seq
-            # the additive mask rides next to the activation slot under its own flag
-            nat.ext().wait_flags(ch.local.mask_flag_ptr(j), 1, ch.epoch_ptr, 1, ch.error_ptr,
-                                 torch.cuda.current_stream().cuda_stream)
-            x = ch.act_view(j, rows, ch.cols).view(self.mb_batch, self.seq, ch.cols)
-            x.requires_grad_(True)
-            mask = ch.mask_view(j, self.mb_batch * self.seq).view(self.mb_batch, 1, 1, self.seq)
-            return (x, mask)
+            return self._fused_inputs(j)
         return None  # filled by the comm path
 
     def _forward(self, j: int, args, labels_chunks):
@@ -195,16 +148,7 @@ class PipelineEngine(EngineBase):
         self._mark(("F", j, "end"))
         if self.out_fused and self.is_first:
             self.fused.next.send_mask(outs[-1], j)  # produced by the embeddings of this stage
-        loss = None
-        if self.is_last:
-            logits = outs[0]
-            if hasattr(self.loss_fn, "fused") and logits.is_cuda and self._loss_acc.dtype == torch.float32:
-                # (dlogits,) instead of a scalar loss: see _NativeCrossEntropy.fused
-                loss = (self.loss_fn.fused(logits, labels_chunks[j], 1.0 / self.m,
-                                           self._loss_acc.view(1)),)
-            else:
-                loss = self.loss_fn(logits, labels_chunks[j]) / self.m
-                self._loss_acc += loss.detach().float()
+        loss = self._last_stage_loss(outs[0], labels_chunks[j]) if self.is_last else None
         return outs, loss
 
     def _backward(self, j: int, outs, loss, grads, args):
@@ -220,62 +164,23 @@ class PipelineEngine(EngineBase):
         self._mark(("B", j, "begin"))
         st.begin_backward()
         if self.is_last:
-            if isinstance(loss, tuple):
-                torch.autograd.backward([outs[0]], [loss[0].to(outs[0].dtype)])
-            else:
-                loss.backward()
+            self._backward_from_loss(outs, loss)
         elif self.out_fused:
             dummy = outs[0]
             torch.autograd.backward([dummy], [torch.zeros_like(dummy)])
         else:
-            ts, gs = [], []
-            for o, g in zip(outs, grads):
-                if g is not None and torch.is_tensor(o) and o.requires_grad:
-                    ts.append(o)
-                    gs.append(g.to(o.dtype))
-            torch.autograd.backward(ts, gs)
+            self._backward_from_grads(outs, grads)
         st.end_backward()
         self._mark(("B", j, "end"))
         if self.is_first or self.in_fused:
             return None
         return self._in_grads(args)
 
-    def _slowdown_factor(self) -> float:
-        return float(getattr(self.stage, "_slowdown", 0) or 0)
-
     # ------------------------------------------------------------------ comm helpers (unfused)
-    @staticmethod
-    def _diff_flags(tensors) -> List[bool]:
-        """Which boundary tensors carry gradients: floating tensors, except a trailing additive
-        mask when several tensors cross the boundary.  Both sides of a link apply this rule, so
-        gradient messages need no metadata handshake."""
-        n = len(tensors)
-        return [torch.is_tensor(t) and t.is_floating_point() and (i < n - 1 or n == 1)
-                for i, t in enumerate(tensors)]
-
     def _recv_forward(self):
         outs, reqs = self.comm.recv(self.prev_rank, "fwd")
         self.comm.wait(reqs)
         return self._prep_inputs(outs)
-
-    def _prep_inputs(self, tensors):
-        for t, d in zip(tensors, self._diff_flags(tensors)):
-            if d:
-                t.requires_grad_(True)
-        return tuple(tensors)
-
-    def _grad_metas(self, outs):
-        return [(o.dtype, tuple(o.shape)) if d else None
-                for o, d in zip(outs, self._diff_flags(outs))]
-
-    def _in_grads(self, args):
-        out = []
-        for a, d in zip(args, self._diff_flags(args)):
-            if not d:
-                out.append(None)
-            else:
-                out.append(a.grad if a.grad is not None else torch.zeros_like(a))
-        return out
 
     def _send_forward(self, outs):
         self._pending_sends += self.comm.send([o.detach() if torch.is_tensor(o) else None
@@ -305,17 +210,7 @@ class PipelineEngine(EngineBase):
 
     # ------------------------------------------------------------------ one optimisation step
     def _step_body(self, inputs, labels):
-        from ..models.bert_layers import advance_rng
-
-        if self.fused is not None:
-            self.fused.begin_step()
-        if self._advance_rng and self._native_active():
-            advance_rng()
-        self._loss_acc.zero_()
-        self._trace_tags = []
-        self._mark(("STEP", 0, "begin"))
-        chunks = [t.chunk(self.m, dim=0) for t in inputs] if self.is_first else None
-        label_chunks = labels.chunk(self.m, dim=0) if (self.is_last and labels is not None) else None
+        chunks, label_chunks = self._begin_step(inputs, labels)
         need_recv_f = not self.is_first and not self.in_fused
         need_send_f = not self.is_last and not self.out_fused
         need_recv_b = need_send_f
@@ -355,54 +250,7 @@ class PipelineEngine(EngineBase):
         self._join_wgrads()
         if self.fused is not None:
             self.fused.end_of_backward()
-        self._mark(("OPT", 0, "begin"))
-        if self.comm is not None and self._sends_before_optimizer():
-            self.comm.wait(self._pending_sends)
-            self._pending_sends = []
-        self.optimizer.step()
-        self._mark(("OPT", 0, "end"))
-        if self.comm is not None:
-            self.comm.wait(self._pending_sends)
-            self._pending_sends = []
-
-    def train_step(self, inputs: Optional[Sequence[torch.Tensor]] = None,
-                   labels: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
-        """Run one optimisation step; returns the (mean) loss tensor on the last stage."""
-        if not self._setup_done:
-            self._setup(inputs)
-            self._loss_acc = torch.zeros((), dtype=torch.float32, device=self.device)
-        self._check_batch(inputs, labels)
-        if not self.graphable:
-            self._step_body(inputs, labels)
-            return self._loss_acc if self.is_last else None
-        # ---- CUDA-graph path: static input buffers, 3 eager steps, then capture + replay ----
-        if self._static_inputs is None:
-            self._static_inputs = [t.clone() for t in inputs] if self.is_first else []
-            self._static_labels = labels.clone() if (self.is_last and labels is not None) else None
-        if self.is_first:
-            for s, t in zip(self._static_inputs, inputs):
-                s.copy_(t, non_blocking=True)
-        if self._static_labels is not None and labels is not None:
-            self._static_labels.copy_(labels, non_blocking=True)
-        if self._graph is None and self._eager_steps < 3:
-            self._step_body(self._static_inputs, self._static_labels)
-            self._eager_steps += 1
-            return self._loss_acc if self.is_last else None
-        if self._graph is None:
-            torch.cuda.synchronize(self.device)
-            from ..ops import native as nat
-
-            g = torch.cuda.CUDAGraph()
-            before = nat.launch_count()
-            with torch.cuda.graph(g):
-                self._step_body(self._static_inputs, self._static_labels)
-            self.launches_per_step = nat.launch_count() - before
-            self._graph = g
-            # capture only records: replay right away so that this step's batch is trained on
-            self._graph.replay()
-            return self._loss_acc if self.is_last else None
-        self._graph.replay()
-        return self._loss_acc if self.is_last else None
+        self._optimizer_step(self._pending_sends)
 
     # ------------------------------------------------------------------ forward only (eval)
     def _eval_comm(self):
@@ -450,61 +298,21 @@ class PipelineEngine(EngineBase):
             return None
         return results[0] if m == 1 else results
 
-    def eval_step(self, inputs: Optional[Sequence[torch.Tensor]], labels: Optional[torch.Tensor],
-                  accum, micro_batches: Optional[int] = None) -> None:
-        """One evaluation batch: ``forward_only`` and, on the last stage, ``accum.add(logits,
-        labels)`` per micro-batch.  On one GPU with the native kernels and ``use_cuda_graph`` the
-        whole batch (forward + accumulation) is captured into its own CUDA graph after one eager
-        pass and replayed; it touches neither the dropout RNG, the boundary epochs, the training
-        loss nor the optimizer."""
-        m = int(micro_batches or self.m)
-        if self.is_first and inputs[0].shape[0] % m:
-            raise ValueError("an evaluation batch of {} samples cannot be split into {} equal "
-                             "micro-batches".format(inputs[0].shape[0], m))
-        with self.stage.suspend_forward_probes():
-            # the graph reads the bf16 weight copies in place: only an optimizer that refreshes
-            # them on the device (graph_safe) keeps a captured evaluation current
-            if self.P == 1 and self._want_graph and self._native_active() and \
-                    bool(getattr(self.optimizer, "graph_safe", False)):
-                self._eval_graph_step(inputs, labels, accum, m)
-            else:
-                self._eval_body(inputs, labels, accum, m)
-
-    def _eval_body(self, inputs, labels, accum, m: int) -> None:
-        res = self.forward_only(inputs, micro_batches=m)
-        if self.is_last:
-            res = [res] if m == 1 else res
-            for outs, lab in zip(res, labels.chunk(m, dim=0)):
-                accum.add(outs[0], lab)
-
-    def _eval_graph_step(self, inputs, labels, accum, m: int) -> None:
-        key = (tuple((tuple(t.shape), t.dtype) for t in inputs), tuple(labels.shape), m, id(accum))
-        ev = self._eval
-        if ev is None or ev["key"] != key:
-            # one evaluation graph per engine: a new shape / accumulator replaces the old one
-            ev = self._eval = dict(key=key, inputs=[t.clone() for t in inputs],
-                                   labels=labels.clone(), graph=None, eager=0, accum=accum)
-        for s_, t in zip(ev["inputs"], inputs):
-            s_.copy_(t, non_blocking=True)
-        ev["labels"].copy_(labels, non_blocking=True)
-        if ev["graph"] is None and ev["eager"] < 1:
-            self._eval_body(ev["inputs"], ev["labels"], accum, m)   # warm-up: allocations, attrs
-            ev["eager"] += 1
+    def _eval_pass(self, inputs, labels, accum, m: int) -> None:
+        """On one GPU with the native kernels and ``use_cuda_graph`` the whole batch (forward +
+        accumulation) is captured into its own CUDA graph after one eager pass and replayed; it
+        touches neither the dropout RNG, the boundary epochs, the training loss nor the optimizer.
+        One evaluation graph per engine: a batch of other shapes, another ``m`` or another
+        accumulator replaces it."""
+        # the graph reads the bf16 weight copies in place: only an optimizer that refreshes them
+        # on the device (graph_safe) keeps a captured evaluation current
+        if not (self.P == 1 and self._want_graph and self._native_active() and
+                bool(getattr(self.optimizer, "graph_safe", False))):
+            self._eval_body(inputs, labels, accum, m)
             return
-        if ev["graph"] is None:
-            torch.cuda.synchronize(self.device)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._eval_body(ev["inputs"], ev["labels"], accum, m)
-            ev["graph"] = g
-        ev["graph"].replay()
-
-    def close(self) -> None:
-        if self.device.type == "cuda":
-            torch.cuda.synchronize(self.device)  # nothing of ours may still touch a peer region
-        self._eval = None   # the evaluation graph is rebuilt by the next engine
-        self._close_grad_norm()
-        if self.fused is not None:
-            self.fused.close()
-            self.fused = None
-        self._release_wgrad_switches()
+        # the accumulator object is part of the key: the graph adds into its buffer, which the
+        # key keeps alive
+        key = (tuple((tuple(t.shape), t.dtype) for t in inputs), tuple(labels.shape), m, accum)
+        if self._eval is None or self._eval["key"] != key:
+            self._eval = graph_state(warmup=1, key=key)
+        self._run_graphed(self._eval, lambda x, y: self._eval_body(x, y, accum, m), inputs, labels)

@@ -14,18 +14,17 @@ costs 1/v of a rank's work, so the step is ``m x T + (P - 1) x (F + B) / v`` as 
 easily for the models this framework targets.  Weight gradients use the same deferral as the
 plain engine.
 
-Transport: ``torch.distributed`` point-to-point by default (gloo on CPU, NCCL on GPUs) - both ends
-of a link post their transfers in the same (chunk, micro-batch) order, so plain FIFO matching is
-enough and no tags are needed.  ``boundary="fused"`` (``SKY_LOOPED_FUSED=1``) switches to the
-plain engine's peer-memory boundary: the ranks form a RING of ``FusedChannel``s (incl. the
-wrap-around link), one slot per (chunk, micro-batch), and the whole step is captured into one CUDA
-graph.  The p2p path is covered by the CPU tests (tests/test_pipeline_cpu.py); the fused path is
-written against the same kernels / flag protocol but has not been run on GPUs yet (DESIGN.md §7),
-which is why it is opt-in.
+Transport: ``boundary="auto"`` / ``"fused"`` uses the plain engine's peer-memory boundary when
+every chunk of every rank supports it on the native path: the ranks form a RING of
+``FusedChannel``s (incl. the wrap-around link), one slot per (chunk, micro-batch), and the whole
+step is captured into one CUDA graph.  The Runner selects it by default (``SKY_LOOPED_FUSED=0``
+turns it off); tests/test_multi_gpu.py runs it on 2, 4 and 8 GPUs.  Otherwise the boundaries are
+``torch.distributed`` point-to-point (gloo on CPU, NCCL on GPUs): both ends of a link post their
+transfers in the same (chunk, micro-batch) order, so plain FIFO matching is enough; the CPU tests
+(tests/test_pipeline_cpu.py) run this path.
 """
 from __future__ import annotations
 
-import contextlib
 from typing import Callable, List, Optional, Sequence
 
 import torch
@@ -49,7 +48,8 @@ class LoopedPipelineEngine(EngineBase):
                  advance_rng: bool = True, boundary: str = "dist", use_cuda_graph: bool = True):
         """``stages[i]`` is the ModuleWrapper of virtual stage ``virtual_indices[i]``; ``ring[p]`` is
         the process rank at ring position p (virtual stage k lives at position k % num_ranks)."""
-        self.stages = list(stages)
+        super().__init__(stages, device, optimizer, loss_fn, micro_batches, boundary,
+                         use_cuda_graph, group, advance_rng)
         self.vidx = list(virtual_indices)
         self.P = num_ranks
         self.v = len(self.stages)
@@ -60,37 +60,13 @@ class LoopedPipelineEngine(EngineBase):
         self.s = self.pos                                 # ring position (trace / log naming)
         assert self.vidx == [c * self.P + self.pos for c in range(self.v)], self.vidx
         self.ring = list(ring)
-        self.device = device
-        self.optimizer = optimizer
-        self.loss_fn = loss_fn
-        self.m = micro_batches
-        self.group = group
         self.prev_rank = self.ring[(self.pos - 1) % self.P]
         self.next_rank = self.ring[(self.pos + 1) % self.P]
         self.is_first = self.vidx[0] == 0                 # owns the stage that reads the data
         self.is_last = self.vidx[-1] == self.total - 1    # owns the stage that computes the loss
         self._comm: Optional[TorchDistComm] = None       # created on first use (p2p path only)
-        self._loss_acc: Optional[torch.Tensor] = None
-        self._advance_rng = advance_rng
-        self._pending: list = []
         self._order = looped_order(self.v, self.m)
-        for st in self.stages:
-            st.engine_managed_backward = True
-        # attributes the Runner / bench read on any engine
         self.schedule = "looped"
-        self.fused = None
-        self.in_fused = self.out_fused = False
-        self.launches_per_step = 0
-        self._graph = None
-        self._init_common()
-        self._setup_done = False
-        self.boundary = boundary
-        self._want_graph = use_cuda_graph and device.type == "cuda"
-        self.graphable = False
-        self._static_inputs: Optional[list] = None
-        self._static_labels: Optional[torch.Tensor] = None
-        self._eager_steps = 0
-        self.mb_batch = self.seq = 0
 
     # ------------------------------------------------------------------ helpers
     @property
@@ -102,35 +78,11 @@ class LoopedPipelineEngine(EngineBase):
             self._comm = TorchDistComm(self.device, group=self.group, directional=True)
         return self._comm
 
-    @staticmethod
-    def _diff_flags(tensors) -> List[bool]:
-        n = len(tensors)
-        return [torch.is_tensor(t) and t.is_floating_point() and (i < n - 1 or n == 1)
-                for i, t in enumerate(tensors)]
-
-    def _prep_inputs(self, tensors):
-        for t, d in zip(tensors, self._diff_flags(tensors)):
-            if d:
-                t.requires_grad_(True)
-        return tuple(tensors)
-
-    def _slowdown_factor(self) -> float:
-        return max(float(getattr(st, "_slowdown", 0) or 0) for st in self.stages)
-
-    def _trace_slots(self) -> int:
-        return 8 * (2 * self.v * self.m + 4) + 64
-
     # ------------------------------------------------------------------ setup (collective)
     def _setup(self, inputs) -> None:
-        self._loss_acc = torch.zeros((), dtype=torch.float32, device=self.device)
         self._configure_wgrad(True)
         want_fused = self.boundary in ("auto", "fused") and self._native_active()
-        shape = [0, 0]
-        if self.is_first:
-            shape = [inputs[0].shape[0] // self.m, int(inputs[0].shape[1]) if inputs[0].dim() > 1 else 0]
-        box = [shape]
-        dist.broadcast_object_list(box, src=self.ring[0], group=self.group)
-        self.mb_batch, self.seq = box[0]
+        self._setup_batch_shape(inputs, self.ring[0])
         ok, hidden = False, 0
         if want_fused:
             ok = True
@@ -156,11 +108,7 @@ class LoopedPipelineEngine(EngineBase):
                                               max(f[1] for f in flags), rows, self.device,
                                               group=self.group, ring=True)
             self.in_fused = self.out_fused = True
-            self.graphable = self._want_graph and bool(getattr(self.optimizer, "graph_safe", False))
-            if self.graphable:
-                for st in self.stages:
-                    st._record_forward_time = False
-                    st._logger = None
+            self._setup_graphable(True)
         if self.fused is None:
             # collective: one communicator per direction so crossed sends cannot dead-lock NCCL
             self._comm = TorchDistComm(self.device, group=self.group, directional=True)
@@ -168,31 +116,16 @@ class LoopedPipelineEngine(EngineBase):
         self._setup_grad_norm(self.pos, self.P, self.ring, [f[2] for f in flags])
         self._setup_done = True
 
-    def _fused_inputs(self, slot: int):
-        from ..ops import native as nat
-
-        ch = self.fused.prev
-        rows = self.mb_batch * self.seq
-        nat.ext().wait_flags(ch.local.mask_flag_ptr(slot), 1, ch.epoch_ptr, 1, ch.error_ptr,
-                             torch.cuda.current_stream().cuda_stream)
-        x = ch.act_view(slot, rows, ch.cols).view(self.mb_batch, self.seq, ch.cols)
-        x.requires_grad_(True)
-        mask = ch.mask_view(slot, rows).view(self.mb_batch, 1, 1, self.seq)
-        return (x, mask)
+    def _step_body(self, inputs, labels) -> None:
+        if self.fused is not None:
+            self._step_body_fused(inputs, labels)
+        else:
+            self._step_body_p2p(inputs, labels)
 
     def _step_body_fused(self, inputs, labels) -> None:
         """The same (chunk, micro-batch) order with every boundary in peer memory: no host-side
         transfers at all, the kernels of neighbouring ranks hand panels to each other."""
-        from ..models.bert_layers import advance_rng
-
-        self.fused.begin_step()
-        if self._advance_rng:
-            advance_rng()
-        self._loss_acc.zero_()
-        self._trace_tags = []
-        self._mark(("STEP", 0, "begin"))
-        chunks_in = [t.chunk(self.m, dim=0) for t in inputs] if self.is_first else None
-        label_chunks = labels.chunk(self.m, dim=0) if (self.is_last and labels is not None) else None
+        chunks_in, label_chunks = self._begin_step(inputs, labels)
         saved = {}
         for kind, c, j in self._order:
             k = self.vidx[c]
@@ -215,14 +148,7 @@ class LoopedPipelineEngine(EngineBase):
                 self._mark(("F", slot, "end"))
                 if not last_stage and first_stage:
                     self.fused.next.send_mask(outs[-1], out_slot)   # produced by the embeddings here
-                loss = None
-                if last_stage:
-                    if hasattr(self.loss_fn, "fused"):
-                        loss = (self.loss_fn.fused(outs[0], label_chunks[j], 1.0 / self.m,
-                                                   self._loss_acc.view(1)),)
-                    else:
-                        loss = self.loss_fn(outs[0], label_chunks[j]) / self.m
-                        self._loss_acc += loss.detach().float()
+                loss = self._last_stage_loss(outs[0], label_chunks[j]) if last_stage else None
                 saved[(c, j)] = (outs, loss)
             else:
                 outs, loss = saved.pop((c, j))
@@ -230,10 +156,7 @@ class LoopedPipelineEngine(EngineBase):
                 self._mark(("B", slot, "begin"))
                 st.begin_backward()
                 if last_stage:
-                    if isinstance(loss, tuple):
-                        torch.autograd.backward([outs[0]], [loss[0].to(outs[0].dtype)])
-                    else:
-                        loss.backward()
+                    self._backward_from_loss(outs, loss)
                 else:
                     torch.autograd.backward([outs[0]], [torch.zeros_like(outs[0])])
                 st.end_backward()
@@ -241,18 +164,10 @@ class LoopedPipelineEngine(EngineBase):
         self._flush_wgrads()
         self._join_wgrads()
         self.fused.end_of_backward()
-        self._mark(("OPT", 0, "begin"))
-        self.optimizer.step()
-        self._mark(("OPT", 0, "end"))
+        self._optimizer_step([])
 
-    # ------------------------------------------------------------------ one optimisation step
-    def train_step(self, inputs: Optional[Sequence[torch.Tensor]] = None,
-                   labels: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
-        if not self._setup_done:
-            self._setup(inputs)
-        self._check_batch(inputs, labels)
-        if self.fused is not None:
-            return self._train_step_fused(inputs, labels)
+    def _step_body_p2p(self, inputs, labels) -> None:
+        """The (chunk, micro-batch) order over torch.distributed p2p, one tagged FIFO per chunk."""
         if self._advance_rng and self._native_active():
             from ..models.bert_layers import advance_rng
 
@@ -280,7 +195,7 @@ class LoopedPipelineEngine(EngineBase):
                     loss = self.loss_fn(outs[0], label_chunks[j]) / self.m
                     self._loss_acc += loss.detach().float()
                 else:
-                    self._pending += self.comm.send(
+                    self._pending_sends += self.comm.send(
                         [o.detach() if torch.is_tensor(o) else None for o in outs],
                         self.next_rank, f"fwd{c}")
                 saved[(c, j)] = (args, outs, loss)
@@ -289,64 +204,25 @@ class LoopedPipelineEngine(EngineBase):
                 self._flush_wgrads()
                 st.begin_backward()
                 if last_stage:
-                    loss.backward()
+                    self._backward_from_loss(outs, loss)
                 else:
-                    metas = [(o.dtype, tuple(o.shape)) if d else None
-                             for o, d in zip(outs, self._diff_flags(outs))]
-                    grads, reqs = self.comm.recv(self.next_rank, f"bwd{c}", metas=metas)
+                    grads, reqs = self.comm.recv(self.next_rank, f"bwd{c}",
+                                                 metas=self._grad_metas(outs))
                     self.comm.wait(reqs)
-                    ts, gs = [], []
-                    for o, g in zip(outs, grads):
-                        if g is not None and torch.is_tensor(o) and o.requires_grad:
-                            ts.append(o)
-                            gs.append(g.to(o.dtype))
-                    torch.autograd.backward(ts, gs)
+                    self._backward_from_grads(outs, grads)
                 st.end_backward()
                 if not first_stage:
-                    in_grads = [(a.grad if a.grad is not None else torch.zeros_like(a)) if d else None
-                                for a, d in zip(args, self._diff_flags(args))]
-                    self._pending += self.comm.send(in_grads, self.prev_rank, f"bwd{c}",
-                                                    with_meta=False)
+                    self._pending_sends += self.comm.send(self._in_grads(args), self.prev_rank,
+                                                          f"bwd{c}", with_meta=False)
         self._flush_wgrads()
         self._join_wgrads()
+        # _optimizer_step without its OPT marks: this path records no phases on the timeline
         if self._sends_before_optimizer():
-            self.comm.wait(self._pending)
-            self._pending = []
+            self.comm.wait(self._pending_sends)
+            self._pending_sends = []
         self.optimizer.step()
-        self.comm.wait(self._pending)
-        self._pending = []
-        return self._loss_acc if self.is_last else None
-
-    def _train_step_fused(self, inputs, labels):
-        """Static buffers, 3 eager steps, then one CUDA graph per step (as in PipelineEngine)."""
-        out = self._loss_acc if self.is_last else None
-        if not self.graphable:
-            self._step_body_fused(inputs, labels)
-            return out
-        if self._static_inputs is None:
-            self._static_inputs = [t.clone() for t in inputs] if self.is_first else []
-            self._static_labels = labels.clone() if (self.is_last and labels is not None) else None
-        if self.is_first:
-            for s_, t in zip(self._static_inputs, inputs):
-                s_.copy_(t, non_blocking=True)
-        if self._static_labels is not None and labels is not None:
-            self._static_labels.copy_(labels, non_blocking=True)
-        if self._graph is None and self._eager_steps < 3:
-            self._step_body_fused(self._static_inputs, self._static_labels)
-            self._eager_steps += 1
-            return out
-        if self._graph is None:
-            from ..ops import native as nat
-
-            torch.cuda.synchronize(self.device)
-            g = torch.cuda.CUDAGraph()
-            before = nat.launch_count()
-            with torch.cuda.graph(g):
-                self._step_body_fused(self._static_inputs, self._static_labels)
-            self.launches_per_step = nat.launch_count() - before
-            self._graph = g
-        self._graph.replay()
-        return out
+        self.comm.wait(self._pending_sends)
+        self._pending_sends = []
 
     # ------------------------------------------------------------------ plain forward (eval)
     @torch.no_grad()
@@ -379,33 +255,3 @@ class LoopedPipelineEngine(EngineBase):
         if not results:
             return None
         return results[0] if m == 1 else results
-
-    def eval_step(self, inputs: Optional[Sequence[torch.Tensor]], labels: Optional[torch.Tensor],
-                  accum, micro_batches: Optional[int] = None) -> None:
-        """``forward_only`` + ``accum.add(logits, labels)`` per micro-batch on the last stage."""
-        m = int(micro_batches or self.m)
-        if self.is_first and inputs[0].shape[0] % m:
-            raise ValueError("an evaluation batch of {} samples cannot be split into {} equal "
-                             "micro-batches".format(inputs[0].shape[0], m))
-        with contextlib.ExitStack() as stack:
-            for st in self.stages:
-                stack.enter_context(st.suspend_forward_probes())
-            res = self.forward_only(inputs, micro_batches=m)
-        if self.is_last:
-            res = [res] if m == 1 else res
-            for outs, lab in zip(res, labels.chunk(m, dim=0)):
-                accum.add(outs[0], lab)
-
-    def close(self) -> None:
-        if self.device.type == "cuda":
-            torch.cuda.synchronize(self.device)
-        self._close_grad_norm()
-        if self.fused is not None:
-            self.fused.close()
-            self.fused = None
-        self._release_wgrad_switches()
-
-    @staticmethod
-    def barrier(group=None) -> None:
-        if dist.is_available() and dist.is_initialized():
-            dist.barrier(group=group)
