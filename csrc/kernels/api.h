@@ -146,9 +146,6 @@ struct AttnArgs {
 };
 int launch_attention_fwd(const AttnArgs& a, cudaStream_t stream);
 int launch_attention_bwd(const AttnArgs& a, cudaStream_t stream);
-// any S with S % 8 == 0 (flash-style tiling over 128-key blocks; backward = dQ kernel + dK/dV kernel)
-int launch_attention_fwd_tiled(const AttnArgs& a, cudaStream_t stream);
-int launch_attention_bwd_tiled(const AttnArgs& a, cudaStream_t stream);
 bool attention_supported(int S, int head_dim);
 
 // ---------------------------------------------------------------------------------------------

@@ -287,12 +287,15 @@ __device__ __forceinline__ void wgmma_k16(float (&d)[N / 2], uint64_t desc_a, ui
   if constexpr (N == 128) wgmma_m64n128k16<TA, TB>(d, desc_a, desc_b, scale_d);
   if constexpr (N == 256) wgmma_m64n256k16<TA, TB>(d, desc_a, desc_b, scale_d);
 }
+// Accumulator fragment of one warpgroup thread: warp w of the group owns rows 16w .. 16w+15; lane l
+// holds, for every 8-column block j, d[4j], d[4j+1] = (row 16w + l/4, columns 8j + 2(l%4) + {0,1})
+// and d[4j+2], d[4j+3] = the same columns of row + 8.
 
 // Register-A wgmma: D[64 x N] (+)= A[64 x 16] (registers) * B (shared memory).  Only B takes a
 // transpose bit in this form (TB = 1: B is MN-major).  A thread's A fragment is four bf16x2 words:
 //   a[0] = (row fr, k 2(l%4) + {0,1}),     a[1] = (row fr + 8, the same k),
 //   a[2] = (row fr, k 8 + 2(l%4) + {0,1}), a[3] = (row fr + 8, the same k),
-// with fr = 16 (warp % 4) + l / 4.  That is the accumulator layout of acc_store_smem restricted to
+// with fr = 16 (warp % 4) + l / 4.  That is the accumulator fragment layout above restricted to
 // 16 columns, so the accumulator d of columns 16k .. 16k + 15 IS the A fragment of K step k:
 //   a[0] = pack(d[8k], d[8k+1]), a[1] = pack(d[8k+2], d[8k+3]),
 //   a[2] = pack(d[8k+4], d[8k+5]), a[3] = pack(d[8k+6], d[8k+7])
@@ -358,44 +361,6 @@ __device__ __forceinline__ void wgmma_rs_k16(float (&d)[N / 2], const uint32_t (
   static_assert(N == 64 || N == 128, "unsupported register-A wgmma width");
   if constexpr (N == 64) wgmma_m64n64k16_rs<TB>(d, a, desc_b, scale_d);
   if constexpr (N == 128) wgmma_m64n128k16_rs<TB>(d, a, desc_b, scale_d);
-}
-// Accumulator fragment of one warpgroup thread: warp w of the group owns rows 16w .. 16w+15; lane l
-// holds, for every 8-column block j, d[4j], d[4j+1] = (row 16w + l/4, columns 8j + 2(l%4) + {0,1})
-// and d[4j+2], d[4j+3] = the same columns of row + 8.  Stores columns [C0, C0 + NC) of the
-// fragment (C0 must be a constant after unrolling: the fragment lives in registers) into an fp32 tile `dst` (leading dimension `ld` floats) at rows row0 + (0..63), tile
-// columns col0 + (0..NC), so that other threads can walk whole rows.
-template <int NC, int NREG>
-__device__ __forceinline__ void acc_store_smem(const float (&d)[NREG], int C0, float* dst, int ld,
-                                               int row0, int col0, int wg_tid) {
-  const int r = row0 + (wg_tid >> 5) * 16 + ((wg_tid & 31) >> 2);
-  float* p0 = dst + r * ld + col0 + (wg_tid & 3) * 2;
-#pragma unroll
-  for (int j = 0; j < NC / 8; ++j) {
-    *reinterpret_cast<float2*>(p0 + j * 8) = make_float2(d[(C0 / 8 + j) * 4], d[(C0 / 8 + j) * 4 + 1]);
-    *reinterpret_cast<float2*>(p0 + 8 * ld + j * 8) =
-        make_float2(d[(C0 / 8 + j) * 4 + 2], d[(C0 / 8 + j) * 4 + 3]);
-  }
-}
-// 32 consecutive floats of one staged row -> registers
-__device__ __forceinline__ void row_load32(const float* src, uint32_t (&v)[32]) {
-#pragma unroll
-  for (int j = 0; j < 32; j += 4) {
-    const uint4 x = *reinterpret_cast<const uint4*>(src + j);
-    v[j] = x.x;
-    v[j + 1] = x.y;
-    v[j + 2] = x.z;
-    v[j + 3] = x.w;
-  }
-}
-__device__ __forceinline__ void row_load16(const float* src, uint32_t (&v)[16]) {
-#pragma unroll
-  for (int j = 0; j < 16; j += 4) {
-    const uint4 x = *reinterpret_cast<const uint4*>(src + j);
-    v[j] = x.x;
-    v[j + 1] = x.y;
-    v[j + 2] = x.z;
-    v[j + 3] = x.w;
-  }
 }
 // TMA load delivered to every CTA of `mask` at the same CTA-relative offsets (data and barrier)
 __device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar,
@@ -524,7 +489,7 @@ __device__ __forceinline__ uint32_t dropout_keep4(uint64_t seed, uint64_t idx4, 
 // ----------------------------------------------------------------------------------------------
 // A thread holds, of each 64-column group of its warpgroup's 64 x N accumulator, f[4j], f[4j+1] =
 // (row fr, columns 8j + fc + {0,1}) and f[4j+2], f[4j+3] = (row fr + 8, the same columns), j =
-// 0..7, with fr = lane / 4 and fc = 2 (lane % 4) (see acc_store_smem).
+// 0..7, with fr = lane / 4 and fc = 2 (lane % 4) (see the accumulator fragment layout above).
 //
 // Per-warp bf16 staging buffer: the warp's 16 fragment rows x 64 columns, rows 144 B apart (128 B +
 // 16 B pad).  With that stride both the fragment side (4-byte column pairs, 8 rows x 4 lanes) and
@@ -578,14 +543,15 @@ __device__ __forceinline__ uint32_t frag_keep_bits(uint64_t seed, uint32_t thr16
   const uint32_t mb = (odd ? h : o) >> sh;
   return (ma & 3u) | ((mb & 3u) << 2);
 }
-// dropout on a 64-column fragment group: kept elements are multiplied by `scale`, dropped ones
-// become 0
-__device__ __forceinline__ void frag_dropout(float (&f)[32], uint64_t seed, uint32_t thr16,
+// dropout on the 64-column fragment groups of f (columns col0, col0 + 64, ...): kept elements are
+// multiplied by `scale`, dropped ones become 0
+template <int NREG>
+__device__ __forceinline__ void frag_dropout(float (&f)[NREG], uint64_t seed, uint32_t thr16,
                                              float scale, long long row_a, int col0, int n,
                                              int lane) {
 #pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const uint32_t m = frag_keep_bits(seed, thr16, row_a, col0, n, lane, j);
+  for (int j = 0; j < NREG / 4; ++j) {
+    const uint32_t m = frag_keep_bits(seed, thr16, row_a, col0 + (j >> 3) * 64, n, lane, j & 7);
     f[4 * j] = (m & 1u) ? f[4 * j] * scale : 0.f;
     f[4 * j + 1] = (m & 2u) ? f[4 * j + 1] * scale : 0.f;
     f[4 * j + 2] = (m & 4u) ? f[4 * j + 2] * scale : 0.f;
@@ -602,25 +568,6 @@ __device__ __forceinline__ void frag_to_a(const float (&d)[NREG], int k, uint32_
   a[3] = pack_bf16x2(d[8 * k + 6], d[8 * k + 7]);
 }
 
-// One warpgroup (128 threads): dst[128 x N] (fp32 tile in shared memory, leading dimension `ld`
-// floats) = A[128 x 16 KSTEPS] * B[N x 16 KSTEPS]^T as two 64-row wgmma halves.  a_desc(k, mh) /
-// b_desc(k) give the operand descriptors of K step k (and 64-row half mh of A).  The caller
-// synchronises the CTA before other threads read `dst`.
-template <int N, int TA, int TB, int KSTEPS, class FA, class FB>
-__device__ __forceinline__ void wg_mma_to_smem(float* dst, int ld, FA a_desc, FB b_desc, int tid) {
-#pragma unroll
-  for (int mh = 0; mh < 2; ++mh) {
-    float d[N / 2];
-#pragma unroll
-    for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < KSTEPS; ++k) wgmma_k16<N, TA, TB>(d, a_desc(k, mh), b_desc(k), 1u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    acc_store_smem<N>(d, 0, dst, ld, mh * 64, 0, tid);
-  }
-}
 // descriptor of K step k of a K-major [rows x 64 * nblk] bf16 operand kept as 64-wide K blocks
 // `blk_bytes` apart (row offset row0, a multiple of 8) / of an MN-major operand
 __device__ __forceinline__ uint64_t desc_kmajor(uint32_t base, int k, uint32_t blk_bytes, int row0) {

@@ -31,7 +31,6 @@ CUDA_SOURCES = [
     "kernels/gemm_sm100.cu",
     "kernels/elementwise_sm100.cu",
     "kernels/attention_sm100.cu",
-    "kernels/attention_tiled_sm100.cu",
     "bench/device_bench.cu",
 ]
 CUDA_BINDINGS = "bindings_cuda.cpp"

@@ -423,11 +423,12 @@ def test_attention_tiled_any_sequence_length(nat, S):
     _close(dqkv[:, 2 * H:], qf.grad[:, 2 * H:], rtol=3e-2, atol=3e-2)   # dV
 
 
-@pytest.mark.parametrize("S", [128, 256])
+@pytest.mark.parametrize("S", [128, 256, 72])
 def test_attention_dropout_exact_mask_parity(nat, S):
     """Dropout on the probabilities: the host replica of the device RNG gives the exact keep mask
     of the [B, heads, S, S] site; forward and gradients must match the fp32 reference that applies
-    that mask (S = 128: single-tile kernels, S = 256: tiled kernels - same element indexing)."""
+    that mask (S = 128: single-tile kernels, S = 256: tiled kernels - same element indexing,
+    S = 72: a ragged tile whose fragment rows past the end still take part in the mask shuffles)."""
     from skycomputing_b200.ops.dropout_ref import keep_mask_from_state
 
     torch.manual_seed(31)

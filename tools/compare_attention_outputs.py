@@ -1,12 +1,13 @@
-"""Comparison of the S = 128 attention kernels' outputs between two builds of the project.
+"""Comparison of the attention kernels' outputs between two builds of the project.
 
-    python tools/compare_attention_outputs.py dump --root TREE --out DIR
+    python tools/compare_attention_outputs.py dump --root TREE --out DIR [--seq S]
     python tools/compare_attention_outputs.py compare DIR_A DIR_B
 
 ``dump`` imports the package from TREE (a source tree with a built extension) and runs the
 attention forward and backward at the BERT-large training step's configuration (B = 32, 16 heads,
-S = 128, head size 64, additive padding mask) on seeded inputs, without dropout and with dropout
-0.1 from an ``RngState``.  It stores the raw bits of ``ctx``, ``lse`` and ``dqkv`` as
+head size 64, additive padding mask) on seeded inputs, without dropout and with dropout 0.1 from an
+``RngState``.  The sequence length is ``--seq`` (default 128, the single-tile kernels; any other
+length runs the tiled kernels).  It stores the raw bits of ``ctx``, ``lse`` and ``dqkv`` as
 DIR/<name>.npy.  ``compare`` reports, per output, whether the bits agree, the largest absolute
 difference, the largest difference in bf16 ulps of the value and relative to the output's largest
 magnitude (bf16 outputs) or relative to the value (fp32 ``lse``).  ``dqkv_torchfwd_*`` runs the
@@ -19,10 +20,10 @@ import argparse
 import os
 import sys
 
-B, S, HEADS, D = 32, 128, 16, 64
+B, HEADS, D = 32, 16, 64
 
 
-def _torch_forward(torch, qkv, mask, ctx_like):
+def _torch_forward(torch, qkv, mask, ctx_like, S):
     """lse (log2 domain) from torch in fp32, and a seeded random bf16 ctx (the backward reads ctx
     only for delta = rowsum(dO * O)); neither depends on the build."""
     import math
@@ -35,7 +36,7 @@ def _torch_forward(torch, qkv, mask, ctx_like):
     return ctx, lse
 
 
-def dump(root: str, out_dir: str) -> None:
+def dump(root: str, out_dir: str, S: int) -> None:
     sys.path.insert(0, os.path.abspath(root))
     import numpy as np
     import torch
@@ -58,7 +59,7 @@ def dump(root: str, out_dir: str) -> None:
         outs[f"lse_{tag}"] = lse
         outs[f"dqkv_{tag}"] = nat.attention_bwd(qkv, mask, ctx, lse, dctx, B, S, HEADS, **kw)
         # the backward alone, on a forward (ctx, lse) computed by torch, the same in every build
-        ctx_t, lse_t = _torch_forward(torch, qkv, mask, ctx)
+        ctx_t, lse_t = _torch_forward(torch, qkv, mask, ctx, S)
         outs[f"dqkv_torchfwd_{tag}"] = nat.attention_bwd(qkv, mask, ctx_t, lse_t, dctx, B, S,
                                                          HEADS, **kw)
     torch.cuda.synchronize()
@@ -106,12 +107,13 @@ def main() -> int:
     d = sub.add_parser("dump")
     d.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
     d.add_argument("--out", required=True)
+    d.add_argument("--seq", type=int, default=128)
     c = sub.add_parser("compare")
     c.add_argument("a")
     c.add_argument("b")
     args = ap.parse_args()
     if args.cmd == "dump":
-        dump(args.root, args.out)
+        dump(args.root, args.out, args.seq)
         return 0
     return compare(args.a, args.b)
 
