@@ -58,7 +58,10 @@ struct GemmArgs {
   int block_n = 0;            // 0 = auto (128 or 256)
   int stream_k = -1;          // stream-K schedule: -1 auto, 0 off, 1 on
   int pair = -1;              // -1 auto, 0 single CTAs, 1 = 2-CTA clusters (B multicast), 2 = 4-CTA clusters (A and B multicast)
-  int debug = 0;              // perf triage: 1 = epilogue discards the tile, 2 = epilogue math but no stores
+  // perf triage: 1 = full main loop, the epilogue discards the tile; 2 = epilogue math but no
+  // stores; 3 = MMAs only (no TMA loads: the MMAs read stale shared memory), no epilogue; 4 = TMA
+  // loads only (no MMAs), no epilogue.  With clusters (pair != 0), 3 and 4 only drop the epilogue.
+  int debug = 0;
   int max_ctas = 0;           // 0 = all SMs
 };
 
@@ -71,8 +74,6 @@ int gemm_ln_block_n(int M, int N, bool force = false);
 int gemm_ln_tiles_per_panel(int M, int N, bool force = false);
 int gemm_tiles_per_panel(int N, int block_n);  // number of signals per 128-row panel
 int gemm_pick_block_n(int M, int N);
-bool gemm_pick_pair(int M, int N, int K);
-bool gemm_pick_quad(int M, int N, int K);
 
 // ---------------------------------------------------------------------------------------------
 // LayerNorm (rows of H), bf16 in/out, fp32 statistics

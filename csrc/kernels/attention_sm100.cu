@@ -105,22 +105,6 @@ __device__ __forceinline__ Frag frag_of_thread() {
   return f;
 }
 
-struct Dropout {
-  bool on;
-  uint64_t seed;
-  uint32_t thr16;
-  float scale;  // 1 / (1 - p) for kept elements
-};
-__device__ __forceinline__ Dropout dropout_of(const AttnDev& p) {
-  Dropout d{p.dropout_p > 0.f, 0, 0, 1.f};
-  if (d.on) {
-    d.seed = dropout_seed(p.rng_state, p.rng_stream);
-    d.thr16 = static_cast<uint32_t>(p.dropout_p * 65536.f);
-    d.scale = 1.f / (1.f - p.dropout_p);
-  }
-  return d;
-}
-
 // additive mask (log2 domain) of keys key0 .. key0 + 127 -> sMask; keys past the end get -1e30
 __device__ __forceinline__ void load_mask(float* sMask, const AttnDev& p, int b, int S, int key0,
                                           int tid) {
@@ -378,7 +362,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnDev
   exp_rows(s, mx0, mx1, sum0, sum1);
   // the row sum is taken before dropout: it normalises the un-dropped probabilities
   quad_sum(sum0, sum1);
-  const Dropout dr = dropout_of(p);
+  const Dropout dr = dropout_of(p.dropout_p, p.rng_state, p.rng_stream);
   if (dr.on) frag_dropout(s, dr.seed, dr.thr16, 1.f, static_cast<long long>(bh) * kT + f.q0, 0, kT,
                           f.lane);
   if (p.lse != nullptr && (f.lane & 3) == 0) {
@@ -445,7 +429,7 @@ attention_fwd_tiled_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const A
   }
 
   const float sc = p.scale * kLog2e;
-  const Dropout dr = dropout_of(p);
+  const Dropout dr = dropout_of(p.dropout_p, p.rng_state, p.rng_stream);
   const long long row_a = static_cast<long long>(bh) * p.S + qt * kT + f.q0;
   float o[32];
 #pragma unroll
@@ -595,7 +579,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
   const uint32_t aQ = smem_u32(m.sQ), aK = smem_u32(m.sK), aV = smem_u32(m.sV);
   const uint32_t adO = smem_u32(m.sdO), aP = smem_u32(m.sP), adS = smem_u32(m.sdS);
   const float sc = p.scale * kLog2e;
-  const Dropout dr = dropout_of(p);
+  const Dropout dr = dropout_of(p.dropout_p, p.rng_state, p.rng_stream);
   const long long row_a = static_cast<long long>(bh) * kT + f.q0;
 #pragma unroll 1
   for (int kh = 0; kh < 2; ++kh)
@@ -656,7 +640,7 @@ attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
   __syncthreads();
   const BwdRows r{m.sLse[f.q0], m.sLse[f.q0 + 8], m.sDelta[f.q0], m.sDelta[f.q0 + 8]};
   const float sc = p.scale * kLog2e;
-  const Dropout dr = dropout_of(p);
+  const Dropout dr = dropout_of(p.dropout_p, p.rng_state, p.rng_stream);
   const long long row_a = static_cast<long long>(bh) * p.S + qt * kT + f.q0;
   const uint32_t aQ = smem_u32(m.sQ), aK = smem_u32(m.sK), aV = smem_u32(m.sV);
   const uint32_t adO = smem_u32(m.sdO), adS = smem_u32(m.sdS);
@@ -715,7 +699,7 @@ attention_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
     tma_load_3d(m.sV, &tmap_qkv, bar_kv, 2 * p.H + h * kD, kt * kT, b);
   }
   const float sc = p.scale * kLog2e;
-  const Dropout dr = dropout_of(p);
+  const Dropout dr = dropout_of(p.dropout_p, p.rng_state, p.rng_stream);
   const uint32_t aQ = smem_u32(m.sQ), aK = smem_u32(m.sK), aV = smem_u32(m.sV);
   const uint32_t adO = smem_u32(m.sdO), aP = smem_u32(m.sP), adS = smem_u32(m.sdS);
   float dv[32], dk[32];  // keys 64 wg .. 64 wg + 63 of the tile

@@ -162,15 +162,9 @@ layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* 
   const float inv_h = 1.f / static_cast<float>(H);
   const uint32_t target = wait_flags ? (*wait_epoch) * wait_mult : 0u;
   int last_panel = -1;
-  const bool has_dropout = dropout_p > 0.f && dz_dropped != nullptr;
-  uint64_t seed = 0;
-  uint32_t thr16 = 0;
-  float drop_scale = 1.f;
-  if (has_dropout) {
-    seed = dropout_seed(rng_state, rng_stream);
-    thr16 = static_cast<uint32_t>(dropout_p * 65536.f);
-    drop_scale = 1.f / (1.f - dropout_p);
-  }
+  // the masked copy is written only when dz_dropped is given
+  const Dropout drop =
+      dropout_of(dz_dropped != nullptr ? dropout_p : 0.f, rng_state, rng_stream);
 
   for (int row = warp_global; row < M; row += total_warps) {
     if (wait_flags != nullptr) {
@@ -215,7 +209,7 @@ layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* 
     const float c1 = warp_sum(s1) * inv_h;
     const float c2 = warp_sum(s2) * inv_h;
     uint4* dzr = reinterpret_cast<uint4*>(dz + static_cast<long long>(row) * H);
-    uint4* dzd = has_dropout
+    uint4* dzd = drop.on
                      ? reinterpret_cast<uint4*>(dz_dropped + static_cast<long long>(row) * H)
                      : nullptr;
 #pragma unroll
@@ -227,14 +221,14 @@ layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* 
         for (int t = 0; t < 8; ++t) o[t] = (g[i][t] - c1 - xh[i][t] * c2) * rs;
         dzr[v] = make_uint4(pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], o[3]),
                             pack_bf16x2(o[4], o[5]), pack_bf16x2(o[6], o[7]));
-        if (has_dropout) {
+        if (drop.on) {
           const uint64_t base = (static_cast<uint64_t>(row) * H + v * 8) >> 2;
-          const uint32_t m0 = dropout_keep4(seed, base, thr16);
-          const uint32_t m1 = dropout_keep4(seed, base + 1, thr16);
+          const uint32_t m0 = dropout_keep4(drop.seed, base, drop.thr16);
+          const uint32_t m1 = dropout_keep4(drop.seed, base + 1, drop.thr16);
 #pragma unroll
           for (int t = 0; t < 4; ++t) {
-            o[t] = (m0 >> t) & 1u ? o[t] * drop_scale : 0.f;
-            o[4 + t] = (m1 >> t) & 1u ? o[4 + t] * drop_scale : 0.f;
+            o[t] = (m0 >> t) & 1u ? o[t] * drop.scale : 0.f;
+            o[4 + t] = (m1 >> t) & 1u ? o[4 + t] * drop.scale : 0.f;
           }
           dzd[v] = make_uint4(pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], o[3]),
                               pack_bf16x2(o[4], o[5]), pack_bf16x2(o[6], o[7]));
@@ -366,15 +360,7 @@ embed_fwd_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ tt
   const int row0 = blockIdx.x * warps_per_block + (threadIdx.x >> 5);
   const int total_warps = gridDim.x * warps_per_block;
   const float inv_h = 1.f / static_cast<float>(H);
-  const bool has_dropout = dropout_p > 0.f;
-  uint64_t seed = 0;
-  uint32_t thr16 = 0;
-  float drop_scale = 1.f;
-  if (has_dropout) {
-    seed = dropout_seed(rng_state, rng_stream);
-    thr16 = static_cast<uint32_t>(dropout_p * 65536.f);
-    drop_scale = 1.f / (1.f - dropout_p);
-  }
+  const Dropout drop = dropout_of(dropout_p, rng_state, rng_stream);
   for (int row = row0; row < BS; row += total_warps) {
     const long long id = ids[row];
     const long long tt = tts[row];
@@ -417,12 +403,13 @@ embed_fwd_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ tt
       float o1 = (a.y + b.y + d.y - mu) * rs * g.y + be.y;
       float o2 = (a.z + b.z + d.z - mu) * rs * g.z + be.z;
       float o3 = (a.w + b.w + d.w - mu) * rs * g.w + be.w;
-      if (has_dropout) {
-        const uint32_t m = dropout_keep4(seed, (static_cast<uint64_t>(row) * H + c) >> 2, thr16);
-        o0 = (m & 1u) ? o0 * drop_scale : 0.f;
-        o1 = (m & 2u) ? o1 * drop_scale : 0.f;
-        o2 = (m & 4u) ? o2 * drop_scale : 0.f;
-        o3 = (m & 8u) ? o3 * drop_scale : 0.f;
+      if (drop.on) {
+        const uint32_t m =
+            dropout_keep4(drop.seed, (static_cast<uint64_t>(row) * H + c) >> 2, drop.thr16);
+        o0 = (m & 1u) ? o0 * drop.scale : 0.f;
+        o1 = (m & 2u) ? o1 * drop.scale : 0.f;
+        o2 = (m & 4u) ? o2 * drop.scale : 0.f;
+        o3 = (m & 8u) ? o3 * drop.scale : 0.f;
       }
       uint2 pk;
       pk.x = pack_bf16x2(o0, o1);
@@ -458,15 +445,7 @@ embed_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const int64_t* __restri
   const int row0 = blockIdx.x * warps_per_block + (threadIdx.x >> 5);
   const int total_warps = gridDim.x * warps_per_block;
   const float inv_h = 1.f / static_cast<float>(H);
-  const bool has_dropout = dropout_p > 0.f;
-  uint64_t seed = 0;
-  uint32_t thr16 = 0;
-  float drop_scale = 1.f;
-  if (has_dropout) {
-    seed = dropout_seed(rng_state, rng_stream);
-    thr16 = static_cast<uint32_t>(dropout_p * 65536.f);
-    drop_scale = 1.f / (1.f - dropout_p);
-  }
+  const Dropout drop = dropout_of(dropout_p, rng_state, rng_stream);
   const uint32_t target = wait_flags ? (*wait_epoch) * wait_mult : 0u;
   int last_panel = -1;
   for (int row = row0; row < BS; row += total_warps) {
@@ -491,10 +470,11 @@ embed_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const int64_t* __restri
       const uint2 u = *reinterpret_cast<const uint2*>(drow + c);
       float2 d01 = unpack_bf16x2(u.x), d23 = unpack_bf16x2(u.y);
       float dy[4] = {d01.x, d01.y, d23.x, d23.y};
-      if (has_dropout) {
-        const uint32_t m = dropout_keep4(seed, (static_cast<uint64_t>(row) * H + c) >> 2, thr16);
+      if (drop.on) {
+        const uint32_t m =
+            dropout_keep4(drop.seed, (static_cast<uint64_t>(row) * H + c) >> 2, drop.thr16);
 #pragma unroll
-        for (int t = 0; t < 4; ++t) dy[t] = (m >> t) & 1u ? dy[t] * drop_scale : 0.f;
+        for (int t = 0; t < 4; ++t) dy[t] = (m >> t) & 1u ? dy[t] * drop.scale : 0.f;
       }
       const float4 a = *reinterpret_cast<const float4*>(wr + c);
       const float4 b = *reinterpret_cast<const float4*>(pr + c);
@@ -518,10 +498,11 @@ embed_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const int64_t* __restri
       const uint2 u = *reinterpret_cast<const uint2*>(drow + c);
       float2 d01 = unpack_bf16x2(u.x), d23 = unpack_bf16x2(u.y);
       float dy[4] = {d01.x, d01.y, d23.x, d23.y};
-      if (has_dropout) {
-        const uint32_t m = dropout_keep4(seed, (static_cast<uint64_t>(row) * H + c) >> 2, thr16);
+      if (drop.on) {
+        const uint32_t m =
+            dropout_keep4(drop.seed, (static_cast<uint64_t>(row) * H + c) >> 2, drop.thr16);
 #pragma unroll
-        for (int t = 0; t < 4; ++t) dy[t] = (m >> t) & 1u ? dy[t] * drop_scale : 0.f;
+        for (int t = 0; t < 4; ++t) dy[t] = (m >> t) & 1u ? dy[t] * drop.scale : 0.f;
       }
       const float4 a = *reinterpret_cast<const float4*>(wr + c);
       const float4 b = *reinterpret_cast<const float4*>(pr + c);
@@ -574,20 +555,13 @@ small_linear_fwd_kernel(const void* __restrict__ x, bool x_bf16, long long ldx,
   const long long o = static_cast<long long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (o >= static_cast<long long>(M) * N) return;
   const int m = static_cast<int>(o / N), n = static_cast<int>(o % N);
-  const bool has_dropout = dropout_p > 0.f;
-  uint64_t seed = 0;
-  uint32_t thr16 = 0;
-  float scale = 1.f;
-  if (has_dropout) {
-    seed = dropout_seed(rng_state, rng_stream);
-    thr16 = static_cast<uint32_t>(dropout_p * 65536.f);
-    scale = 1.f / (1.f - dropout_p);
-  }
+  const Dropout drop = dropout_of(dropout_p, rng_state, rng_stream);
   const float* wr = w + static_cast<long long>(n) * K;
   float acc = 0.f;
   for (int k = lane; k < K; k += 32) {
     float xv = load_x(x, x_bf16, m * ldx + k);
-    if (has_dropout) xv = drop1(seed, static_cast<uint64_t>(m) * K + k, thr16, scale, xv);
+    if (drop.on)
+      xv = drop1(drop.seed, static_cast<uint64_t>(m) * K + k, drop.thr16, drop.scale, xv);
     acc += xv * wr[k];
   }
   acc = warp_sum(acc);
@@ -607,15 +581,7 @@ small_linear_dx_kernel(const float* __restrict__ w, const float* __restrict__ y,
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   const int m0 = blockIdx.y * 8;
   if (k >= K) return;
-  const bool has_dropout = dropout_p > 0.f;
-  uint64_t seed = 0;
-  uint32_t thr16 = 0;
-  float scale = 1.f;
-  if (has_dropout) {
-    seed = dropout_seed(rng_state, rng_stream);
-    thr16 = static_cast<uint32_t>(dropout_p * 65536.f);
-    scale = 1.f / (1.f - dropout_p);
-  }
+  const Dropout drop = dropout_of(dropout_p, rng_state, rng_stream);
   float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   for (int n = 0; n < N; ++n) {
     const float wv = w[static_cast<long long>(n) * K + k];
@@ -637,7 +603,8 @@ small_linear_dx_kernel(const float* __restrict__ w, const float* __restrict__ y,
     const int m = m0 + i;
     if (m < M) {
       float v = acc[i];
-      if (has_dropout) v = drop1(seed, static_cast<uint64_t>(m) * K + k, thr16, scale, v);
+      if (drop.on)
+        v = drop1(drop.seed, static_cast<uint64_t>(m) * K + k, drop.thr16, drop.scale, v);
       if (dx_bf16)
         reinterpret_cast<__nv_bfloat16*>(dx)[m * lddx + k] = __float2bfloat16(v);
       else
@@ -655,15 +622,7 @@ small_linear_dw_kernel(const void* __restrict__ x, bool x_bf16, long long ldx,
                        uint32_t rng_stream) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   const int n = blockIdx.y;
-  const bool has_dropout = dropout_p > 0.f;
-  uint64_t seed = 0;
-  uint32_t thr16 = 0;
-  float scale = 1.f;
-  if (has_dropout) {
-    seed = dropout_seed(rng_state, rng_stream);
-    thr16 = static_cast<uint32_t>(dropout_p * 65536.f);
-    scale = 1.f / (1.f - dropout_p);
-  }
+  const Dropout drop = dropout_of(dropout_p, rng_state, rng_stream);
   float acc = 0.f, accb = 0.f;
   for (int m = 0; m < M; ++m) {
     float g = dy[static_cast<long long>(m) * N + n];
@@ -674,7 +633,8 @@ small_linear_dw_kernel(const void* __restrict__ x, bool x_bf16, long long ldx,
     accb += g;
     if (k < K) {
       float xv = load_x(x, x_bf16, m * ldx + k);
-      if (has_dropout) xv = drop1(seed, static_cast<uint64_t>(m) * K + k, thr16, scale, xv);
+      if (drop.on)
+        xv = drop1(drop.seed, static_cast<uint64_t>(m) * K + k, drop.thr16, drop.scale, xv);
       acc += g * xv;
     }
   }

@@ -88,33 +88,59 @@ __device__ __forceinline__ void aux_load(uint4 (&ax)[4], const __nv_bfloat16* au
                 : make_uint4(0, 0, 0, 0);
   }
 }
-// ... -> staging -> fragment pairs: a[2j] = row fr, a[2j+1] = row fr + 8 (bf16x2 each)
-__device__ __forceinline__ void aux_to_frag(const uint4 (&ax)[4], uint8_t* s, int lane,
-                                            uint32_t (&a)[16]) {
+// the block of aux_load -> staging -> fragment pairs (a[2j] = row fr, a[2j+1] = row fr + 8, bf16x2
+// each), then f *= gelu'(aux) (mul_dgelu) or f += aux (add)
+__device__ __forceinline__ void frag_apply_aux(float (&f)[32], const uint4 (&ax)[4], uint8_t* s,
+                                               int lane, bool mul_dgelu, bool add) {
   const int piece = lane & 7;
 #pragma unroll
   for (int i = 0; i < 4; ++i)
     *reinterpret_cast<uint4*>(s + (i * 4 + (lane >> 3)) * kStageLd + piece * 16) = ax[i];
   __syncwarp();
   const uint8_t* mine = s + (lane >> 2) * kStageLd + (lane & 3) * 4;
+  uint32_t a[16];
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     a[2 * j] = *reinterpret_cast<const uint32_t*>(mine + j * 16);
     a[2 * j + 1] = *reinterpret_cast<const uint32_t*>(mine + 8 * kStageLd + j * 16);
   }
   __syncwarp();
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float2 xa = unpack_bf16x2(a[2 * j]);
+    const float2 xb = unpack_bf16x2(a[2 * j + 1]);
+    if (mul_dgelu) {
+      f[4 * j] *= dgelu_fast(xa.x);
+      f[4 * j + 1] *= dgelu_fast(xa.y);
+      f[4 * j + 2] *= dgelu_fast(xb.x);
+      f[4 * j + 3] *= dgelu_fast(xb.y);
+    } else if (add) {
+      f[4 * j] += xa.x;
+      f[4 * j + 1] += xa.y;
+      f[4 * j + 2] += xb.x;
+      f[4 * j + 3] += xb.y;
+    }
+  }
+}
+// f += the bias of the group's 64 columns ct .. ct + 63 of the tile (staged in shared memory at sb)
+__device__ __forceinline__ void frag_add_bias(float (&f)[32], const float* sb, int ct, int fc) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float2 bb = *reinterpret_cast<const float2*>(sb + ct + j * 8 + fc);  // broadcast
+    f[4 * j] = f[4 * j] + bb.x;
+    f[4 * j + 1] = f[4 * j + 1] + bb.y;
+    f[4 * j + 2] = f[4 * j + 2] + bb.x;
+    f[4 * j + 3] = f[4 * j + 3] + bb.y;
+  }
 }
 
-struct GemmDev {
+// Parameters both kernels read: the shape, the epilogue inputs they share, dropout and the
+// stage-boundary flags (see GemmArgs in api.h).
+struct GemmCommon {
   int M, N, K;
-  void* out;
-  void* out2;
   const float* bias;
   const __nv_bfloat16* aux;
-  long long ldo, ldo2, ldaux;
-  int act;
-  int add_aux;
-  int accumulate;
+  long long ldaux;
   float dropout_p;
   const uint64_t* rng_state;
   uint32_t rng_stream;
@@ -123,6 +149,15 @@ struct GemmDev {
   const uint32_t* wait_epoch;
   uint32_t wait_mult;
   int* error_flag;
+};
+
+struct GemmDev : GemmCommon {
+  void* out;
+  void* out2;
+  long long ldo, ldo2;
+  int act;
+  int add_aux;
+  int accumulate;
   int debug;
   // stream-K: the flattened (tile, k-block) space is cut into one contiguous range per CTA (cluster);
   // tiles shared by several CTAs are reduced through `ws` by whichever CTA arrives last
@@ -181,6 +216,136 @@ struct Sched {
   __device__ __forceinline__ int first_tile(int u) const { return static_cast<int>(bound(u) / nk); }
 };
 
+// A position in the operand ring: the stage and the parity of its current fill.
+template <int kStages>
+struct Ring {
+  int stage = 0;
+  uint32_t phase = 0;
+  __device__ __forceinline__ void advance() {
+    if (++stage == kStages) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+};
+
+// The operand ring in the 1024-byte aligned dynamic shared memory (SWIZZLE_128B tiles need that
+// alignment): kStages A tiles, kStages B tiles, then the full and empty barriers at kOffBars.
+struct Operands {
+  uint8_t* base;  // the aligned shared memory
+  uint8_t* a;
+  uint8_t* b;
+  uint64_t* full_bar;   // [kStages]
+  uint64_t* empty_bar;  // [kStages]; the kernel's own barriers follow
+};
+
+// Prologue of both kernels, before their cluster / CTA sync: warp 0 prefetches the tensor maps,
+// lane 0 of warp 1 initialises the ring barriers.  A stage is free again after `empty_count`
+// arrivals: one per consumer warpgroup of every CTA that loads into it.
+template <int BLOCK_N>
+__device__ __forceinline__ Operands ring_prologue(uint8_t* smem_raw, const CUtensorMap* tmap_a,
+                                                  const CUtensorMap* tmap_b, int warp_idx,
+                                                  int lane, uint32_t empty_count) {
+  using C = Cfg<BLOCK_N>;
+  Operands op;
+  op.base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                       ~static_cast<uintptr_t>(1023));
+  op.a = op.base;
+  op.b = op.base + C::kStages * C::kABytes;
+  op.full_bar = reinterpret_cast<uint64_t*>(op.base + C::kOffBars);
+  op.empty_bar = op.full_bar + C::kStages;
+  if (warp_idx == 0 && lane == 0) {
+    tma_prefetch_desc(tmap_a);
+    tma_prefetch_desc(tmap_b);
+  }
+  if (warp_idx == 1 && lane == 0) {
+    for (int i = 0; i < C::kStages; ++i) {
+      mbar_init(&op.full_bar[i], 1);
+      mbar_init(&op.empty_bar[i], empty_count);
+    }
+    fence_barrier_init();
+  }
+  return op;
+}
+
+// Producer: wait until the inbound 128-row panel m_blk of A is complete (GEMM -> GEMM boundary).
+// A timeout sets error code 1 and the loads go ahead.
+__device__ __forceinline__ void wait_inbound_panel(const GemmCommon& p, int m_blk) {
+  if (elect_one_sync()) {
+    const uint32_t target = (*p.wait_epoch) * p.wait_mult;
+    if (!wait_flag_ge(p.wait_flags + m_blk, target, kFlagTimeoutNs)) {
+      if (p.error_flag) atomicExch(p.error_flag, 1);
+    }
+    fence_proxy_async();  // peer generic-proxy writes -> our async-proxy (TMA) reads
+  }
+  __syncwarp();
+}
+
+// Producer: TMA loads of k-block kb into ring stage `stage`, whose empty barrier the caller has
+// waited on.  A: rows a_row0 .. a_row0 + 127; B: rows b_row0 .. of this CTA's share of the tile.
+// cl_rank = rank in the cluster (CL, see gemm_wgmma_kernel).  no_loads (debug mode 3, single CTAs
+// only) completes the stage without loading: the MMAs then read stale shared memory.
+template <int BLOCK_N, bool A_MN, bool B_MN, int CL>
+__device__ __forceinline__ void load_k_block(const Operands& op, int stage,
+                                             const CUtensorMap* tmap_a, const CUtensorMap* tmap_b,
+                                             int kb, int a_row0, int b_row0, uint32_t cl_rank,
+                                             bool no_loads) {
+  constexpr bool PAIR = CL >= 2;
+  constexpr bool MC = CL == 4;
+  using C = Cfg<BLOCK_N>;
+  constexpr int kBRows = PAIR ? BLOCK_N / 2 : BLOCK_N;  // B rows fetched by ONE CTA
+  uint64_t* full = &op.full_bar[stage];
+  if (!PAIR && no_loads) {
+    if (elect_one_sync()) mbar_arrive(full);
+    __syncwarp();
+    return;
+  }
+  if (elect_one_sync()) {
+    const uint32_t cta_rank = cl_rank & 1u;  // rank in the pair
+    const uint16_t mask_b = static_cast<uint16_t>(3u << (cl_rank & ~1u));  // my pair
+    const uint16_t mask_a = static_cast<uint16_t>((1u << cl_rank) | (1u << (cl_rank ^ 2u)));
+    mbar_expect_tx(full, C::kStageBytes);
+    uint8_t* sa = op.a + stage * C::kABytes;
+    uint8_t* sb = op.b + stage * C::kBBytes;
+    // ---- A: my 128 rows (MC: my half of them, delivered to me and to the other pair) ----
+    if constexpr (MC) {
+      const int h = static_cast<int>(cl_rank >> 1);
+      if constexpr (!A_MN)
+        tma_load_2d_mc(sa + h * (64 * 128), tmap_a, full, kb * BLOCK_K, a_row0 + h * 64, mask_a);
+      else
+        tma_load_2d_mc(sa + h * (BLOCK_K * 128), tmap_a, full, a_row0 + h * 64, kb * BLOCK_K,
+                       mask_a);
+    } else if constexpr (!A_MN) {
+      tma_load_2d(sa, tmap_a, full, kb * BLOCK_K, a_row0);
+    } else {
+#pragma unroll
+      for (int c = 0; c < BLOCK_M / 64; ++c)
+        tma_load_2d(sa + c * (BLOCK_K * 128), tmap_a, full, a_row0 + c * 64, kb * BLOCK_K);
+    }
+    // ---- B: the whole tile, or (clusters) my half of it multicast to my pair ----
+    if constexpr (!PAIR) {
+      if constexpr (!B_MN) {
+        tma_load_2d(sb, tmap_b, full, kb * BLOCK_K, b_row0);
+      } else {
+#pragma unroll
+        for (int c = 0; c < BLOCK_N / 64; ++c)
+          tma_load_2d(sb + c * (BLOCK_K * 128), tmap_b, full, b_row0 + c * 64, kb * BLOCK_K);
+      }
+    } else {
+      uint8_t* sbh = sb + cta_rank * (C::kBBytes / 2);
+      if constexpr (!B_MN) {
+        tma_load_2d_mc(sbh, tmap_b, full, kb * BLOCK_K, b_row0, mask_b);
+      } else {
+#pragma unroll
+        for (int c = 0; c < kBRows / 64; ++c)
+          tma_load_2d_mc(sbh + c * (BLOCK_K * 128), tmap_b, full, b_row0 + c * 64, kb * BLOCK_K,
+                         mask_b);
+      }
+    }
+  }  // elected lane
+  __syncwarp();
+}
+
 // A consumer warpgroup hands a smem stage back to the producer(s): with clusters every CTA that
 // multicasts into this stage waits for all CTAs' consumers, so the arrival goes to every CTA.
 template <int CL>
@@ -198,10 +363,10 @@ __device__ __forceinline__ void release_stage(uint64_t* empty_bar) {
 // One wgmma group stays in flight; a stage is released once the group that read it has retired.
 template <int BLOCK_N, bool A_MN, bool B_MN, int CL, int kStages>
 __device__ __forceinline__ void consumer_mainloop(float (&acc)[BLOCK_N / 2], int kb0, int kb1,
-                                                  uint32_t a_base, uint32_t b_base, int a_bytes,
-                                                  int b_bytes, uint64_t* full_bar,
-                                                  uint64_t* empty_bar, int& stage, uint32_t& phase,
+                                                  uint32_t a_base, uint32_t b_base,
+                                                  const Operands& op, Ring<kStages>& ring,
                                                   bool elected, bool skip_mma) {
+  using C = Cfg<BLOCK_N>;
   // K-major  SW128: 8-row atoms 1024B apart (SBO), LBO unused (1); K advance = 32B per MMA_K
   // MN-major SW128: 64-element MN chunks BLOCK_K*128B apart (LBO), 8-k-row groups 1024B apart
   //                 (SBO); K advance = 16 rows * 128B = 2048B per MMA_K
@@ -210,11 +375,11 @@ __device__ __forceinline__ void consumer_mainloop(float (&acc)[BLOCK_N / 2], int
   constexpr uint32_t a_kadv = (A_MN ? MMA_K * 128 : MMA_K * 2) >> 4;
   constexpr uint32_t b_kadv = (B_MN ? MMA_K * 128 : MMA_K * 2) >> 4;
   int prev = -1;
-  for (int kb = kb0; kb < kb1; ++kb) {
-    mbar_wait(&full_bar[stage], phase);
+  for (int kb = kb0; kb < kb1; ++kb, ring.advance()) {
+    mbar_wait(&op.full_bar[ring.stage], ring.phase);
     if (!skip_mma) {
-      const uint64_t desc_a = make_smem_desc_sw128(a_base + stage * a_bytes, a_lbo, 1024);
-      const uint64_t desc_b = make_smem_desc_sw128(b_base + stage * b_bytes, b_lbo, 1024);
+      const uint64_t desc_a = make_smem_desc_sw128(a_base + ring.stage * C::kABytes, a_lbo, 1024);
+      const uint64_t desc_b = make_smem_desc_sw128(b_base + ring.stage * C::kBBytes, b_lbo, 1024);
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < BLOCK_K / MMA_K; ++k)
@@ -223,15 +388,47 @@ __device__ __forceinline__ void consumer_mainloop(float (&acc)[BLOCK_N / 2], int
       wgmma_commit();
       wgmma_wait<1>();
     }
-    if (prev >= 0 && elected) release_stage<CL>(&empty_bar[prev]);
-    prev = stage;
-    if (++stage == kStages) {
-      stage = 0;
-      phase ^= 1;
-    }
+    if (prev >= 0 && elected) release_stage<CL>(&op.empty_bar[prev]);
+    prev = ring.stage;
   }
   wgmma_wait<0>();
-  if (prev >= 0 && elected) release_stage<CL>(&empty_bar[prev]);
+  if (prev >= 0 && elected) release_stage<CL>(&op.empty_bar[prev]);
+}
+
+// A consumer thread's place in the tile: consumer warpgroup wg owns rows 64 wg .. 64 wg + 63 of
+// the tile, its warp q rows 16 q .. 16 q + 15 (warp_row = 64 wg + 16 q), and the thread the
+// fragment rows fr and fr + 8 of those (see frag_store_bf16).
+struct Consumer {
+  int wg;
+  int epi_tid;     // 0..255
+  bool elected;    // thread 0 of its warpgroup: hands ring stages back
+  int fr;
+  int fc;          // fragment column pair inside every 8-column block
+  int warp_row;
+  uint8_t* stage;  // the warp's bf16 staging buffer
+  Dropout dr;
+};
+__device__ __forceinline__ Consumer consumer_of(int warp_idx, int lane, uint8_t* out_stage,
+                                                const GemmCommon& p) {
+  const int e = warp_idx - kEpiWarp0;
+  Consumer c;
+  c.wg = e >> 2;
+  c.epi_tid = threadIdx.x - kEpiWarp0 * 32;
+  c.elected = (c.epi_tid & 127) == 0;
+  c.fr = lane >> 2;
+  c.fc = (lane & 3) * 2;
+  c.warp_row = c.wg * 64 + (e & 3) * 16;
+  c.stage = out_stage + e * kWarpStageBytes;
+  c.dr = dropout_of(p.dropout_p, p.rng_state, p.rng_stream);
+  return c;
+}
+
+// publish a finished tile of panel m_blk: all 256 epilogue threads' stores -> fence -> barrier ->
+// one release.sys on the panel's flag
+__device__ __forceinline__ void publish_panel(uint32_t* signal_flags, int m_blk, int epi_tid) {
+  __threadfence_system();
+  asm volatile("bar.sync 2, 256;" ::: "memory");
+  if (epi_tid == 0) red_release_sys_add(signal_flags + m_blk, 1u);
 }
 
 // CL = CTAs per cluster: 1 = independent CTAs; 2 = two CTAs that compute vertically neighbouring
@@ -254,17 +451,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   const uint32_t pair_idx = cl_rank >> 1;                  // which pair of the cluster (MC)
 
   extern __shared__ uint8_t smem_raw[];
-  // SWIZZLE_128B tiles need 1024-byte alignment.
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + kStages * C::kABytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::kOffBars);
-  uint64_t* full_bar = bars;             // [kStages]
-  uint64_t* empty_bar = bars + kStages;  // [kStages]
-  uint32_t* s_ticket = reinterpret_cast<uint32_t*>(bars + 2 * kStages);
-  float* s_bias = reinterpret_cast<float*>(smem + C::kOffBias);
-
   const int warp_idx = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
 
@@ -280,17 +466,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   const int unit_id = static_cast<int>(blockIdx.x) / CL;
   const int num_units = static_cast<int>(gridDim.x) / CL;
 
-  if (warp_idx == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-  }
-  if (warp_idx == 1 && lane == 0) {
-    for (int i = 0; i < kStages; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 2 * CL);  // one arrival per consumer warpgroup of every CTA
-    }
-    fence_barrier_init();
-  }
+  const Operands op = ring_prologue<BLOCK_N>(smem_raw, &tmap_a, &tmap_b, warp_idx, lane, 2 * CL);
+  uint32_t* s_ticket = reinterpret_cast<uint32_t*>(op.empty_bar + kStages);
+  float* s_bias = reinterpret_cast<float*>(op.base + C::kOffBias);
   __syncwarp();
   if constexpr (PAIR)
     cluster_sync_all();  // the peers' barriers must be initialised before anything signals them
@@ -305,11 +483,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (warp_idx == 0) {
       // ===================================== TMA producer =====================================
-      int stage = 0;
-      uint32_t phase = 0;
-      const uint16_t mask_b = static_cast<uint16_t>(3u << (cl_rank & ~1u));  // my pair
-      const uint16_t mask_a = static_cast<uint16_t>((1u << cl_rank) | (1u << (cl_rank ^ 2u)));
-      constexpr int kBRows = PAIR ? BLOCK_N / 2 : BLOCK_N;  // B rows fetched by ONE CTA
+      Ring<kStages> ring;
       Sched sched;
       sched.init(SK ? 1 : 0, unit_id, num_units, num_tiles, num_k_blks);
       Work w;
@@ -318,113 +492,29 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
         const int m_blk = (tile % num_m_units) * (PAIR ? 2 : 1) + static_cast<int>(cta_rank);
         const int n_blk =
             (tile / num_m_units) * (MC ? 2 : 1) + (MC ? static_cast<int>(pair_idx) : 0);
-        const int b_row0 = n_blk * BLOCK_N + static_cast<int>(cta_rank) * (PAIR ? kBRows : 0);
-        if (p.wait_flags != nullptr && m_blk * BLOCK_M < p.M) {
-          if (elect_one_sync()) {
-            const uint32_t target = (*p.wait_epoch) * p.wait_mult;
-            if (!wait_flag_ge(p.wait_flags + m_blk, target, kFlagTimeoutNs)) {
-              if (p.error_flag) atomicExch(p.error_flag, 1);
-            }
-            fence_proxy_async();  // peer generic-proxy writes -> our async-proxy (TMA) reads
-          }
-          __syncwarp();
-        }
-        for (int kb = w.kb0; kb < w.kb1; ++kb) {
-          mbar_wait_cluster(&empty_bar[stage], phase ^ 1);
-          if (!PAIR && p.debug == 3) {  // triage: no loads at all, the MMAs chew on stale smem
-            if (elect_one_sync()) mbar_arrive(&full_bar[stage]);
-            __syncwarp();
-            if (++stage == kStages) {
-              stage = 0;
-              phase ^= 1;
-            }
-            continue;
-          }
-          if (elect_one_sync()) {
-            mbar_expect_tx(&full_bar[stage], C::kStageBytes);
-            uint8_t* sa = smem_a + stage * C::kABytes;
-            uint8_t* sb = smem_b + stage * C::kBBytes;
-            // ---- A: my 128 rows (MC: my half of them, delivered to me and to the other pair) ----
-            if constexpr (MC) {
-              const int h = static_cast<int>(pair_idx);
-              if constexpr (!A_MN)
-                tma_load_2d_mc(sa + h * (64 * 128), &tmap_a, &full_bar[stage], kb * BLOCK_K,
-                               m_blk * BLOCK_M + h * 64, mask_a);
-              else
-                tma_load_2d_mc(sa + h * (BLOCK_K * 128), &tmap_a, &full_bar[stage],
-                               m_blk * BLOCK_M + h * 64, kb * BLOCK_K, mask_a);
-            } else if constexpr (!A_MN) {
-              tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * BLOCK_K, m_blk * BLOCK_M);
-            } else {
-#pragma unroll
-              for (int c = 0; c < BLOCK_M / 64; ++c)
-                tma_load_2d(sa + c * (BLOCK_K * 128), &tmap_a, &full_bar[stage],
-                            m_blk * BLOCK_M + c * 64, kb * BLOCK_K);
-            }
-            // ---- B: the whole tile, or (clusters) my half of it multicast to my pair ----
-            if constexpr (!PAIR) {
-              if constexpr (!B_MN) {
-                tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BLOCK_K, b_row0);
-              } else {
-#pragma unroll
-                for (int c = 0; c < BLOCK_N / 64; ++c)
-                  tma_load_2d(sb + c * (BLOCK_K * 128), &tmap_b, &full_bar[stage], b_row0 + c * 64,
-                              kb * BLOCK_K);
-              }
-            } else {
-              uint8_t* sbh = sb + cta_rank * (C::kBBytes / 2);
-              if constexpr (!B_MN) {
-                tma_load_2d_mc(sbh, &tmap_b, &full_bar[stage], kb * BLOCK_K, b_row0, mask_b);
-              } else {
-#pragma unroll
-                for (int c = 0; c < kBRows / 64; ++c)
-                  tma_load_2d_mc(sbh + c * (BLOCK_K * 128), &tmap_b, &full_bar[stage],
-                                 b_row0 + c * 64, kb * BLOCK_K, mask_b);
-              }
-            }
-          }  // elected lane
-          __syncwarp();
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
+        const int b_row0 = n_blk * BLOCK_N + static_cast<int>(cta_rank) * (PAIR ? BLOCK_N / 2 : 0);
+        if (p.wait_flags != nullptr && m_blk * BLOCK_M < p.M) wait_inbound_panel(p, m_blk);
+        for (int kb = w.kb0; kb < w.kb1; ++kb, ring.advance()) {
+          mbar_wait_cluster(&op.empty_bar[ring.stage], ring.phase ^ 1);
+          load_k_block<BLOCK_N, A_MN, B_MN, CL>(op, ring.stage, &tmap_a, &tmap_b, kb,
+                                                m_blk * BLOCK_M, b_row0, cl_rank, p.debug == 3);
         }
       }
     }
   } else {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     // ============================ consumers: wgmma main loop + epilogue ============================
-    // Warpgroup wg owns rows 64 wg .. 64 wg + 63 of the tile, warp q of it rows 16 q .. 16 q + 15.
     // The epilogue runs on the accumulator fragments in registers, 64 columns at a time; bias for
     // the tile is staged once in shared memory, aux (residual / pre-activation) blocks are loaded
     // before the epilogue math, fp32 gradient accumulation uses red.global.add (no
     // read-modify-write).
-    const int e = warp_idx - kEpiWarp0;
-    const int q = e & 3;
-    const int wg = e >> 2;  // consumer warpgroup 0 / 1
-    const int epi_tid = threadIdx.x - kEpiWarp0 * 32;  // 0..255
-    const int wg_tid = epi_tid & 127;
-    const bool elected = wg_tid == 0;
-    uint8_t* s_stage = smem + C::kOffOut + e * kWarpStageBytes;
-    const int fr = lane >> 2;        // fragment rows fr and fr + 8 of the warp's 16
-    const int fc = (lane & 3) * 2;   // fragment column pair inside every 8-column block
-    const int warp_row_in_tile = wg * 64 + q * 16;
-    const bool has_dropout = p.dropout_p > 0.f;
+    const Consumer c = consumer_of(warp_idx, lane, op.base + C::kOffOut, p);
     const bool has_aux = p.aux != nullptr;
-    uint64_t seed = 0;
-    uint32_t thr16 = 0;
-    float drop_scale = 1.f;
-    if (has_dropout) {
-      seed = dropout_seed(p.rng_state, p.rng_stream);
-      thr16 = static_cast<uint32_t>(p.dropout_p * 65536.f);
-      drop_scale = 1.f / (1.f - p.dropout_p);
-    }
     int it = 0;
-    int stage = 0;
-    uint32_t phase = 0;
+    Ring<kStages> ring;
     // both MN- and K-major A tiles keep rows 64..127 one 8 KB block after rows 0..63
-    const uint32_t a_base = smem_u32(smem_a) + wg * 8192;
-    const uint32_t b_base = smem_u32(smem_b);
+    const uint32_t a_base = smem_u32(op.a) + c.wg * 8192;
+    const uint32_t b_base = smem_u32(op.b);
     Sched sched;
     sched.init(SK ? 1 : 0, unit_id, num_units, num_tiles, num_k_blks);
     Work w;
@@ -435,18 +525,17 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       const int tile = w.tile;
       const int m_blk = (tile % num_m_units) * (PAIR ? 2 : 1) + static_cast<int>(cta_rank);
       const int n_blk = (tile / num_m_units) * (MC ? 2 : 1) + (MC ? static_cast<int>(pair_idx) : 0);
-      const long long warp_row0 = static_cast<long long>(m_blk) * BLOCK_M + warp_row_in_tile;
-      const long long row_a = warp_row0 + fr;  // and row_a + 8
+      const long long warp_row0 = static_cast<long long>(m_blk) * BLOCK_M + c.warp_row;
+      const long long row_a = warp_row0 + c.fr;  // and row_a + 8
       // ---- stage bias (overlaps the main loop of the other warpgroup) ----
       float* sb = s_bias + (it & 1) * BLOCK_N;
-      if (epi_tid < BLOCK_N) {
-        const int gc = n_blk * BLOCK_N + epi_tid;
-        sb[epi_tid] = (p.bias != nullptr && gc < p.N) ? __ldg(p.bias + gc) : 0.f;
+      if (c.epi_tid < BLOCK_N) {
+        const int gc = n_blk * BLOCK_N + c.epi_tid;
+        sb[c.epi_tid] = (p.bias != nullptr && gc < p.N) ? __ldg(p.bias + gc) : 0.f;
       }
 
-      consumer_mainloop<BLOCK_N, A_MN, B_MN, CL, kStages>(
-          acc, w.kb0, w.kb1, a_base, b_base, C::kABytes, C::kBBytes, full_bar, empty_bar, stage,
-          phase, elected, !PAIR && p.debug == 4);
+      consumer_mainloop<BLOCK_N, A_MN, B_MN, CL>(acc, w.kb0, w.kb1, a_base, b_base, op, ring,
+                                                 c.elected, !PAIR && p.debug == 4);
 
       // ---- stream-K: is this CTA the one that finishes the tile? ----
       // Every contributor takes a ticket once its share of the K range is accumulated.  All but the
@@ -463,14 +552,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
         const int u_last = sched.unit_of(static_cast<long long>(tile + 1) * num_k_blks - 1);
         n_contrib = u_last - u_first + 1;
         asm volatile("bar.sync 1, 256;" ::: "memory");  // the previous tile's ticket has been read
-        if (epi_tid == 0) *s_ticket = atomicAdd(p.counters + 2 * ctile, 1u);
+        if (c.epi_tid == 0) *s_ticket = atomicAdd(p.counters + 2 * ctile, 1u);
         asm volatile("bar.sync 1, 256;" ::: "memory");
         finisher = (*s_ticket == static_cast<uint32_t>(n_contrib - 1));
         const int which = (tile == sched.first_tile(unit_id)) ? 0 : 1;
         ws_mine = p.ws + static_cast<size_t>((2 * unit_id + which) * kCtasPerUnit + cl_rank) *
                              kTileElems;
         if (finisher) {
-          if (epi_tid == 0) {
+          if (c.epi_tid == 0) {
             const uint64_t t0 = globaltimer_ns();
             while (ld_acquire_sys(p.counters + 2 * ctile + 1) <
                    static_cast<uint32_t>(n_contrib - 1)) {
@@ -488,7 +577,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       // workspace layout of one 128 x BLOCK_N tile: [8-column block][consumer thread][4] floats,
       // the fragment registers as they are, so that a warp's float4 accesses are contiguous
       auto ws_ptr = [&](float* base, int j) {
-        return reinterpret_cast<float4*>(base) + j * 256 + epi_tid;
+        return reinterpret_cast<float4*>(base) + j * 256 + c.epi_tid;
       };
       // every consumer thread has staged its share of this tile's bias (and, through the barrier of
       // the previous tile, nobody still reads the buffer that was overwritten)
@@ -527,17 +616,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
             }
           }
         }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float2 bb = *reinterpret_cast<const float2*>(sb + ct + j * 8 + fc);  // broadcast
-          f[4 * j] = f[4 * j] + bb.x;
-          f[4 * j + 1] = f[4 * j + 1] + bb.y;
-          f[4 * j + 2] = f[4 * j + 2] + bb.x;
-          f[4 * j + 3] = f[4 * j + 3] + bb.y;
-        }
+        frag_add_bias(f, sb, ct, c.fc);
         if (p.act == ACT_GELU) {
           if (p.out2 != nullptr && p.debug != 2)
-            frag_store_bf16(f, s_stage, lane, reinterpret_cast<__nv_bfloat16*>(p.out2), p.ldo2,
+            frag_store_bf16(f, c.stage, lane, reinterpret_cast<__nv_bfloat16*>(p.out2), p.ldo2,
                             warp_row0, p.M, col0, p.N);
 #pragma unroll
           for (int i = 0; i < 32; ++i) f[i] = gelu_fast(f[i]);
@@ -545,34 +627,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
 #pragma unroll
           for (int i = 0; i < 32; ++i) f[i] = tanh_fast(f[i]);
         }
-        if (has_dropout) frag_dropout(f, seed, thr16, drop_scale, row_a, col0, p.N, lane);
-        if (has_aux) {
-          uint32_t aw[16];
-          aux_to_frag(ax, s_stage, lane, aw);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float2 xa = unpack_bf16x2(aw[2 * j]);
-            const float2 xb = unpack_bf16x2(aw[2 * j + 1]);
-            if (p.act == ACT_DGELU_MUL_AUX) {
-              f[4 * j] *= dgelu_fast(xa.x);
-              f[4 * j + 1] *= dgelu_fast(xa.y);
-              f[4 * j + 2] *= dgelu_fast(xb.x);
-              f[4 * j + 3] *= dgelu_fast(xb.y);
-            } else if (p.add_aux) {
-              f[4 * j] += xa.x;
-              f[4 * j + 1] += xa.y;
-              f[4 * j + 2] += xb.x;
-              f[4 * j + 3] += xb.y;
-            }
-          }
-        }
+        if (c.dr.on) frag_dropout(f, c.dr.seed, c.dr.thr16, c.dr.scale, row_a, col0, p.N, lane);
+        if (has_aux) frag_apply_aux(f, ax, c.stage, lane, p.act == ACT_DGELU_MUL_AUX, p.add_aux);
         if (p.debug != 2) {
           if constexpr (OUT_F32) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               const long long row = row_a + 8 * h;
               if (row < p.M) {
-                float* o = reinterpret_cast<float*>(p.out) + row * p.ldo + col0 + fc;
+                float* o = reinterpret_cast<float*>(p.out) + row * p.ldo + col0 + c.fc;
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                   // covers columns fc, fc + 1 only because N % 8 == 0 (launch_gemm checks it)
@@ -587,7 +650,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
               }
             }
           } else {
-            frag_store_bf16(f, s_stage, lane, reinterpret_cast<__nv_bfloat16*>(p.out), p.ldo,
+            frag_store_bf16(f, c.stage, lane, reinterpret_cast<__nv_bfloat16*>(p.out), p.ldo,
                             warp_row0, p.M, col0, p.N);
           }
         }
@@ -596,14 +659,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
         // publish the parked partial: all stores -> fence -> barrier -> one counter bump
         __threadfence();
         asm volatile("bar.sync 2, 256;" ::: "memory");
-        if (epi_tid == 0) atomicAdd(p.counters + 2 * ctile + 1, 1u);
+        if (c.epi_tid == 0) atomicAdd(p.counters + 2 * ctile + 1, 1u);
       }
-      if (finisher && p.signal_flags != nullptr && m_blk * BLOCK_M < p.M) {
-        // publish this tile: all 256 epilogue threads' stores -> barrier -> one release.sys
-        __threadfence_system();
-        asm volatile("bar.sync 2, 256;" ::: "memory");
-        if (epi_tid == 0) red_release_sys_add(p.signal_flags + m_blk, 1u);
-      }
+      if (finisher && p.signal_flags != nullptr && m_blk * BLOCK_M < p.M)
+        publish_panel(p.signal_flags, m_blk, c.epi_tid);
     }
   }
 
@@ -622,7 +681,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
 //
 // A LayerNorm row spans all N columns, a CTA's accumulator only BLOCK_N of them, so the N / BLOCK_N
 // CTAs that own the column tiles of one 128-row panel form a THREAD-BLOCK CLUSTER (2..8 CTAs) and
-// exchange per-row partial sums through distributed shared memory:
+// exchange per-row partial sums through distributed shared memory.  The prologue, the producer,
+// the main loop and the epilogue steps of pass 1 are those of gemm_wgmma_kernel:
 //
 //   pass 1  on the accumulator fragments: + bias, dropout, + residual; store z (bf16, saved for
 //           backward); accumulate row sum / sum of squares (the quad that holds a row combines
@@ -638,26 +698,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
 // Reference ops replaced: scaelum/model/bert_layers.py:285-289 (BertSelfOutput) and :323-327
 // (BertOutput); hop replaced: scaelum/builder/module_wrapper.py:148-175.
 // ------------------------------------------------------------------------------------------
-struct GemmLnDev {
-  int M, N, K;
+struct GemmLnDev : GemmCommon {
   void* y;
   void* z;
-  long long ldy, ldz, ldaux;
-  const float* bias;
-  const __nv_bfloat16* aux;
+  long long ldy, ldz;
   const float* gamma;
   const float* beta;
   float* mean;
   float* rstd;
   float eps;
-  float dropout_p;
-  const uint64_t* rng_state;
-  uint32_t rng_stream;
-  uint32_t* signal_flags;
-  const uint32_t* wait_flags;
-  const uint32_t* wait_epoch;
-  uint32_t wait_mult;
-  int* error_flag;
 };
 
 constexpr int kLnMaxCluster = 8;
@@ -665,11 +714,9 @@ constexpr int kLnMaxCluster = 8;
 template <int BLOCK_N>
 struct LnCfg {
   using C = Cfg<BLOCK_N>;
-  static constexpr int kStages = C::kStages;
   static constexpr int kVecBytes = 3 * BLOCK_N * 4;                 // bias, gamma, beta
   static constexpr int kStatsBytes = kLnMaxCluster * BLOCK_M * 8;   // float2 per (cta, row)
-  static constexpr int kOffBars = kStages * C::kStageBytes;
-  static constexpr int kOffVec = kOffBars + 256;
+  static constexpr int kOffVec = C::kOffBars + 256;
   static constexpr int kOffOut = kOffVec + kVecBytes;
   static constexpr int kOffStats = kOffOut + C::kOutStageBytes;
   static constexpr int kSmemBytes = kOffStats + kStatsBytes + 1024 /*align slack*/;
@@ -681,39 +728,23 @@ __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
                      const __grid_constant__ CUtensorMap tmap_b, const GemmLnDev p) {
   using L = LnCfg<BLOCK_N>;
-  using C = typename L::C;
-  constexpr int kStages = L::kStages;
+  constexpr int kStages = L::C::kStages;
   const uint32_t cln = cluster_nctarank();     // CTAs per cluster == column tiles per row panel
   const uint32_t n_blk = cluster_ctarank();    // this CTA's column tile
   const int m_blk = static_cast<int>(blockIdx.x / cln);
 
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + kStages * C::kABytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kOffBars);
-  uint64_t* full_bar = bars;               // [kStages]
-  uint64_t* empty_bar = bars + kStages;    // [kStages]
-  uint64_t* stats_bar = bars + 2 * kStages;
-  float* s_bias = reinterpret_cast<float*>(smem + L::kOffVec);
-  float* s_gamma = s_bias + BLOCK_N;
-  float* s_beta = s_gamma + BLOCK_N;
-  float2* s_stats = reinterpret_cast<float2*>(smem + L::kOffStats);   // [cln][128]
-
   const int warp_idx = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
   const int num_k_blks = (p.K + BLOCK_K - 1) / BLOCK_K;
 
-  if (warp_idx == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-  }
+  const Operands op = ring_prologue<BLOCK_N>(smem_raw, &tmap_a, &tmap_b, warp_idx, lane, 2);
+  uint64_t* stats_bar = op.empty_bar + kStages;
+  float* s_bias = reinterpret_cast<float*>(op.base + L::kOffVec);
+  float* s_gamma = s_bias + BLOCK_N;
+  float* s_beta = s_gamma + BLOCK_N;
+  float2* s_stats = reinterpret_cast<float2*>(op.base + L::kOffStats);   // [cln][128]
   if (warp_idx == 1 && lane == 0) {
-    for (int i = 0; i < kStages; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 2);
-    }
     mbar_init(stats_bar, cln * BLOCK_M);   // one arrival per row-owner thread of every CTA
     fence_barrier_init();
   }
@@ -726,62 +757,23 @@ gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (warp_idx == 0) {
       // ===================================== TMA producer =====================================
-      int stage = 0;
-      uint32_t phase = 0;
-      if (p.wait_flags != nullptr) {
-        if (elect_one_sync()) {
-          const uint32_t target = (*p.wait_epoch) * p.wait_mult;
-          if (!wait_flag_ge(p.wait_flags + m_blk, target, kFlagTimeoutNs)) {
-            if (p.error_flag) atomicExch(p.error_flag, 1);
-          }
-          fence_proxy_async();
-        }
-        __syncwarp();
-      }
-      for (int kb = 0; kb < num_k_blks; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        if (elect_one_sync()) {
-          mbar_expect_tx(&full_bar[stage], C::kStageBytes);
-          tma_load_2d(smem_a + stage * C::kABytes, &tmap_a, &full_bar[stage], kb * BLOCK_K,
-                      m_blk * BLOCK_M);
-          tma_load_2d(smem_b + stage * C::kBBytes, &tmap_b, &full_bar[stage], kb * BLOCK_K,
-                      static_cast<int>(n_blk) * BLOCK_N);
-        }
-        __syncwarp();
-        if (++stage == kStages) {
-          stage = 0;
-          phase ^= 1;
-        }
+      Ring<kStages> ring;
+      if (p.wait_flags != nullptr) wait_inbound_panel(p, m_blk);
+      for (int kb = 0; kb < num_k_blks; ++kb, ring.advance()) {
+        mbar_wait(&op.empty_bar[ring.stage], ring.phase ^ 1);
+        load_k_block<BLOCK_N, false, false, 1>(op, ring.stage, &tmap_a, &tmap_b, kb,
+                                               m_blk * BLOCK_M, static_cast<int>(n_blk) * BLOCK_N,
+                                               0u, false);
       }
     }
   } else {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     // ============================ consumers: wgmma main loop + epilogue ============================
-    // warpgroup wg owns rows 64 wg .. + 63 of the panel, warp q of it rows 16 q .. + 15; the whole
-    // epilogue runs on the accumulator fragments (rows fr and fr + 8 of the warp, see
-    // frag_store_bf16)
-    const int e = warp_idx - kEpiWarp0;
-    const int q = e & 3;
-    const int wg = e >> 2;
-    const int epi_tid = threadIdx.x - kEpiWarp0 * 32;
-    const int wg_tid = epi_tid & 127;
-    uint8_t* s_stage = smem + L::kOffOut + e * kWarpStageBytes;
-    const int fr = lane >> 2;
-    const int fc = (lane & 3) * 2;
-    const int warp_row_in_tile = wg * 64 + q * 16;
-    const long long warp_row0 = static_cast<long long>(m_blk) * BLOCK_M + warp_row_in_tile;
-    const long long row_a = warp_row0 + fr;  // and row_a + 8
-    const bool has_dropout = p.dropout_p > 0.f;
+    const Consumer c = consumer_of(warp_idx, lane, op.base + L::kOffOut, p);
+    const long long warp_row0 = static_cast<long long>(m_blk) * BLOCK_M + c.warp_row;
+    const long long row_a = warp_row0 + c.fr;  // and row_a + 8
     const bool has_aux = p.aux != nullptr;
-    uint64_t seed = 0;
-    uint32_t thr16 = 0;
-    float drop_scale = 1.f;
-    if (has_dropout) {
-      seed = dropout_seed(p.rng_state, p.rng_stream);
-      thr16 = static_cast<uint32_t>(p.dropout_p * 65536.f);
-      drop_scale = 1.f / (1.f - p.dropout_p);
-    }
-    for (int i = epi_tid; i < BLOCK_N; i += 256) {
+    for (int i = c.epi_tid; i < BLOCK_N; i += 256) {
       const int gc = static_cast<int>(n_blk) * BLOCK_N + i;
       s_bias[i] = p.bias != nullptr ? __ldg(p.bias + gc) : 0.f;
       s_gamma[i] = __ldg(p.gamma + gc);
@@ -790,11 +782,9 @@ gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
 
     float acc[BLOCK_N / 2];
     {
-      int stage = 0;
-      uint32_t phase = 0;
-      consumer_mainloop<BLOCK_N, false, false, 1, kStages>(
-          acc, 0, num_k_blks, smem_u32(smem_a) + wg * 8192, smem_u32(smem_b), C::kABytes,
-          C::kBBytes, full_bar, empty_bar, stage, phase, wg_tid == 0, false);
+      Ring<kStages> ring;
+      consumer_mainloop<BLOCK_N, false, false, 1>(acc, 0, num_k_blks, smem_u32(op.a) + c.wg * 8192,
+                                                  smem_u32(op.b), op, ring, c.elected, false);
     }
     asm volatile("bar.sync 1, 256;" ::: "memory");   // bias / gamma / beta staged
 
@@ -809,27 +799,10 @@ gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       if (has_aux) aux_load(ax, p.aux, p.ldaux, warp_row0, p.M, col0, p.N, lane);
       float f[32];
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float2 bb = *reinterpret_cast<const float2*>(s_bias + ct + j * 8 + fc);
-        f[4 * j] = acc[g * 32 + 4 * j] + bb.x;
-        f[4 * j + 1] = acc[g * 32 + 4 * j + 1] + bb.y;
-        f[4 * j + 2] = acc[g * 32 + 4 * j + 2] + bb.x;
-        f[4 * j + 3] = acc[g * 32 + 4 * j + 3] + bb.y;
-      }
-      if (has_dropout) frag_dropout(f, seed, thr16, drop_scale, row_a, col0, p.N, lane);
-      if (has_aux) {
-        uint32_t aw[16];
-        aux_to_frag(ax, s_stage, lane, aw);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float2 xa = unpack_bf16x2(aw[2 * j]);
-          const float2 xb = unpack_bf16x2(aw[2 * j + 1]);
-          f[4 * j] += xa.x;
-          f[4 * j + 1] += xa.y;
-          f[4 * j + 2] += xb.x;
-          f[4 * j + 3] += xb.y;
-        }
-      }
+      for (int i = 0; i < 32; ++i) f[i] = acc[g * 32 + i];
+      frag_add_bias(f, s_bias, ct, c.fc);
+      if (c.dr.on) frag_dropout(f, c.dr.seed, c.dr.thr16, c.dr.scale, row_a, col0, p.N, lane);
+      if (has_aux) frag_apply_aux(f, ax, c.stage, lane, false, true);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         s1a += f[4 * j] + f[4 * j + 1];
@@ -840,7 +813,7 @@ gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
 #pragma unroll
       for (int i = 0; i < 32; ++i) acc[g * 32 + i] = f[i];
       if (p.z != nullptr)
-        frag_store_bf16(f, s_stage, lane, reinterpret_cast<__nv_bfloat16*>(p.z), p.ldz, warp_row0,
+        frag_store_bf16(f, c.stage, lane, reinterpret_cast<__nv_bfloat16*>(p.z), p.ldz, warp_row0,
                         p.M, col0, p.N);
     }
     // ---------------- cluster-wide row statistics through distributed shared memory ----------------
@@ -853,7 +826,7 @@ gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       s1b += __shfl_xor_sync(0xffffffffu, s1b, o);
       s2b += __shfl_xor_sync(0xffffffffu, s2b, o);
     }
-    const int row_a_in_tile = warp_row_in_tile + fr;
+    const int row_a_in_tile = c.warp_row + c.fr;
     if ((lane & 3) < 2) {
       const int hb = lane & 1;
       const uint32_t slot = smem_u32(&s_stats[n_blk * BLOCK_M + row_a_in_tile + 8 * hb]);
@@ -896,23 +869,19 @@ gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       float f[32];
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const float2 gm = *reinterpret_cast<const float2*>(s_gamma + ct + j * 8 + fc);
-        const float2 bt = *reinterpret_cast<const float2*>(s_beta + ct + j * 8 + fc);
+        const float2 gm = *reinterpret_cast<const float2*>(s_gamma + ct + j * 8 + c.fc);
+        const float2 bt = *reinterpret_cast<const float2*>(s_beta + ct + j * 8 + c.fc);
         f[4 * j] = fmaf((acc[g * 32 + 4 * j] - mean_a) * rstd_a, gm.x, bt.x);
         f[4 * j + 1] = fmaf((acc[g * 32 + 4 * j + 1] - mean_a) * rstd_a, gm.y, bt.y);
         f[4 * j + 2] = fmaf((acc[g * 32 + 4 * j + 2] - mean_b) * rstd_b, gm.x, bt.x);
         f[4 * j + 3] = fmaf((acc[g * 32 + 4 * j + 3] - mean_b) * rstd_b, gm.y, bt.y);
       }
-      frag_store_bf16(f, s_stage, lane, reinterpret_cast<__nv_bfloat16*>(p.y), p.ldy, warp_row0,
+      frag_store_bf16(f, c.stage, lane, reinterpret_cast<__nv_bfloat16*>(p.y), p.ldy, warp_row0,
                       p.M, col0, p.N);
     }
-    if (p.signal_flags != nullptr) {
-      // publish this CTA's 128 x BLOCK_N tile of the panel: stores -> fence -> barrier -> one
-      // release.sys; the consumer waits for epoch x (N / BLOCK_N) signals per panel
-      __threadfence_system();
-      asm volatile("bar.sync 2, 256;" ::: "memory");
-      if (epi_tid == 0) red_release_sys_add(p.signal_flags + m_blk, 1u);
-    }
+    // publish this CTA's 128 x BLOCK_N tile of the panel; the consumer waits for epoch x
+    // (N / BLOCK_N) signals per panel
+    if (p.signal_flags != nullptr) publish_panel(p.signal_flags, m_blk, c.epi_tid);
   }
 
   __syncwarp();
@@ -984,36 +953,38 @@ int gemm_pick_block_n(int M, int N) {
   return 256;
 }
 
-bool gemm_pick_quad(int M, int N, int K) {
-  // 4-CTA clusters (two pairs, A and B multicast).  Opt-in (SKY_GEMM_QUAD=1): not yet measured
-  // against independent CTAs on H100.
-  (void)M;
-  (void)N;
-  (void)K;
-  static int env = -2;
-  if (env == -2) {
-    const char* e = std::getenv("SKY_GEMM_QUAD");
-    env = e ? std::atoi(e) : -1;
-  }
-  return env > 0;
-}
-
-bool gemm_pick_pair(int M, int N, int K) {
-  (void)N;
-  (void)K;
-  static int env = -2;
-  if (env == -2) {
-    const char* e = std::getenv("SKY_GEMM_PAIR");
-    env = e ? std::atoi(e) : -1;
-  }
-  if (env >= 0) return env != 0 && M > 128;
-  return false;  // opt-in (SKY_GEMM_PAIR=1): not yet measured against independent CTAs on H100
-}
-
 int gemm_tiles_per_panel(int N, int block_n) { return (N + block_n - 1) / block_n; }
 
 namespace {
-static int g_num_sms = 0;
+// SKY_GEMM_PAIR, SKY_GEMM_QUAD and SKY_GEMM_STREAMK (-1 when unset), read once per process
+struct GemmEnv {
+  int pair, quad, stream_k;
+};
+const GemmEnv& gemm_env() {
+  static const GemmEnv env = [] {
+    auto get = [](const char* name) {
+      const char* e = std::getenv(name);
+      return e ? std::atoi(e) : -1;
+    };
+    return GemmEnv{get("SKY_GEMM_PAIR"), get("SKY_GEMM_QUAD"), get("SKY_GEMM_STREAMK")};
+  }();
+  return env;
+}
+
+// 2-CTA clusters (B multicast) and 4-CTA clusters (two pairs, A and B multicast) are opt-in
+// (SKY_GEMM_PAIR=1, SKY_GEMM_QUAD=1): not yet measured against independent CTAs on H100.
+bool pick_pair(int M) { return gemm_env().pair > 0 && M > 128; }
+bool pick_quad() { return gemm_env().quad > 0; }
+
+int num_sms() {
+  static int n = 0;
+  if (n == 0) {
+    int dev_id = 0;
+    cudaGetDevice(&dev_id);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev_id);
+  }
+  return n;
+}
 
 // ---- stream-K workspace: one per (device, stream), because GEMMs on different streams overlap ----
 constexpr size_t kWsSlotBytes = static_cast<size_t>(BLOCK_M) * 256 * 4;  // one 128 x 256 fp32 tile
@@ -1054,32 +1025,54 @@ const StreamKWs* get_ws(cudaStream_t stream) {
   return &g_ws[key];
 }
 
-// Stream-K pays when the classic schedule leaves SMs idle (few tiles) or ends on a ragged wave:
-// compare ceil(tiles / U) * nk against tiles * nk / U k-blocks per CTA (+ a fix-up allowance).
-bool want_stream_k(long long tiles, int nk, int units, bool accumulate) {
-  static int env = -2;
-  if (env == -2) {
-    const char* e = std::getenv("SKY_GEMM_STREAMK");
-    env = e ? std::atoi(e) : -1;
+// Stream-K is opt-in (SKY_GEMM_STREAMK=1) and then runs where the classic schedule ends on a
+// ragged wave.  The fix-up of split tiles (park + re-read 128 KB per CTA, finisher wait) eats what
+// the idle SMs would recover on the BERT shapes.  It pays for fp32 `+=` outputs (weight
+// gradients: partials are red.add'ed, no fix-up) with few tiles and a deep K in isolation, but
+// inside the training step those weight gradients run on the side stream NEXT TO the dgrad chain,
+// where an all-SM stream-K grid takes SMs away from the critical path.
+bool want_stream_k(long long tiles, int nk, int units) {
+  return gemm_env().stream_k == 1 && tiles > 0 && nk >= 8 && tiles % units != 0;
+}
+
+// sets the kernel's dynamic shared memory limit once, then launches `ctas` CTAs in clusters of
+// `cluster`
+template <auto Kern, class... Args>
+int launch(int ctas, int cluster, int smem, cudaStream_t stream, const Args&... args) {
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return static_cast<int>(e);
+    attr = true;
   }
-  if (env == 0) return false;
-  if (tiles <= 0 || nk < 8) return false;
-  const long long classic = (tiles + units - 1) / units * nk;
-  const long long streamed = (tiles * nk + units - 1) / units + 6;
-  if (streamed < 4) return false;
-  if (env == 1) return tiles % units != 0;
-  // The fix-up of split tiles (park + re-read 128 KB per CTA, finisher wait) eats what the idle
-  // SMs would recover on the BERT shapes.  It pays for fp32 `+=`
-  // outputs (weight gradients: partials are red.add'ed, no fix-up) with few tiles and a deep K.
-  // ... in isolation.  Inside the training step those weight gradients run on the side stream
-  // NEXT TO the dgrad chain, where an all-SM stream-K grid takes SMs away from the critical path
-  // => opt-in only.
-  (void)accumulate;
-  return false;
+  cudaError_t le = launch_pdl_cluster(Kern, dim3(ctas), dim3(kNumThreads), smem, stream, cluster,
+                                      args...);
+  if (le != cudaSuccess) return static_cast<int>(le);
+  return static_cast<int>(cudaGetLastError());
+}
+
+// the parameters both kernels take straight from GemmArgs
+GemmCommon common_of(const GemmArgs& a) {
+  GemmCommon c;
+  c.M = a.M;
+  c.N = a.N;
+  c.K = a.K;
+  c.bias = a.bias;
+  c.aux = reinterpret_cast<const __nv_bfloat16*>(a.aux);
+  c.ldaux = a.ldaux;
+  c.dropout_p = a.dropout_p;
+  c.rng_state = a.rng_state;
+  c.rng_stream = a.rng_stream;
+  c.signal_flags = a.signal_flags;
+  c.wait_flags = a.wait_flags;
+  c.wait_epoch = a.wait_epoch;
+  c.wait_mult = a.wait_mult;
+  c.error_flag = a.error_flag;
+  return c;
 }
 
 template <int BLOCK_N, bool A_MN, bool B_MN, bool OUT_F32, int CL>
-int launch_inst(const GemmArgs& a, const GemmDev& dev, cudaStream_t stream) {
+int launch_inst(const GemmArgs& a, GemmDev d, cudaStream_t stream) {
   constexpr bool PAIR = CL >= 2;
   constexpr bool MC = CL == 4;
   using C = Cfg<BLOCK_N>;
@@ -1096,71 +1089,46 @@ int launch_inst(const GemmArgs& a, const GemmDev& dev, cudaStream_t stream) {
     rc = make_tmap_bf16_2d(&tmb, a.B, a.N, a.K, a.ldb, 64, BLOCK_K);
   if (rc) return rc;
 
-  GemmDev devp = dev;
-  {
-    if (g_num_sms == 0) {
-      int dev_id = 0;
-      cudaGetDevice(&dev_id);
-      cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev_id);
-    }
-    constexpr int UM = PAIR ? 2 * BLOCK_M : BLOCK_M;
-    const long long m_units = (a.M + UM - 1) / UM;
-    const long long n_blks = (a.N + BLOCK_N - 1) / BLOCK_N;
-    const long long tiles = m_units * (MC ? n_blks / 2 : n_blks);
+  // a scheduling unit is one CTA (128 rows) or one CTA pair (256 rows); MC units span two N tiles
+  constexpr int UNIT_M = PAIR ? 2 * BLOCK_M : BLOCK_M;
+  const long long m_units = (a.M + UNIT_M - 1) / UNIT_M;
+  const long long n_blks = (a.N + BLOCK_N - 1) / BLOCK_N;
+  const long long tiles = m_units * (MC ? n_blks / 2 : n_blks);
+  const int sms = num_sms();
+  const int max_units = sms / CL;
+  int units = max_units;
+  if (a.max_ctas > 0 && units > a.max_ctas / CL) units = a.max_ctas / CL;
+  if (units < 1) units = 1;
+  // stream-K instantiations exist for independent CTAs only (pairs / clusters did not profit)
+  if constexpr (CL == 1) {
     const int nk = (a.K + BLOCK_K - 1) / BLOCK_K;
-    int units = g_num_sms / CL;
-    if (a.max_ctas > 0 && units > a.max_ctas / CL) units = a.max_ctas / CL;
-    if (units < 1) units = 1;
-    bool sk = a.stream_k < 0 ? want_stream_k(tiles, nk, units, a.accumulate) : (a.stream_k != 0);
+    bool sk = a.stream_k < 0 ? want_stream_k(tiles, nk, units) : (a.stream_k != 0);
     // every CTA must own at least 4 k-blocks, the CTA tiles must fit the counter array, a bias
     // must not be added once per partial, and the grid must fit the workspace
     if (tiles * nk < 4LL * units) sk = false;
-    if (m_units * (PAIR ? 2 : 1) * n_blks > kWsMaxCtaTiles || g_num_sms > kWsMaxCtas) sk = false;
+    if (m_units * n_blks > kWsMaxCtaTiles || sms > kWsMaxCtas) sk = false;
     if (a.accumulate && a.bias != nullptr) sk = false;
-    devp.stream_k = 0;
-    devp.ws = nullptr;
-    devp.counters = nullptr;
     if (sk) {
       if (a.accumulate) {
-        devp.stream_k = 1;  // partial sums go straight to the fp32 output with red.add
+        d.stream_k = 1;  // partial sums go straight to the fp32 output with red.add
       } else if (const StreamKWs* w = get_ws(stream)) {
-        devp.stream_k = 1;
-        devp.ws = w->ws;
-        devp.counters = w->counters;
+        d.stream_k = 1;
+        d.ws = w->ws;
+        d.counters = w->counters;
       }
     }
   }
-  // stream-K instantiations exist for independent CTAs only (pairs / clusters did not profit)
-  if (CL != 1) devp.stream_k = 0;
-  void (*kern)(CUtensorMap, CUtensorMap, GemmDev) =
-      gemm_wgmma_kernel<BLOCK_N, A_MN, B_MN, OUT_F32, CL, false>;
-  if constexpr (CL == 1) {
-    if (devp.stream_k) kern = gemm_wgmma_kernel<BLOCK_N, A_MN, B_MN, OUT_F32, CL, true>;
-  }
-  static bool attr_set[2] = {false, false};
-  if (!attr_set[devp.stream_k ? 1 : 0]) {
-    cudaError_t e =
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
-    if (e != cudaSuccess) return static_cast<int>(e);
-    attr_set[devp.stream_k ? 1 : 0] = true;
-  }
-  if (g_num_sms == 0) {
-    int dev_id = 0;
-    cudaGetDevice(&dev_id);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev_id);
-  }
-  constexpr int UNIT_M = PAIR ? 2 * BLOCK_M : BLOCK_M;
-  const int num_tiles =
-      ((a.M + UNIT_M - 1) / UNIT_M) * (((a.N + BLOCK_N - 1) / BLOCK_N) / (MC ? 2 : 1));
-  const int max_units = g_num_sms / CL;
-  int grid = (num_tiles < max_units && !devp.stream_k) ? num_tiles : max_units;
+  int grid = (tiles < max_units && !d.stream_k) ? static_cast<int>(tiles) : max_units;
   if (a.max_ctas > 0 && grid > a.max_ctas / CL) grid = a.max_ctas / CL;
   if (grid < 1) grid = 1;
   grid *= CL;
-  cudaError_t le = launch_pdl_cluster(kern, dim3(grid), dim3(kNumThreads), C::kSmemBytes, stream,
-                              CL, tma, tmb, devp);
-  if (le != cudaSuccess) return static_cast<int>(le);
-  return static_cast<int>(cudaGetLastError());
+  if constexpr (CL == 1) {
+    if (d.stream_k)
+      return launch<gemm_wgmma_kernel<BLOCK_N, A_MN, B_MN, OUT_F32, 1, true>>(
+          grid, 1, C::kSmemBytes, stream, tma, tmb, d);
+  }
+  return launch<gemm_wgmma_kernel<BLOCK_N, A_MN, B_MN, OUT_F32, CL, false>>(
+      grid, CL, C::kSmemBytes, stream, tma, tmb, d);
 }
 
 template <int BLOCK_N, int PAIR>
@@ -1202,28 +1170,16 @@ int gemm_ln_tiles_per_panel(int M, int N, bool force) {
 
 namespace {
 template <int BLOCK_N>
-int launch_ln_inst(const GemmArgs& a, const GemmLnDev& dev, cudaStream_t stream) {
-  using L = LnCfg<BLOCK_N>;
-  using C = typename L::C;
+int launch_ln_inst(const GemmArgs& a, const GemmLnDev& d, cudaStream_t stream) {
   CUtensorMap tma, tmb;
   int rc = make_tmap_bf16_2d(&tma, a.A, a.K, a.M, a.lda, BLOCK_K, BLOCK_M);
   if (rc) return rc;
   rc = make_tmap_bf16_2d(&tmb, a.B, a.K, a.N, a.ldb, BLOCK_K, BLOCK_N);
   if (rc) return rc;
-  void (*kern)(CUtensorMap, CUtensorMap, GemmLnDev) = gemm_ln_wgmma_kernel<BLOCK_N>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         L::kSmemBytes);
-    if (e != cudaSuccess) return static_cast<int>(e);
-    attr_set = true;
-  }
   const int cln = a.N / BLOCK_N;
   const int panels = (a.M + BLOCK_M - 1) / BLOCK_M;
-  cudaError_t le = launch_pdl_cluster(kern, dim3(panels * cln), dim3(kNumThreads), L::kSmemBytes,
-                                      stream, cln, tma, tmb, dev);
-  if (le != cudaSuccess) return static_cast<int>(le);
-  return static_cast<int>(cudaGetLastError());
+  return launch<gemm_ln_wgmma_kernel<BLOCK_N>>(panels * cln, cln, LnCfg<BLOCK_N>::kSmemBytes,
+                                               stream, tma, tmb, d);
 }
 }  // namespace
 
@@ -1238,30 +1194,16 @@ int launch_gemm_ln(const GemmArgs& a, cudaStream_t stream) {
   if (a.aux != nullptr && !a.add_aux) return 908;
   const int bn = a.block_n ? a.block_n : gemm_ln_block_n(a.M, a.N, true);
   if (bn == 0 || (a.N % bn) != 0 || a.N / bn > kLnMaxCluster) return 907;
-  GemmLnDev d;
-  d.M = a.M;
-  d.N = a.N;
-  d.K = a.K;
+  GemmLnDev d{common_of(a)};
   d.y = a.out;
   d.ldy = a.ldo;
   d.z = a.out2;
   d.ldz = a.ldo2;
-  d.bias = a.bias;
-  d.aux = reinterpret_cast<const __nv_bfloat16*>(a.aux);
-  d.ldaux = a.ldaux;
   d.gamma = a.ln_gamma;
   d.beta = a.ln_beta;
   d.mean = a.ln_mean;
   d.rstd = a.ln_rstd;
   d.eps = a.ln_eps;
-  d.dropout_p = a.dropout_p;
-  d.rng_state = a.rng_state;
-  d.rng_stream = a.rng_stream;
-  d.signal_flags = a.signal_flags;
-  d.wait_flags = a.wait_flags;
-  d.wait_epoch = a.wait_epoch;
-  d.wait_mult = a.wait_mult;
-  d.error_flag = a.error_flag;
   if (bn == 256) return launch_ln_inst<256>(a, d, stream);
   if (bn == 128) return launch_ln_inst<128>(a, d, stream);
   return 905;
@@ -1274,35 +1216,18 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   if (a.a_mn && (a.M % 8) != 0) return 902;
   if (a.dropout_p > 0.f && a.rng_state == nullptr) return 903;
   if (a.accumulate && !a.out_f32) return 904;
-  GemmDev d;
-  d.M = a.M;
-  d.N = a.N;
-  d.K = a.K;
+  GemmDev d{common_of(a)};  // no stream-K until launch_inst picks it
   d.out = a.out;
   d.out2 = a.out2;
-  d.bias = a.bias;
-  d.aux = reinterpret_cast<const __nv_bfloat16*>(a.aux);
   d.ldo = a.ldo;
   d.ldo2 = a.ldo2;
-  d.ldaux = a.ldaux;
   d.act = a.act;
   d.add_aux = a.add_aux ? 1 : 0;
   d.accumulate = a.accumulate ? 1 : 0;
-  d.dropout_p = a.dropout_p;
-  d.rng_state = a.rng_state;
-  d.rng_stream = a.rng_stream;
-  d.signal_flags = a.signal_flags;
-  d.wait_flags = a.wait_flags;
-  d.wait_epoch = a.wait_epoch;
-  d.wait_mult = a.wait_mult;
-  d.error_flag = a.error_flag;
   d.debug = a.debug;
-  d.stream_k = 0;
-  d.ws = nullptr;
-  d.counters = nullptr;
   const int bn = a.block_n ? a.block_n : gemm_pick_block_n(a.M, a.N);
-  const bool auto_quad = a.pair < 0 && a.block_n == 0 && gemm_pick_quad(a.M, a.N, a.K);
-  const bool pair = a.pair < 0 ? (auto_quad || gemm_pick_pair(a.M, a.N, a.K)) : (a.pair != 0);
+  const bool auto_quad = a.pair < 0 && a.block_n == 0 && pick_quad();
+  const bool pair = a.pair < 0 ? (auto_quad || pick_pair(a.M)) : (a.pair != 0);
   if (pair) {
     // two pairs + A multicast needs an even number of N tiles
     const bool quad = (a.pair == 2 || auto_quad) &&

@@ -473,6 +473,23 @@ __device__ __forceinline__ uint64_t dropout_seed(const uint64_t* rng_state, uint
   return splitmix64(rng_state[0] + 0x632BE59BD9B4E019ull * (rng_state[1] + 1)) ^
          (static_cast<uint64_t>(stream) << 32);
 }
+// Dropout parameters of one launch.  The seed is read only when p > 0: rng_state may be null
+// otherwise.
+struct Dropout {
+  bool on;
+  uint64_t seed;
+  uint32_t thr16;  // p * 65536
+  float scale;     // 1 / (1 - p) for kept elements
+};
+__device__ __forceinline__ Dropout dropout_of(float p, const uint64_t* rng_state, uint32_t stream) {
+  Dropout d{p > 0.f, 0, 0, 1.f};
+  if (d.on) {
+    d.seed = dropout_seed(rng_state, stream);
+    d.thr16 = static_cast<uint32_t>(p * 65536.f);
+    d.scale = 1.f / (1.f - p);
+  }
+  return d;
+}
 // keep-mask for 4 consecutive elements starting at element index `idx4*4`; thr16 = p * 65536.
 __device__ __forceinline__ uint32_t dropout_keep4(uint64_t seed, uint64_t idx4, uint32_t thr16) {
   const uint64_t r = splitmix64(seed ^ (idx4 * 0xD1342543DE82EF95ull));

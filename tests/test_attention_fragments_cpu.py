@@ -54,7 +54,9 @@ def _ptxas(src_path, tmp_path):
             continue
         m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", line)
         if m and current:
-            out.setdefault(current, {})["spill"] = int(m.group(1)) + int(m.group(2))
+            props = out.setdefault(current, {})
+            props["spill_stores"], props["spill_loads"] = int(m.group(1)), int(m.group(2))
+            props["spill"] = props["spill_stores"] + props["spill_loads"]
         m = re.search(r"Used (\d+) registers", line)
         if m and current:
             out.setdefault(current, {})["regs"] = int(m.group(1))

@@ -5,9 +5,11 @@
 
 ``dump`` imports the package from TREE (a source tree with a built extension), runs every GEMM the
 BERT-large training step issues at its shapes (32 x 128 tokens) on seeded inputs, plus the
-dropout, tanh / fp32 and ragged variants, and stores each output's raw bits as DIR/<name>.npy.
-``compare`` reports, per output, whether the bits agree and the largest difference.  The GEMM +
-LayerNorm kernel is left out: its row statistics may legitimately differ in the last bit.
+dropout, tanh / fp32 and ragged variants, the GEMM + LayerNorm kernel (y, z, mean and rstd at
+K = 1024 and 4096, with and without dropout, at BLOCK_N = 256 and 128) and the opt-in schedules
+(CTA pairs, 4-CTA clusters, stream-K) with a bf16 epilogue and with fp32 accumulation, and stores
+each output's raw bits as DIR/<name>.npy.  ``compare`` reports, per output, whether the bits agree
+and the largest difference.
 """
 from __future__ import annotations
 
@@ -53,6 +55,21 @@ def dump(root: str, out_dir: str) -> None:
         outs[f"{name}_wgrad"] = dw.clone()
         nat.gemm(dy, act, a_mn=True, b_mn=True, out=dw, accumulate=True)
         outs[f"{name}_wgrad_acc"] = dw
+    for name, kw in {"pair1": dict(pair=1), "pair2": dict(pair=2),
+                     "streamk": dict(pair=0, stream_k=1)}.items():
+        outs[f"qkv_fwd_{name}"] = nat.gemm(x, wqkv, bias=bqkv, **kw)
+        dw = outs["w1_wgrad"].clone()
+        nat.gemm(dh, x, a_mn=True, b_mn=True, out=dw, accumulate=True, **kw)
+        outs[f"w1_wgrad_acc_{name}"] = dw
+    gamma = 1 + 0.1 * torch.randn(H, device="cuda", generator=g)
+    beta = 0.1 * torch.randn(H, device="cuda", generator=g)
+    for k, (a_in, w) in {1024: (x, wo), 4096: (inter, w2)}.items():
+        for p in (0.0, 0.1):
+            for bn in (256, 128):
+                res = nat.gemm_ln(a_in, w, gamma, beta, bias=bo, residual=x1, dropout_p=p, rng=rng,
+                                  rng_stream=5, block_n=bn)
+                tag = f"ln_k{k}{'_dropout' if p else ''}_bn{bn}"
+                outs.update({f"{tag}_{n}": v for n, v in zip(("y", "z", "mean", "rstd"), res)})
     outs["pooler_tanh_f32"] = nat.gemm(x[:32], wo, bias=bo, act=nat.ACT_TANH, out_dtype=torch.float32)
     outs["ragged_gelu"] = nat.gemm(x[:4000], w1[:1000], bias=b1[:1000], act=nat.ACT_GELU)
     torch.cuda.synchronize()
@@ -76,7 +93,7 @@ def compare(a: str, b: str) -> int:
         fy = np.load(os.path.join(b, n + ".f32.npy"))
         diff = float(np.nanmax(np.abs(fx - fy))) if fx.shape == fy.shape else float("nan")
         ndiff = int((x != y).sum()) if x.shape == y.shape else -1
-        print(f"{n:24s} {'bit-identical' if same else 'DIFFERENT'}  elements differing {ndiff}"
+        print(f"{n:28s} {'bit-identical' if same else 'DIFFERENT'}  elements differing {ndiff}"
               f"  max |diff| {diff:.3g}")
         bad += not same
     print("all bit-identical" if not bad else f"{bad} of {len(names)} outputs differ")
