@@ -270,6 +270,26 @@ void classify_eval(uintptr_t logits, int ldl, uintptr_t labels, int M, int C,
                                   ignore_index, P<sky::EvalAccum>(acc), S(stream)),
         "classify_eval");
 }
+// returns the number of kernels launched (launch accounting in ops/native.py)
+int vocab_ce(uintptr_t logits, long long ldl, uintptr_t labels, int M, int V,
+              long long ignore_index, uintptr_t dlogits, float grad_scale, uintptr_t loss_out,
+              uintptr_t loss_acc, uintptr_t acc, uintptr_t workspace, uintptr_t stream) {
+  sky::VocabCeArgs a;
+  a.logits = P<const void>(logits);
+  a.ldl = ldl;
+  a.labels = P<const int64_t>(labels);
+  a.M = M;
+  a.V = V;
+  a.ignore_index = ignore_index;
+  a.dlogits = P<void>(dlogits);
+  a.grad_scale = grad_scale;
+  a.loss_out = P<float>(loss_out);
+  a.loss_acc = P<float>(loss_acc);
+  a.acc = P<sky::VocabEvalAccum>(acc);
+  a.workspace = P<void>(workspace);
+  check(sky::launch_vocab_ce(a, S(stream)), "vocab_ce");
+  return sky::vocab_ce_launches(a);
+}
 
 // descriptors: list of (p, g, mom, p_bf16, numel) -> packed host bytes to upload once
 py::bytes pack_sgd_descriptors(
@@ -484,6 +504,12 @@ PYBIND11_MODULE(_cuda, m) {
         py::arg("M"), py::arg("C"), py::arg("ignore_index"), py::arg("acc"),
         py::arg("stream") = 0);
   m.def("eval_max_classes", []() { return sky::kEvalMaxClasses; });
+  m.def("vocab_ce", &vocab_ce, py::arg("logits"), py::arg("ldl"), py::arg("labels"), py::arg("M"),
+        py::arg("V"), py::arg("ignore_index") = -100, py::arg("dlogits") = 0,
+        py::arg("grad_scale") = 1.f, py::arg("loss_out") = 0, py::arg("loss_acc") = 0,
+        py::arg("acc") = 0, py::arg("workspace") = 0, py::arg("stream") = 0);
+  m.def("vocab_ce_workspace_bytes", [](int M) { return sky::vocab_ce_workspace_bytes(M); });
+  m.def("vocab_ce_max_v", []() { return sky::kVocabCeMaxV; });
   m.def("pack_sgd_descriptors", &pack_sgd_descriptors);
   m.def("sgd_multi", &sgd_multi, py::arg("d_tensors"), py::arg("n"), py::arg("max_numel"),
         py::arg("lr"), py::arg("momentum") = 0.f, py::arg("weight_decay") = 0.f,

@@ -232,6 +232,46 @@ constexpr int kEvalMaxClasses = 1024;
 int launch_classify_eval(const float* logits, int ldl, const int64_t* labels, int M, int C,
                          long long ignore_index, EvalAccum* acc, cudaStream_t stream);
 
+// Vocabulary cross entropy over bf16 logits [M, V] (row stride ldl), the masked-language-model
+// loss.  Rows labelled ignore_index are neither read nor counted; n_valid = the other rows.
+// Training mode (dlogits != null, acc == null):
+//   dlogits = (softmax - onehot) * grad_scale / n_valid as bf16, with row stride ldl; it may be
+//   the logits buffer itself (in place), otherwise it must not overlap it.  Ignored rows get an
+//   exact 0.  loss_out[0] = mean loss, loss_acc[0] += mean * grad_scale (either may be null).
+//   n_valid == 0 gives loss 0 and an all-zero gradient (torch's mean reduction gives NaN).  A
+//   label outside [0, V) that is not ignore_index makes the loss NaN and its gradient row 0.
+// Eval mode (acc != null, dlogits == null): adds {fp64 loss sum, labelled rows, top-1 correct,
+//   invalid labels} into *acc; argmax as torch.argmax (first maximum, NaN is the maximum).
+// One CTA per row reads the row from HBM once into shared memory; per-row results are summed by
+// one CTA in a fixed order (no float atomics: graph replays are bit-identical); no host sync.
+// Launches: 3 in training mode, 2 in eval mode (vocab_ce_launches).  workspace: vocab_ce_workspace_bytes(M), any
+// contents; an empty batch (M == 0) may pass null data pointers.  Errors: 950 V outside [1, kVocabCeMaxV], 951 bad shape / null pointer, 952 not
+// exactly one of dlogits / acc, 953 dlogits partially overlaps logits.
+struct VocabEvalAccum {
+  double loss_sum;
+  unsigned long long count;    // labelled rows with a label in [0, V)
+  unsigned long long correct;  // ... whose argmax is the label
+  unsigned long long invalid;  // rows whose label is neither ignore_index nor in [0, V)
+};
+constexpr int kVocabCeMaxV = 98304;  // the bf16 row must fit in shared memory (192 KiB)
+struct VocabCeArgs {
+  const void* logits = nullptr;  // bf16
+  long long ldl = 0;
+  const int64_t* labels = nullptr;
+  int M = 0, V = 0;
+  long long ignore_index = -100;
+  void* dlogits = nullptr;       // bf16, training mode
+  float grad_scale = 1.f;
+  float* loss_out = nullptr;
+  float* loss_acc = nullptr;
+  VocabEvalAccum* acc = nullptr;  // eval mode
+  void* workspace = nullptr;
+};
+size_t vocab_ce_workspace_bytes(int M);
+int launch_vocab_ce(const VocabCeArgs& a, cudaStream_t stream);
+// kernels a successful launch_vocab_ce(a) issues: 3 (training), 2 (eval), fewer when M == 0
+int vocab_ce_launches(const VocabCeArgs& a);
+
 // ---------------------------------------------------------------------------------------------
 // Optimizer / parameter maintenance
 // ---------------------------------------------------------------------------------------------

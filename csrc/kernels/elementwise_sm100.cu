@@ -762,6 +762,234 @@ classify_eval_kernel(const float* __restrict__ logits, long long ldl,
 }
 
 // ------------------------------------------------------------------------------------------
+// Vocabulary cross entropy over bf16 logits [M, V] (masked-language-model loss).
+//   vocab_ce_count_kernel     1 CTA: n_valid = #labels != ignore_index (training mode only)
+//   vocab_ce_row_kernel       1 CTA per row: the row is read from HBM once into shared memory,
+//                             max (argmax) / exp-sum / loss from there, and in training mode the
+//                             bf16 gradient is written from the shared copy (may alias the logits)
+//   vocab_ce_finalize_kernel  1 CTA: the per-row results summed in a fixed order (fp64), added
+//                             into loss_acc (training) or the VocabEvalAccum (eval)
+// Rows whose label is ignore_index are not read at all.  No float atomics anywhere: graph replays
+// are bit-identical.
+// ------------------------------------------------------------------------------------------
+constexpr int kVceThreads = 512;
+constexpr int kVceWarps = kVceThreads / 32;
+constexpr int kVceFinThreads = 1024;
+enum : int { kVceCounted = 1, kVceCorrect = 2, kVceInvalid = 4 };
+
+__global__ void __launch_bounds__(kVceFinThreads)
+vocab_ce_count_kernel(const int64_t* __restrict__ labels, int M, long long ignore_index,
+                      int* __restrict__ n_valid) {
+  __shared__ int red[kVceFinThreads / 32];
+  int n = 0;
+  for (int m = threadIdx.x; m < M; m += blockDim.x) n += labels[m] != ignore_index ? 1 : 0;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = n;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int t = 0;
+    for (int w = 0; w < kVceFinThreads / 32; ++w) t += red[w];
+    *n_valid = t;
+  }
+}
+
+__device__ __forceinline__ float bf16_at(uint4 v, int j) {
+  const __nv_bfloat16* h = reinterpret_cast<const __nv_bfloat16*>(&v);
+  return __bfloat162float(h[j]);
+}
+
+// kEval: argmax + counters, no gradient.  kVec: the row start is 16-byte aligned (16 B loads /
+// stores for the first V/8*8 columns, scalar tail); otherwise every access is scalar.
+template <bool kEval, bool kVec>
+__global__ void __launch_bounds__(kVceThreads)
+vocab_ce_row_kernel(const __nv_bfloat16* logits, long long ldl, const int64_t* __restrict__ labels,
+                    int V, long long ignore_index, __nv_bfloat16* dlogits, float grad_scale,
+                    const int* __restrict__ n_valid, double* __restrict__ row_loss,
+                    int* __restrict__ row_flags) {
+  extern __shared__ __align__(16) unsigned char vce_smem[];
+  __nv_bfloat16* row = reinterpret_cast<__nv_bfloat16*>(vce_smem);
+  __shared__ float red_v[kVceWarps];
+  __shared__ int red_i[kVceWarps];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const long long m = blockIdx.x;
+  const long long lab = labels[m];
+  const __nv_bfloat16* src = logits + m * ldl;
+  const int V8 = kVec ? (V / 8) * 8 : 0;
+
+  if (lab == ignore_index) {  // not read; zero gradient, nothing counted
+    if (!kEval) {
+      __nv_bfloat16* dst = dlogits + m * ldl;
+      for (int c = tid * 8; c < V8; c += kVceThreads * 8)
+        *reinterpret_cast<uint4*>(dst + c) = make_uint4(0, 0, 0, 0);
+      for (int c = V8 + tid; c < V; c += kVceThreads) dst[c] = __float2bfloat16(0.f);
+    }
+    if (tid == 0) {
+      row_loss[m] = 0.0;
+      row_flags[m] = 0;
+    }
+    return;
+  }
+
+  // pass 1: HBM -> shared memory, thread-local max (eval: argmax candidate as in classify_eval)
+  float mx = -INFINITY;
+  int arg = V;  // no candidate yet
+  auto take = [&](float v, int c) {
+    if (kEval) {
+      if (arg == V || eval_better(v, c, mx, arg)) {
+        mx = v;
+        arg = c;
+      }
+    } else {
+      mx = fmaxf(mx, v);
+    }
+  };
+  for (int c = tid * 8; c < V8; c += kVceThreads * 8) {
+    const uint4 v = *reinterpret_cast<const uint4*>(src + c);
+    *reinterpret_cast<uint4*>(row + c) = v;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) take(bf16_at(v, j), c + j);
+  }
+  for (int c = V8 + tid; c < V; c += kVceThreads) {
+    const __nv_bfloat16 v = src[c];
+    row[c] = v;
+    take(__bfloat162float(v), c);
+  }
+  // block max / argmax: fixed xor pattern, then the warps' results in warp order
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float omx = __shfl_xor_sync(0xffffffffu, mx, o);
+    if (kEval) {
+      const int oarg = __shfl_xor_sync(0xffffffffu, arg, o);
+      if (oarg < V && (arg == V || eval_better(omx, oarg, mx, arg))) {
+        mx = omx;
+        arg = oarg;
+      }
+    } else {
+      mx = fmaxf(mx, omx);
+    }
+  }
+  if (lane == 0) {
+    red_v[warp] = mx;
+    red_i[warp] = arg;
+  }
+  __syncthreads();  // also publishes the shared row
+  mx = red_v[0];
+  arg = red_i[0];
+  for (int w = 1; w < kVceWarps; ++w) {
+    if (kEval) {
+      if (red_i[w] < V && (arg == V || eval_better(red_v[w], red_i[w], mx, arg))) {
+        mx = red_v[w];
+        arg = red_i[w];
+      }
+    } else {
+      mx = fmaxf(mx, red_v[w]);
+    }
+  }
+  __syncthreads();  // red_v is reused below
+
+  // pass 2: sum exp(l - max) from shared memory
+  const int V8s = (V / 8) * 8;  // the shared row is always 16-byte aligned
+  float se = 0.f;
+  for (int c = tid * 8; c < V8s; c += kVceThreads * 8) {
+    const uint4 v = *reinterpret_cast<const uint4*>(row + c);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) se += __expf(bf16_at(v, j) - mx);
+  }
+  for (int c = V8s + tid; c < V; c += kVceThreads) se += __expf(__bfloat162float(row[c]) - mx);
+  se = warp_sum(se);
+  if (lane == 0) red_v[warp] = se;
+  __syncthreads();
+  se = 0.f;
+  for (int w = 0; w < kVceWarps; ++w) se += red_v[w];
+  const float lse = mx + logf(se);
+  const bool valid = lab >= 0 && lab < V;
+
+  if (!kEval) {
+    // dlogits = (softmax - onehot) * grad_scale / n_valid; an out-of-range label (neither
+    // ignore_index nor in [0, V)) gets a zero gradient and a NaN loss
+    const int nv = *n_valid;
+    const float coef = valid ? grad_scale / static_cast<float>(nv) : 0.f;
+    __nv_bfloat16* dst = dlogits + m * ldl;
+    for (int c = tid * 8; c < V8; c += kVceThreads * 8) {
+      const uint4 v = *reinterpret_cast<const uint4*>(row + c);
+      uint4 o;
+      __nv_bfloat16* oh = reinterpret_cast<__nv_bfloat16*>(&o);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float p = __expf(bf16_at(v, j) - lse) - (c + j == lab ? 1.f : 0.f);
+        oh[j] = __float2bfloat16(p * coef);
+      }
+      *reinterpret_cast<uint4*>(dst + c) = o;
+    }
+    for (int c = V8 + tid; c < V; c += kVceThreads) {
+      const float p = __expf(__bfloat162float(row[c]) - lse) - (c == lab ? 1.f : 0.f);
+      dst[c] = __float2bfloat16(p * coef);
+    }
+  }
+  if (tid == 0) {
+    if (valid) {
+      row_loss[m] = static_cast<double>(lse - __bfloat162float(row[lab]));
+      row_flags[m] = kVceCounted | (kEval && arg == lab ? kVceCorrect : 0);
+    } else {
+      row_loss[m] = kEval ? 0.0 : static_cast<double>(NAN);
+      row_flags[m] = kVceInvalid;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kVceFinThreads)
+vocab_ce_finalize_kernel(const double* __restrict__ row_loss, const int* __restrict__ row_flags,
+                         int M, const int* __restrict__ n_valid, float grad_scale,
+                         float* __restrict__ loss_out, float* __restrict__ loss_acc,
+                         VocabEvalAccum* __restrict__ acc) {
+  __shared__ double red[kVceFinThreads];
+  __shared__ int cnt[3][kVceFinThreads / 32];
+  double s = 0.0;
+  int counted = 0, correct = 0, invalid = 0;
+  for (int m = threadIdx.x; m < M; m += blockDim.x) {
+    s += row_loss[m];
+    const int f = row_flags[m];
+    counted += f & kVceCounted ? 1 : 0;
+    correct += f & kVceCorrect ? 1 : 0;
+    invalid += f & kVceInvalid ? 1 : 0;
+  }
+  red[threadIdx.x] = s;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    counted += __shfl_xor_sync(0xffffffffu, counted, o);
+    correct += __shfl_xor_sync(0xffffffffu, correct, o);
+    invalid += __shfl_xor_sync(0xffffffffu, invalid, o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    cnt[0][threadIdx.x >> 5] = counted;
+    cnt[1][threadIdx.x >> 5] = correct;
+    cnt[2][threadIdx.x >> 5] = invalid;
+  }
+  __syncthreads();
+  for (int k = kVceFinThreads / 2; k > 0; k >>= 1) {
+    if (threadIdx.x < k) red[threadIdx.x] += red[threadIdx.x + k];
+    __syncthreads();
+  }
+  if (threadIdx.x != 0) return;
+  if (acc != nullptr) {
+    unsigned long long c[3] = {0, 0, 0};
+    for (int k = 0; k < 3; ++k)
+      for (int w = 0; w < kVceFinThreads / 32; ++w) c[k] += cnt[k][w];
+    acc->loss_sum += red[0];
+    acc->count += c[0];
+    acc->correct += c[1];
+    acc->invalid += c[2];
+  } else {
+    // no labelled row: the loss is 0 (torch's mean over an empty selection would be NaN)
+    const int nv = *n_valid;
+    const float mean = nv > 0 ? static_cast<float>(red[0] / nv) : 0.f;
+    if (loss_out != nullptr) loss_out[0] = mean;
+    if (loss_acc != nullptr) loss_acc[0] += mean * grad_scale;
+  }
+}
+
+// ------------------------------------------------------------------------------------------
 // Optimizer
 // ------------------------------------------------------------------------------------------
 // kScalars: lr and the clip coefficient come from the device-side OptimScalars (schedule / global
@@ -1283,6 +1511,76 @@ int launch_classify_eval(const float* logits, int ldl, const int64_t* labels, in
   if (M <= 0) return 0;
   classify_eval_kernel<<<1, kEvalWarps * 32, 0, stream>>>(logits, ldl, labels, M, C, ignore_index,
                                                           acc);
+  SKY_LAUNCH_CHECK();
+}
+
+size_t vocab_ce_workspace_bytes(int M) {
+  return static_cast<size_t>(M > 0 ? M : 0) * (sizeof(double) + sizeof(int)) + 16;
+}
+
+namespace {
+template <bool kEval, bool kVec>
+int launch_vocab_ce_rows(const VocabCeArgs& a, size_t smem, double* row_loss, int* row_flags,
+                         const int* n_valid, cudaStream_t stream) {
+  auto kern = vocab_ce_row_kernel<kEval, kVec>;
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         kVocabCeMaxV * 2);
+    if (e != cudaSuccess) return static_cast<int>(e);
+    attr = true;
+  }
+  kern<<<a.M, kVceThreads, smem, stream>>>(
+      reinterpret_cast<const __nv_bfloat16*>(a.logits), a.ldl, a.labels, a.V, a.ignore_index,
+      reinterpret_cast<__nv_bfloat16*>(a.dlogits), a.grad_scale, n_valid, row_loss, row_flags);
+  return static_cast<int>(cudaGetLastError());
+}
+}  // namespace
+
+int vocab_ce_launches(const VocabCeArgs& a) {
+  if (a.acc != nullptr) return a.M > 0 ? 2 : 0;
+  return a.M > 0 ? 3 : 2;
+}
+
+int launch_vocab_ce(const VocabCeArgs& a, cudaStream_t stream) {
+  const bool eval = a.acc != nullptr;
+  if (a.V < 1 || a.V > kVocabCeMaxV) return 950;
+  // an empty batch (M == 0) may come with null data pointers: nothing is read or written there
+  if (a.M < 0 || a.ldl < a.V || a.workspace == nullptr) return 951;
+  if (a.M > 0 && (a.logits == nullptr || a.labels == nullptr)) return 951;
+  // exactly one of gradient (training) / accumulator (eval)
+  if (eval ? a.dlogits != nullptr : (a.M > 0 && a.dlogits == nullptr)) return 952;
+  if (a.M > 0 && a.dlogits != nullptr && a.dlogits != a.logits) {
+    // a separate gradient buffer must not overlap the logits (in place is fine: each row is
+    // staged in shared memory before it is overwritten)
+    const char* l0 = static_cast<const char*>(a.logits);
+    const char* d0 = static_cast<const char*>(a.dlogits);
+    const long long bytes = (static_cast<long long>(a.M > 0 ? a.M - 1 : 0) * a.ldl + a.V) * 2;
+    if (d0 < l0 + bytes && l0 < d0 + bytes) return 953;
+  }
+  char* ws = static_cast<char*>(a.workspace);
+  double* row_loss = reinterpret_cast<double*>(ws);
+  int* row_flags = reinterpret_cast<int*>(ws + static_cast<size_t>(a.M) * sizeof(double));
+  int* n_valid = row_flags + a.M;
+  if (!eval) {
+    vocab_ce_count_kernel<<<1, kVceFinThreads, 0, stream>>>(a.labels, a.M, a.ignore_index,
+                                                            n_valid);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return static_cast<int>(e);
+  }
+  if (a.M > 0) {
+    const size_t smem = ((static_cast<size_t>(a.V) * 2 + 15) / 16) * 16;
+    const bool vec = (reinterpret_cast<uintptr_t>(a.logits) % 16 == 0) && (a.ldl % 8 == 0) &&
+                     (eval || reinterpret_cast<uintptr_t>(a.dlogits) % 16 == 0);
+    int rc = eval ? (vec ? launch_vocab_ce_rows<true, true>(a, smem, row_loss, row_flags, n_valid, stream)
+                         : launch_vocab_ce_rows<true, false>(a, smem, row_loss, row_flags, n_valid, stream))
+                  : (vec ? launch_vocab_ce_rows<false, true>(a, smem, row_loss, row_flags, n_valid, stream)
+                         : launch_vocab_ce_rows<false, false>(a, smem, row_loss, row_flags, n_valid, stream));
+    if (rc != 0) return rc;
+  }
+  if (eval && a.M == 0) return 0;
+  vocab_ce_finalize_kernel<<<1, kVceFinThreads, 0, stream>>>(
+      row_loss, row_flags, a.M, n_valid, a.grad_scale, a.loss_out, a.loss_acc, a.acc);
   SKY_LAUNCH_CHECK();
 }
 

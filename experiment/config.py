@@ -39,12 +39,20 @@ MAX_GRAD_NORM = float(os.getenv("MAX_GRAD_NORM")) if os.getenv("MAX_GRAD_NORM") 
 EVAL_EVERY = int(os.getenv("EVAL_EVERY")) if os.getenv("EVAL_EVERY") else None
 EVAL_SAMPLES = int(os.getenv("EVAL_SAMPLES", "256"))
 TINY = os.getenv("TINY", "0") == "1"                          # shrink the geometry for CPU smoke runs
+# TASK=mlm: masked-language-model pretraining (RoBERTa style, no next-sentence head) on the
+# learnable SynthMLMDataset with a BertTailForMaskedLM head and MaskedLMLoss; the vocabulary is
+# padded to a multiple of 8 (30522 -> 30528) for the head's GEMMs.  Default: classification
+TASK = os.getenv("TASK", "cls")
+if TASK not in ("cls", "mlm"):
+    raise ValueError("TASK must be 'cls' or 'mlm', got {!r}".format(TASK))
 
 _config = BertConfig.bert_large()                              # wwm_uncased_L-24_H-1024_A-16 geometry
 if TINY:
     _config = BertConfig(1000, hidden_size=64, num_hidden_layers=LAYER_NUM, num_attention_heads=4,
                          intermediate_size=128, max_position_embeddings=128)
 _SEQ = int(os.getenv("SEQ_LEN", "128" if not TINY else "16"))
+if TASK == "mlm":
+    _config.vocab_size = (_config.vocab_size + 7) // 8 * 8
 
 _ENCODER = [
     dict(layer_type="BertLayer_Head", config=_config.__dict__),
@@ -52,16 +60,16 @@ _ENCODER = [
     dict(layer_type="BertLayer_Tail", config=_config.__dict__),
 ] * LAYER_NUM
 
-model_config = (
-    [dict(layer_type="BertEmbeddings", config=_config.__dict__)]
-    + _ENCODER
-    + [
-        dict(layer_type="BertPooler", config=_config.__dict__),
-        dict(layer_type="BertTailForClassification",
-             hidden_dropout_prob=_config.hidden_dropout_prob,
-             hidden_size=_config.hidden_size, num_classes=3),
-    ]
-)
+_TAIL = [
+    dict(layer_type="BertPooler", config=_config.__dict__),
+    dict(layer_type="BertTailForClassification",
+         hidden_dropout_prob=_config.hidden_dropout_prob,
+         hidden_size=_config.hidden_size, num_classes=3),
+]
+if TASK == "mlm":
+    _TAIL = [dict(layer_type="BertTailForMaskedLM", config=_config.__dict__)]
+
+model_config = [dict(layer_type="BertEmbeddings", config=_config.__dict__)] + _ENCODER + _TAIL
 
 rpc_config = dict(MASTER_ADDR="127.0.0.1", MASTER_PORT="29500", GLOO_SOCKET_IFNAME="ipogif0")
 
@@ -93,7 +101,14 @@ data_config = dict(
                      max_seq_length=_SEQ, vocab_size=_config.vocab_size, num_classes=3, seed=0),
     dataloader_cfg=dict(batch_size=BATCH_SIZE, shuffle=True, num_workers=0, drop_last=True),
 )
-if EVAL_EVERY is not None:
+if TASK == "mlm":
+    data_config["dataset_cfg"] = dict(type="SynthMLMDataset", num_samples=BATCH_SIZE * (MAX_ITERS + 2),
+                                      max_seq_length=_SEQ, vocab_size=_config.vocab_size, seed=0)
+    if EVAL_EVERY is not None:  # the held-out split: another seed of the same task
+        data_config["eval_datasets"] = dict(
+            dev=dict(type="SynthMLMDataset", num_samples=EVAL_SAMPLES, max_seq_length=_SEQ,
+                     vocab_size=_config.vocab_size, seed=1))
+elif EVAL_EVERY is not None:
     # a learnable task (label = first token after [CLS] mod 3) for training and the held-out split,
     # so that the dev accuracy measures something; random labels stay at chance
     data_config["dataset_cfg"]["label_rule"] = "token"
@@ -135,7 +150,7 @@ train_config = dict(
     lr_schedule_cfg=(dict(type=LR_SCHEDULE, warmup_steps=WARMUP_STEPS, total_steps=TOTAL_STEPS)
                      if LR_SCHEDULE else None),
     grad_clip_cfg=dict(max_norm=MAX_GRAD_NORM) if MAX_GRAD_NORM is not None else None,
-    loss_cfg=dict(type="CrossEntropyLoss"),
+    loss_cfg=dict(type="MaskedLMLoss" if TASK == "mlm" else "CrossEntropyLoss"),
     runner_cfg=dict(max_epochs=1, max_iters=MAX_ITERS, micro_batches=MICRO_BATCHES),
     hook_config=[dict(type="StopHook", root=_LOG_ROOT), dict(type="DistributedTimerHelperHook")]
     # REALLOCATE_EVERY=N: re-benchmark the devices and re-run the allocator every N iterations,

@@ -2,6 +2,7 @@
 
 * ``SynthMNLIDataset`` - synthetic MNLI-shaped data (three int64 ``[S]`` tensors + a label in
   ``num_classes``): the workload of every benchmark here (there is no network for GLUE).
+* ``SynthMLMDataset`` - a learnable synthetic masked-language-model task (labels ``[S]``).
 * ``RandomMlpDataset`` / ``CIFAR10Dataset`` - parity with scaelum/dataset/dataset.py:14-48.
 """
 from __future__ import annotations
@@ -62,6 +63,82 @@ class SynthMNLIDataset(Dataset):
         else:
             data = (self.input_ids[idx], self.segment_ids[idx], self.input_mask[idx])
         return data, self.labels[idx]
+
+
+def bert_mask(ids: torch.Tensor, maskable: torch.Tensor, mask_id: int, random_low: int,
+              vocab_size: int, mask_prob: float, g: torch.Generator):
+    """BERT masking of one sequence: ``mask_prob`` of the maskable positions (at least one) are
+    labelled with their token; of those 80 % become ``mask_id``, 10 % a random token from
+    ``[random_low, vocab_size)`` and 10 % stay unchanged.  Returns ``(input_ids, labels)`` with
+    -100 on every unlabelled position."""
+    pos = torch.nonzero(maskable, as_tuple=False)[:, 0]
+    labels = torch.full_like(ids, -100)
+    if pos.numel() == 0:
+        return ids.clone(), labels
+    n = max(1, int(round(mask_prob * pos.numel())))
+    chosen = pos[torch.randperm(pos.numel(), generator=g)[:n]]
+    labels[chosen] = ids[chosen]
+    out = ids.clone()
+    r = torch.rand(n, generator=g)
+    out[chosen[r < 0.8]] = mask_id
+    rnd = chosen[(r >= 0.8) & (r < 0.9)]
+    out[rnd] = torch.randint(random_low, vocab_size, (rnd.numel(),), generator=g)
+    return out, labels
+
+
+def _item_generator(seed: int, idx: int) -> torch.Generator:
+    return torch.Generator().manual_seed(int(seed) * 1000003 + int(idx))
+
+
+@DATASET.register_module
+class SynthMLMDataset(Dataset):
+    """Synthetic masked-language-model data that a model can learn: every sequence is
+    ``[CLS] t_1 ... t_{S-2} [SEP]`` with ``t_i = first + (start + i * step) mod (V - first)``, a
+    random ``start`` and a random ``step`` in ``1..max_step``, so a masked token follows from its
+    neighbours.
+    Masking is ``bert_mask``'s (15 % of the body tokens, 80/10/10), deterministic for a given
+    ``(seed, index)``; another ``seed`` draws a held-out split of the same task.
+
+    Items are ``((input_ids, token_type_ids, attention_mask), labels[S])`` (labels -100 where not
+    masked); ``reference_order=True`` yields ``(input_ids, input_mask, segment_ids)`` instead.
+    Vocabularies above 2000 use the BERT ids [CLS] 101, [SEP] 102, [MASK] 103 and body tokens from
+    1000; smaller ones 1, 2, 3 and body tokens from 4."""
+
+    def __init__(self, num_samples: int = 1024, max_seq_length: int = 128,
+                 vocab_size: int = 30528, mask_prob: float = 0.15, seed: int = 0,
+                 reference_order: bool = False, max_step: int = 4):
+        if max_seq_length < 3:
+            raise ValueError("max_seq_length must be at least 3")
+        big = vocab_size > 2000
+        self.cls_id, self.sep_id, self.mask_id = (101, 102, 103) if big else (1, 2, 3)
+        self.first = 1000 if big else 4
+        if vocab_size <= self.first:
+            raise ValueError("vocab_size {} leaves no body tokens".format(vocab_size))
+        self.vocab_size, self.mask_prob, self.seed = vocab_size, mask_prob, seed
+        self.reference_order = reference_order
+        g = torch.Generator().manual_seed(seed)
+        S, span = max_seq_length, vocab_size - self.first
+        start = torch.randint(0, span, (num_samples, 1), generator=g)
+        step = torch.randint(1, max_step + 1, (num_samples, 1), generator=g)
+        body = self.first + (start + torch.arange(S - 2).unsqueeze(0) * step) % span
+        cls = torch.full((num_samples, 1), self.cls_id, dtype=torch.long)
+        sep = torch.full((num_samples, 1), self.sep_id, dtype=torch.long)
+        self.input_ids = torch.cat([cls, body, sep], dim=1)
+        self.input_mask = torch.ones_like(self.input_ids)
+        self.segment_ids = torch.zeros_like(self.input_ids)
+
+    def __len__(self):
+        return self.input_ids.size(0)
+
+    def __getitem__(self, idx):
+        ids = self.input_ids[idx]
+        maskable = torch.ones_like(ids, dtype=torch.bool)
+        maskable[0] = maskable[-1] = False
+        ids, labels = bert_mask(ids, maskable, self.mask_id, self.first, self.vocab_size,
+                                self.mask_prob, _item_generator(self.seed, idx))
+        if self.reference_order:
+            return (ids, self.input_mask[idx], self.segment_ids[idx]), labels
+        return (ids, self.segment_ids[idx], self.input_mask[idx]), labels
 
 
 @DATASET.register_module

@@ -90,9 +90,18 @@ class Estimator:
             mem = (2 * outs + param_scale * params + B * H) * 4 / mb
             return 2.0 * B * H * C, mem, [((B, C), f32)]
         if c is None or lt not in ("BertEmbeddings", "BertLayer_Head", "BertLayer_Body",
-                                   "BertLayer_Tail", "BertPooler"):
+                                   "BertLayer_Tail", "BertPooler", "BertTailForMaskedLM"):
             return None
         H, I, A = c["hidden_size"], c["intermediate_size"], c["num_attention_heads"]
+        if lt == "BertTailForMaskedLM":
+            # transform dense + decoder; every token is decoded, so the decoder dominates (about
+            # 2.5 encoder blocks at BERT-large with a 30K vocabulary)
+            B, S, _ = data[0].shape
+            V = c["vocab_size"]
+            params = H * H + H + 2 * H + V * H + V
+            outs = 3 * B * S * H + 2 * B * S * V   # dense_act, LayerNorm, transform; decoder, layer
+            mem = (2 * outs + param_scale * params + B * S * H + B * S) * 4 / mb
+            return 2.0 * B * S * H * (H + V), mem, [((B, S, V), f32)]
         if lt == "BertEmbeddings":
             B, S = data[0].shape
             params = (c["vocab_size"] + c["max_position_embeddings"] + c["type_vocab_size"]) * H + 2 * H

@@ -8,6 +8,7 @@ Registered names and calling conventions are those of scaelum/model/bert_layers.
     BertLayer_Tail(config)            (inter, attn_out, mask)   -> (hidden, mask)
     BertPooler(config)                (hidden, mask)            -> pooled
     BertTailForClassification(hidden_dropout_prob, hidden_size, num_classes)   pooled -> logits
+    BertTailForMaskedLM(config)       (hidden, mask)            -> logits [B, S, vocab]
 
 Parameter names match the reference (``attention.self.query.weight`` ...), so layer-indexed
 checkpoints interchange.  Every layer has two execution paths behind the same class:
@@ -486,6 +487,57 @@ class BertTailForClassification(nn.Module):
         return logits.view(-1, self.num_classes)
 
 
+class BertPredictionHeadTransform(nn.Module):
+    def __init__(self, config):
+        super().__init__()
+        self.dense_act = LinearActivation(config.hidden_size, config.hidden_size, act=config.hidden_act)
+        self.LayerNorm = BertLayerNorm(config.hidden_size, eps=1e-12)
+
+    def forward(self, hidden_states):
+        return self.LayerNorm(self.dense_act(hidden_states))
+
+
+@LAYER.register_module
+class BertTailForMaskedLM(nn.Module):
+    """Masked-language-model head (HF ``BertLMPredictionHead``): dense + activation + LayerNorm,
+    then a decoder to vocabulary logits.  ``(hidden [B,S,H], mask) -> logits [B,S,V]``; every
+    token is decoded (the layer does not see which positions are masked).
+
+    The decoder weight is a parameter of its own, not tied to the word embeddings.  The native
+    path needs ``H % 8 == 0`` and ``V % 8 == 0`` (GEMM output widths), which is why BERT configs
+    pad the vocabulary (30522 -> 30528); other shapes run the eager path."""
+
+    def __init__(self, config):
+        super().__init__()
+        config = BertConfig.from_dict(config) if isinstance(config, dict) else config
+        self.transform = BertPredictionHeadTransform(config)
+        self.decoder = nn.Linear(config.hidden_size, config.vocab_size)
+        self._native = None
+
+    def _native_params(self):
+        from ..ops.functions import MaskedLMHeadParams
+
+        if self._native is None:
+            object.__setattr__(self, "_native", MaskedLMHeadParams(self))
+        return self._native
+
+    def _supports(self, hidden: torch.Tensor) -> bool:
+        H, V = self.decoder.in_features, self.decoder.out_features
+        return (hidden.dim() == 3 and H % 8 == 0 and V % 8 == 0 and H <= 2048
+                and self.transform.dense_act.act_name in ("gelu", "bias_gelu"))
+
+    def forward(self, hidden_states, attention_mask=None):
+        if _native_enabled(hidden_states) and self._supports(hidden_states):
+            from ..ops.functions import MaskedLMHeadFn
+
+            hp = self._native_params()
+            x = hidden_states.to(torch.bfloat16)
+            if not self.training and not torch.is_grad_enabled():
+                return MaskedLMHeadFn.infer(hp, x)
+            return MaskedLMHeadFn.apply(hp, x, *hp.all_params())
+        return self.decoder(self.transform(hidden_states.float()))
+
+
 def native_param_banks(module: nn.Module):
     """All ParamBanks of `module`'s native layers (created eagerly; used by the fused optimizer).
 
@@ -512,6 +564,8 @@ def native_param_banks(module: nn.Module):
         elif isinstance(m, BertPooler):
             banks.extend(m._native_params().banks)
         elif isinstance(m, BertTailForClassification):
+            banks.extend(m._native_params().banks)
+        elif isinstance(m, BertTailForMaskedLM):
             banks.extend(m._native_params().banks)
         elif isinstance(m, BertLayer_Head):
             banks.extend(_lone_span(m, head=m).params.banks)

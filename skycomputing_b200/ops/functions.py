@@ -681,6 +681,75 @@ class SmallLinearParams:
         return [p for b in self.banks for p in b.params]
 
 
+class MaskedLMHeadParams:
+    """Parameter banks of ``BertTailForMaskedLM``: transform dense (+ GELU), LayerNorm, decoder."""
+
+    def __init__(self, mod):
+        tr = mod.transform
+        self.w_t = ParamBank([tr.dense_act.weight])
+        self.b_t = ParamBank([tr.dense_act.bias], False)
+        self.gamma = ParamBank([tr.LayerNorm.weight], False)
+        self.beta = ParamBank([tr.LayerNorm.bias], False)
+        self.w_dec = ParamBank([mod.decoder.weight])
+        self.b_dec = ParamBank([mod.decoder.bias], False)
+        self.banks = [self.w_t, self.b_t, self.gamma, self.beta, self.w_dec, self.b_dec]
+        self.eps = float(tr.LayerNorm.eps)
+
+    def all_params(self):
+        return [p for b in self.banks for p in b.params]
+
+
+class MaskedLMHeadFn(torch.autograd.Function):
+    """BertTailForMaskedLM on the wgmma GEMM: dense with bias + GELU in the epilogue (the
+    pre-activation kept for backward), LayerNorm, decoder GEMM with bias to bf16 logits.
+    Backward: decoder dgrad GEMM, LayerNorm backward, GELU derivative, transform dgrad GEMM;
+    the weight / bias / LayerNorm parameter gradients go straight into the fp32 bank gradients
+    and follow the same deferral / side-stream policy as the encoder's."""
+
+    @staticmethod
+    def _run(hp: MaskedLMHeadParams, hidden: torch.Tensor, keep: bool):
+        B, S, H = hidden.shape
+        x = hidden.contiguous().view(B * S, H)
+        h1 = torch.empty_like(x) if keep else None
+        t = nat.gemm(x, hp.w_t.shadow(), bias=hp.b_t.master(), act=nat.ACT_GELU, out2=h1)
+        y, mean, rstd = _ln_fwd(t, hp.gamma.master(), hp.beta.master(), hp.eps)
+        logits = nat.gemm(y, hp.w_dec.shadow(), bias=hp.b_dec.master())
+        return logits.view(B, S, -1), (x, h1, t, mean, rstd, y)
+
+    @staticmethod
+    def infer(hp: MaskedLMHeadParams, hidden: torch.Tensor) -> torch.Tensor:
+        """Eval-mode forward without autograd: the same logits, nothing kept for backward."""
+        return MaskedLMHeadFn._run(hp, hidden, False)[0]
+
+    @staticmethod
+    def forward(ctx, hp, hidden, *params):
+        logits, saved = MaskedLMHeadFn._run(hp, hidden, True)
+        ctx.hp, ctx.saved, ctx.shape3 = hp, saved, tuple(hidden.shape)
+        ctx.n_params = len(params)
+        return logits
+
+    @staticmethod
+    def backward(ctx, dlogits):
+        hp = ctx.hp
+        x, h1, t, mean, rstd, y = ctx.saved
+        B, S, H = ctx.shape3
+        g = _flat2d(dlogits)
+        if g.dtype != torch.bfloat16:
+            g = g.to(torch.bfloat16)
+        g = g.contiguous()
+        _wgrad(g, y, hp.w_dec, hp.b_dec)
+        dy = nat.gemm(g, hp.w_dec.shadow(), b_mn=True)
+        dt, _ = nat.layernorm_bwd(dy, t, mean, rstd, hp.gamma.master(), None, None)
+        _ln_pgrad(dy, t, mean, rstd, hp.gamma, hp.beta)
+        dh1 = torch.empty_like(dt)
+        nat.ext().dgelu_mul(dt.data_ptr(), h1.data_ptr(), dh1.data_ptr(), dt.numel(),
+                            torch.cuda.current_stream().cuda_stream)
+        _wgrad(dh1, x, hp.w_t, hp.b_t)
+        dx = nat.gemm(dh1, hp.w_t.shadow(), b_mn=True)
+        ctx.saved = None
+        return (None, dx.view(B, S, H), *([None] * ctx.n_params))
+
+
 class SoftmaxCrossEntropyFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits, labels):

@@ -33,10 +33,12 @@ def available() -> bool:
 
 
 # ---- launch accounting (bench.py reports how many of OUR kernels ran in the timed region) ----
+# kernels per call; -1: the binding returns the number of kernels it launched
 _KERNELS_PER_CALL = {
     "gemm": 1, "layernorm_fwd": 1, "layernorm_bwd": 1, "ln_param_grad": 1, "colsum": 1, "dgelu_mul": 1,
     "attention_fwd": 1, "attention_bwd": 1, "embed_fwd": 1, "embed_bwd": 1,
     "small_linear_fwd": 1, "small_linear_bwd": 2, "softmax_ce": 1, "classify_eval": 1,
+    "vocab_ce": -1,
     "sgd_multi": 1, "adam_multi": 1,
     "grad_sumsq_multi": 1, "optim_finalize": 1,
     "cast_f32_to_bf16": 1, "cast_bf16_to_f32": 1, "advance_counter": 1, "advance_epoch": 1,
@@ -59,7 +61,12 @@ class _CountingExt:
         if fn is None:
             target = getattr(self._mod, name)
             n = _KERNELS_PER_CALL.get(name, 0)
-            if n and callable(target):
+            if n < 0 and callable(target):
+                def fn(*a, __t=target, **k):
+                    launched = __t(*a, **k)
+                    _launches[0] += launched
+                    return launched
+            elif n and callable(target):
                 def fn(*a, __t=target, __n=n, **k):
                     _launches[0] += __n
                     return __t(*a, **k)
@@ -399,6 +406,78 @@ def classify_eval(logits: torch.Tensor, labels: torch.Tensor, accum: torch.Tenso
     ext().classify_eval(logits=logits.data_ptr(), ldl=logits.stride(0),
                         labels=labels.contiguous().data_ptr(), M=M, C=C,
                         ignore_index=int(ignore_index), acc=accum.data_ptr(), stream=_stream())
+
+
+def _vocab_ce_check(logits: torch.Tensor, labels: torch.Tensor):
+    _check(logits, torch.bfloat16, "logits")
+    if logits.dim() != 2:
+        raise ValueError("logits must be 2-D [M, V]")
+    M, V = logits.shape
+    if not labels.is_cuda or labels.dtype != torch.int64 or labels.numel() != M:
+        raise ValueError("labels must be a CUDA int64 tensor with one entry per logits row")
+    if V > ext().vocab_ce_max_v():
+        raise ValueError("vocab_ce stages a logits row in shared memory and supports at most {} "
+                         "classes, got {}".format(ext().vocab_ce_max_v(), V))
+    ws = torch.empty(ext().vocab_ce_workspace_bytes(M), dtype=torch.uint8, device=logits.device)
+    return M, V, labels.reshape(-1).contiguous(), ws
+
+
+def vocab_ce(logits: torch.Tensor, labels: torch.Tensor, grad_scale: float = 1.0,
+             loss_acc: Optional[torch.Tensor] = None, ignore_index: int = -100,
+             in_place: bool = False):
+    """Masked-language-model cross entropy over bf16 logits ``[M, V]`` (row stride may exceed V).
+
+    Returns ``(loss, dlogits)``: the mean loss over the rows whose label is not ``ignore_index``
+    (fp32 ``[1]``) and ``d(loss * grad_scale)/dlogits`` as bf16, 0 on ignored rows; with
+    ``in_place`` the gradient overwrites ``logits``.  ``loss_acc[0] += loss * grad_scale`` when
+    given.  With no labelled row the loss and the gradient are 0, where torch gives NaN.  Three
+    launches, no host synchronisation, deterministic."""
+    M, V, labels, ws = _vocab_ce_check(logits, labels)
+    dlogits = logits if in_place else torch.empty_strided(logits.shape, logits.stride(),
+                                                          dtype=torch.bfloat16,
+                                                          device=logits.device)
+    loss = torch.empty(1, dtype=torch.float32, device=logits.device)
+    ext().vocab_ce(logits=logits.data_ptr(), ldl=logits.stride(0), labels=labels.data_ptr(), M=M,
+                   V=V, ignore_index=int(ignore_index), dlogits=dlogits.data_ptr(),
+                   grad_scale=float(grad_scale), loss_out=loss.data_ptr(),
+                   loss_acc=_ptr(loss_acc), workspace=ws.data_ptr(), stream=_stream())
+    return loss, dlogits
+
+
+class TokenEvalAccumulator:
+    """Device-side token accumulator of one evaluation pass over a vocabulary-sized output:
+    ``{loss_sum (fp64), count, correct, invalid}`` in one int64 buffer (``sky::VocabEvalAccum``).
+
+    ``reset()`` is one memset and ``add()`` two kernel launches of ``vocab_ce`` in eval mode,
+    all capturable into a CUDA graph; ``read()`` is the single device-to-host copy of the pass."""
+
+    def __init__(self, V: int, device=None):
+        if V < 1 or V > ext().vocab_ce_max_v():
+            raise ValueError("TokenEvalAccumulator supports 1 <= V <= {}, got {}".format(
+                ext().vocab_ce_max_v(), V))
+        self.V = int(V)
+        self.buffer = torch.zeros(4, dtype=torch.int64,
+                                  device=device if device is not None else "cuda")
+
+    def reset(self) -> None:
+        self.buffer.zero_()
+
+    def add(self, logits: torch.Tensor, labels: torch.Tensor, ignore_index: int = -100) -> None:
+        logits = logits.detach().reshape(-1, logits.shape[-1])
+        if logits.dtype != torch.bfloat16:
+            logits = logits.to(torch.bfloat16)
+        if logits.shape[1] != self.V:
+            raise ValueError("logits have {} classes, the accumulator {}".format(
+                logits.shape[1], self.V))
+        M, V, labels, ws = _vocab_ce_check(logits, labels)
+        ext().vocab_ce(logits=logits.data_ptr(), ldl=logits.stride(0), labels=labels.data_ptr(),
+                       M=M, V=V, ignore_index=int(ignore_index), acc=self.buffer.data_ptr(),
+                       workspace=ws.data_ptr(), stream=_stream())
+
+    def read(self) -> dict:
+        host = self.buffer.cpu()
+        return dict(loss_sum=float(host[0:1].view(torch.float64)[0]), count=int(host[1]),
+                    correct=int(host[2]), invalid=int(host[3]), classes=self.V)
 
 
 class EvalAccumulator:

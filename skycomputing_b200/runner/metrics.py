@@ -10,8 +10,16 @@ GLUE classification tasks report.
   ``backend="torch"``, and the oracle of the native ``ops.native.EvalAccumulator``;
 * ``LazyEvalAccumulator``: what ``Runner.evaluate`` hands to the engine - picks the native or the
   torch accumulator from the first logits it sees (the class count is only known there).
+
+Token-level outputs (a masked-language-model head: logits ``[B, S, V]``, labels ``[B, S]``) are
+counted per labelled token instead, without a confusion matrix: ``TorchTokenAccumulator`` (the
+oracle) and ``ops.native.TokenEvalAccumulator`` collect the loss sum, the labelled tokens, the
+correct top-1 predictions and the invalid labels, and ``token_metrics`` reports ``n``, ``loss``,
+``accuracy`` and ``perplexity``.
 """
 from __future__ import annotations
+
+import math
 
 import torch
 
@@ -55,6 +63,55 @@ class TorchEvalAccumulator:
                     confusion=self.confusion.cpu().view(self.C, self.C).clone())
 
 
+class TorchTokenAccumulator:
+    """Same totals as the ``vocab_ce`` kernel in eval mode: loss = logsumexp(row) - row[label]
+    (fp64 sum), correct = ``torch.argmax`` equals the label."""
+
+    def __init__(self, V: int, device=None):
+        self.V = int(V)
+        self.device = torch.device(device) if device is not None else torch.device("cpu")
+        self.reset()
+
+    def reset(self) -> None:
+        self.loss_sum = torch.zeros((), dtype=torch.float64, device=self.device)
+        self.count = torch.zeros((), dtype=torch.int64, device=self.device)
+        self.correct = torch.zeros((), dtype=torch.int64, device=self.device)
+        self.invalid = torch.zeros((), dtype=torch.int64, device=self.device)
+
+    @torch.no_grad()
+    def add(self, logits: torch.Tensor, labels: torch.Tensor, ignore_index: int = -100) -> None:
+        logits = logits.detach().reshape(-1, logits.shape[-1]).to(self.device)
+        labels = labels.detach().reshape(-1).to(self.device, torch.int64)
+        if logits.shape[1] != self.V:
+            raise ValueError("logits have {} classes, the accumulator {}".format(
+                logits.shape[1], self.V))
+        keep = labels != ignore_index
+        valid = keep & (labels >= 0) & (labels < self.V)
+        self.invalid += (keep & ~valid).sum()
+        rows = logits[valid].float()
+        lab = labels[valid]
+        loss = torch.logsumexp(rows, dim=1) - rows.gather(1, lab[:, None])[:, 0]
+        self.loss_sum += loss.double().sum()
+        self.count += lab.numel()
+        self.correct += (torch.argmax(logits[valid], dim=1) == lab).sum()
+
+    def read(self) -> dict:
+        return dict(loss_sum=float(self.loss_sum), count=int(self.count),
+                    correct=int(self.correct), invalid=int(self.invalid), classes=self.V)
+
+
+def make_token_accumulator(V: int, device) -> object:
+    """The native token accumulator where the native kernels run, the torch one elsewhere."""
+    device = torch.device(device)
+    if device.type == "cuda":
+        from ..models.bert_layers import get_backend
+        from ..ops import native as nat
+
+        if get_backend() != "torch" and nat.available() and V <= nat.ext().vocab_ce_max_v():
+            return nat.TokenEvalAccumulator(V, device)
+    return TorchTokenAccumulator(V, device)
+
+
 def make_accumulator(C: int, device) -> object:
     """The native accumulator where the native kernels run (CUDA, backend != "torch", C within
     the kernel's limit), the torch one elsewhere."""
@@ -82,7 +139,10 @@ class LazyEvalAccumulator:
 
     def add(self, logits: torch.Tensor, labels: torch.Tensor) -> None:
         if self.inner is None:
-            self.inner = make_accumulator(logits.shape[-1], logits.device)
+            # one prediction per token (MLM head: [B, S, V] logits, [B, S] labels) or per sequence
+            per_token = logits.dim() == 3 or labels.dim() == 2
+            make = make_token_accumulator if per_token else make_accumulator
+            self.inner = make(logits.shape[-1], logits.device)
         self.inner.add(logits, labels, self.ignore_index)
 
     def read(self) -> dict:
@@ -110,9 +170,18 @@ def classification_metrics(confusion, loss_sum: float, count: int) -> dict:
     return out
 
 
+def token_metrics(loss_sum: float, count: int, correct: int) -> dict:
+    """``n`` labelled tokens, mean ``loss``, top-1 ``accuracy`` and ``perplexity = exp(loss)``;
+    None each when n == 0."""
+    n = int(count)
+    loss = (float(loss_sum) / n) if n else None
+    return dict(n=n, loss=loss, accuracy=(int(correct) / n) if n else None,
+                perplexity=math.exp(min(loss, 700.0)) if n else None)
+
+
 def format_metrics(metrics: dict) -> str:
     parts = []
-    for k in ("n", "loss", "accuracy", "f1", "mcc"):
+    for k in ("n", "loss", "accuracy", "perplexity", "f1", "mcc"):
         if k in metrics:
             v = metrics[k]
             parts.append("{}={}".format(k, "None" if v is None else (
@@ -120,5 +189,6 @@ def format_metrics(metrics: dict) -> str:
     return ", ".join(parts)
 
 
-__all__ = ["TorchEvalAccumulator", "LazyEvalAccumulator", "make_accumulator",
-           "classification_metrics", "format_metrics"]
+__all__ = ["TorchEvalAccumulator", "TorchTokenAccumulator", "LazyEvalAccumulator",
+           "make_accumulator", "make_token_accumulator", "classification_metrics", "token_metrics",
+           "format_metrics"]

@@ -48,9 +48,53 @@ class _NativeCrossEntropy(nn.Module):
         return dlogits
 
 
+class MaskedLMLoss(nn.Module):
+    """Token-level cross entropy of a masked-language-model head: logits ``[..., V]``, labels
+    ``[...]`` with ``ignore_index`` on every position that is not predicted.  The mean runs over
+    the labelled positions; with none the loss is 0 (``F.cross_entropy`` would give NaN), so that
+    a micro-batch without a masked token adds nothing to the step.  On the GPU the loss runs on
+    the ``vocab_ce`` kernel, which supports at most 98304 classes (``ops.native.vocab_ce``)."""
+
+    def __init__(self, ignore_index: int = -100):
+        super().__init__()
+        self.ignore_index = int(ignore_index)
+
+    def forward(self, logits, labels):
+        # the mean of F.cross_entropy(ignore_index=...) as sum / count, without a host sync
+        flat = labels.reshape(-1)
+        total = nn.functional.cross_entropy(logits.reshape(-1, logits.shape[-1]).float(), flat,
+                                            ignore_index=self.ignore_index, reduction="sum")
+        return total / (flat != self.ignore_index).sum().clamp(min=1)
+
+
+class _NativeMaskedLMLoss(MaskedLMLoss):
+    def fused(self, logits, labels, scale: float, loss_acc: torch.Tensor) -> torch.Tensor:
+        """Engine fast path (see ``_NativeCrossEntropy.fused``): the ``vocab_ce`` kernel adds
+        ``loss * scale`` to ``loss_acc`` and returns the bf16 gradient of the logits, written over
+        them when they are a bf16 tensor of their own (no second vocabulary-sized buffer)."""
+        from ..ops import native as nat
+
+        V = logits.shape[-1]
+        flat = logits.detach().reshape(-1, V)
+        in_place = flat.dtype == torch.bfloat16 and flat.is_contiguous()
+        if flat.dtype != torch.bfloat16:
+            flat = flat.to(torch.bfloat16)
+        _, dlogits = nat.vocab_ce(flat, labels.reshape(-1), grad_scale=scale, loss_acc=loss_acc,
+                                  ignore_index=self.ignore_index, in_place=in_place)
+        return dlogits.view(logits.shape)
+
+
 def build_loss(loss_cfg: dict, device: torch.device) -> nn.Module:
     cfg = dict(loss_cfg)
     name = cfg.pop("type")
+    if name == "MaskedLMLoss":
+        if device.type == "cuda":
+            from ..models.bert_layers import get_backend
+            from ..ops import native as nat
+
+            if get_backend() != "torch" and nat.available():
+                return _NativeMaskedLMLoss(**cfg)
+        return MaskedLMLoss(**cfg)
     if name == "CrossEntropyLoss" and not cfg and device.type == "cuda":
         from ..models.bert_layers import get_backend
         from ..ops import native as nat
@@ -297,7 +341,9 @@ class Runner:
     def evaluate(self, data_loader, name: str = "val", micro_batches: Optional[int] = None,
                  ignore_index: int = -100) -> dict:
         """Classification metrics of the model on ``data_loader`` (collective: every rank calls
-        it and every rank gets the same dict, broadcast by the last stage).
+        it and every rank gets the same dict, broadcast by the last stage).  For a token-level
+        head (3-D logits / 2-D labels, e.g. ``BertTailForMaskedLM``) the metrics are those of
+        ``token_metrics``: labelled tokens, loss, top-1 accuracy and perplexity.
 
         The model runs in eval mode (the previous mode is restored) through the engine's
         forward-only pass with ``micro_batches`` chunks per batch (default: the training value;
@@ -309,7 +355,8 @@ class Runner:
         """
         import torch.distributed as dist
 
-        from .metrics import LazyEvalAccumulator, classification_metrics, format_metrics
+        from .metrics import (LazyEvalAccumulator, classification_metrics, format_metrics,
+                              token_metrics)
 
         eng = self.engine
         m = int(micro_batches or self.micro_batches)
@@ -338,7 +385,8 @@ class Runner:
                 if n < batch:
                     data = [torch.cat([t, t.new_zeros((batch - n,) + tuple(t.shape[1:]))])
                             for t in data]
-                    labels = torch.cat([labels, labels.new_full((batch - n,), ignore_index)])
+                    labels = torch.cat([labels, labels.new_full((batch - n,) + tuple(labels.shape[1:]),
+                                                                ignore_index)])
                 self._call_hook("before_val_iter")
                 inputs = [self._to_device(t) for t in data] if eng.is_first else None
                 lab = self._to_device(labels) if eng.is_last else None
@@ -347,10 +395,14 @@ class Runner:
                 self._call_hook("after_val_iter")
             totals = acc.read() if eng.is_last else None
             payload = None
-            if totals is not None:
+            if totals is not None and "confusion" not in totals:   # token-level (MLM head)
+                payload = dict(token_metrics(totals["loss_sum"], totals["count"],
+                                             totals["correct"]),
+                               invalid=totals["invalid"], classes=totals["classes"])
+            elif totals is not None:
                 payload = dict(classification_metrics(totals["confusion"], totals["loss_sum"],
                                                       totals["count"]),
-                               invalid=totals["invalid"])
+                               invalid=totals["invalid"], classes=len(totals["confusion"]))
             if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
                 box = [payload]
                 dist.broadcast_object_list(box, src=self.model.stage_to_rank[-1])
@@ -358,10 +410,10 @@ class Runner:
         finally:
             self.model.train(was_training)
             torch.random.set_rng_state(cpu_rng)
-        invalid = payload.pop("invalid")
+        invalid, classes = payload.pop("invalid"), payload.pop("classes")
         if invalid:
             raise ValueError("evaluation {}: {} labels are outside [0, {}) and not ignore_index "
-                             "({})".format(name, invalid, len(payload["confusion"]), ignore_index))
+                             "({})".format(name, invalid, classes, ignore_index))
         self._call_hook("after_val_epoch")
         self._log("eval {}: {}".format(name, format_metrics(payload)))
         if self._metrics_path is not None:
