@@ -119,6 +119,8 @@ struct LayerNormBwdArgs {
   int* error_flag = nullptr;
 };
 int launch_layernorm_bwd(const LayerNormBwdArgs& a, cudaStream_t stream);
+// dgamma += sum_rows dy * xhat, dbeta += sum_rows dy; out2 += sum_rows x2 when x2 != null.
+// H % 8 != 0 returns 916.
 int launch_ln_param_grad(const void* dy, const void* z, const float* mean, const float* rstd,
                          float* dgamma, float* dbeta, int M, int H, const void* x2, float* out2,
                          cudaStream_t stream);
@@ -335,6 +337,9 @@ int launch_optim_finalize(const float* partials, int n_partials, const float* ex
                           int schedule, int warmup,
                           int total, double base_lr, float max_norm, OptimScalars* out,
                           cudaStream_t stream);
+// Round-to-nearest-even casts, bit-identical to torch's .to(torch.bfloat16) / .float() for every
+// non-NaN input.  Subnormals are converted, not flushed, even under --use_fast_math (neither
+// conversion has a flush-to-zero form); a NaN stays a NaN, its payload may differ from torch's.
 int launch_cast_f32_to_bf16(const float* src, void* dst, long long n, cudaStream_t stream);
 int launch_cast_bf16_to_f32(const void* src, float* dst, long long n, cudaStream_t stream);
 

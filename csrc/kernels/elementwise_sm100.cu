@@ -1399,6 +1399,7 @@ int launch_ln_param_grad(const void* dy, const void* z, const float* mean, const
                          float* dgamma, float* dbeta, int M, int H, const void* x2, float* out2,
                          cudaStream_t stream) {
   if (M <= 0) return 0;
+  if (H % 8 != 0) return 916;  // 16-byte row loads
   dim3 g2((H + 255) / 256, 1);
   int ry = (M + 63) / 64;
   if (ry > 64) ry = 64;

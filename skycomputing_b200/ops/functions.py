@@ -509,6 +509,13 @@ def _grad_send_kwargs(in_ch, mb: int, which: int) -> dict:
 # --------------------------------------------------------------------------------------------
 # embeddings / pooler / classifier / loss
 # --------------------------------------------------------------------------------------------
+def _flat_int64(t: torch.Tensor) -> torch.Tensor:
+    """The embedding kernels read ids, token types and the attention mask as contiguous int64:
+    int32 ids or a bool / int32 mask (as HF-style pipelines produce) are converted, not
+    reinterpreted."""
+    return t.reshape(-1).to(torch.int64).contiguous()
+
+
 class EmbeddingsFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, emb, training: bool, out_ch, mb: int, input_ids, token_type_ids,
@@ -516,9 +523,7 @@ class EmbeddingsFn(torch.autograd.Function):
         B, S = input_ids.shape
         H = emb.word.master().shape[1]
         dev = input_ids.device
-        ids = input_ids.reshape(-1).contiguous()
-        tts = token_type_ids.reshape(-1).contiguous()
-        am = attention_mask.reshape(-1).contiguous()
+        ids, tts, am = (_flat_int64(t) for t in (input_ids, token_type_ids, attention_mask))
         out = torch.empty((B * S, H), dtype=torch.bfloat16, device=dev)
         ext_mask = torch.empty((B * S,), dtype=torch.float32, device=dev)
         mean = torch.empty(B * S, dtype=torch.float32, device=dev)

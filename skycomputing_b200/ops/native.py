@@ -381,7 +381,12 @@ def softmax_ce(logits: torch.Tensor, labels: torch.Tensor, grad_scale: float = 1
     """Mean cross entropy and d(loss * grad_scale)/dlogits; ``loss_acc[0] += loss * grad_scale``
     when given (the step loss of a micro-batched step, accumulated without extra launches)."""
     _check(logits, torch.float32, "logits")
+    if logits.dim() != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous 2-D [M, C] tensor")
     M, C = logits.shape
+    if not labels.is_cuda or labels.dtype != torch.int64 or labels.numel() != M:
+        raise ValueError("labels must be a CUDA int64 tensor with one entry per logits row")
+    labels = labels.reshape(-1).contiguous()
     loss = torch.empty(1, dtype=torch.float32, device=logits.device)
     dlogits = torch.empty_like(logits)
     ext().softmax_ce(logits=logits.data_ptr(), labels=labels.data_ptr(), loss=loss.data_ptr(),
