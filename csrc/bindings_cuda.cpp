@@ -290,6 +290,20 @@ int vocab_ce(uintptr_t logits, long long ldl, uintptr_t labels, int M, int V,
   check(sky::launch_vocab_ce(a, S(stream)), "vocab_ce");
   return sky::vocab_ce_launches(a);
 }
+void mlm_gather(uintptr_t hidden, uintptr_t labels, int B, int seq, int H, int max_pred,
+                long long ignore_index, int V, uintptr_t slot_of_row, uintptr_t slot_labels,
+                uintptr_t x_c, uintptr_t stream) {
+  check(sky::launch_mlm_gather(P<const void>(hidden), P<const int64_t>(labels), B, seq, H, max_pred,
+                               ignore_index, V, P<int>(slot_of_row), P<int64_t>(slot_labels),
+                               P<void>(x_c), S(stream)),
+        "mlm_gather");
+}
+void mlm_scatter(uintptr_t dx_c, uintptr_t slot_of_row, long long rows, int H, uintptr_t dhidden,
+                 uintptr_t stream) {
+  check(sky::launch_mlm_scatter(P<const void>(dx_c), P<const int>(slot_of_row), rows, H,
+                                P<void>(dhidden), S(stream)),
+        "mlm_scatter");
+}
 
 // descriptors: list of (p, g, mom, p_bf16, numel) -> packed host bytes to upload once
 py::bytes pack_sgd_descriptors(
@@ -510,6 +524,12 @@ PYBIND11_MODULE(_cuda, m) {
         py::arg("acc") = 0, py::arg("workspace") = 0, py::arg("stream") = 0);
   m.def("vocab_ce_workspace_bytes", [](int M) { return sky::vocab_ce_workspace_bytes(M); });
   m.def("vocab_ce_max_v", []() { return sky::kVocabCeMaxV; });
+  m.def("mlm_gather", &mlm_gather, py::arg("hidden"), py::arg("labels"), py::arg("B"),
+        py::arg("S"), py::arg("H"), py::arg("P"), py::arg("ignore_index"), py::arg("V"),
+        py::arg("slot_of_row"), py::arg("slot_labels"), py::arg("x_c"), py::arg("stream") = 0);
+  m.def("mlm_scatter", &mlm_scatter, py::arg("dx_c"), py::arg("slot_of_row"), py::arg("rows"),
+        py::arg("H"), py::arg("dhidden"), py::arg("stream") = 0);
+  m.def("mlm_max_predictions", []() { return sky::kMlmMaxPredictions; });
   m.def("pack_sgd_descriptors", &pack_sgd_descriptors);
   m.def("sgd_multi", &sgd_multi, py::arg("d_tensors"), py::arg("n"), py::arg("max_numel"),
         py::arg("lr"), py::arg("momentum") = 0.f, py::arg("weight_decay") = 0.f,

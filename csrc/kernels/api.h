@@ -274,6 +274,26 @@ int launch_vocab_ce(const VocabCeArgs& a, cudaStream_t stream);
 // kernels a successful launch_vocab_ce(a) issues: 3 (training), 2 (eval), fewer when M == 0
 int vocab_ce_launches(const VocabCeArgs& a);
 
+// Sparse masked-language-model decoding.  Sequence b owns slots [b*P, (b+1)*P); its labelled
+// positions (label != ignore_index), in position order, fill them from the front.
+// mlm_gather (one launch, one CTA per sequence):
+//   slot_of_row[B*S] (int32) = the row's slot, -1 where the row is not decoded;
+//   slot_labels[B*P] = the slot's label, ignore_index in an empty slot; when a sequence has more
+//   than P labelled positions the extra ones are dropped and its last slot gets the label V (out
+//   of range: the vocab_ce loss turns NaN and the eval accumulator counts it as invalid);
+//   x_c[B*P, H] (bf16) = hidden[row_of_slot] (hidden is [B*S, H] bf16), zeros in an empty slot.
+// mlm_scatter (one launch): dhidden[r] = dx_c[slot_of_row[r]] for a decoded row, zeros otherwise;
+//   every row of dhidden [rows, H] is written exactly once.
+// Both: H % 8 == 0, hidden / x_c / dx_c / dhidden 16-byte aligned; integer scans and copies only
+// (deterministic), no host sync.  Errors: 960 bad shape (B, S, P >= 1, P <= kMlmMaxPredictions,
+// H a positive multiple of 8), 961 null pointer, 962 a bf16 buffer is not 16-byte aligned.
+constexpr int kMlmMaxPredictions = 8192;  // slot map of one sequence in shared memory
+int launch_mlm_gather(const void* hidden, const int64_t* labels, int B, int S, int H, int P,
+                      long long ignore_index, int V, int* slot_of_row, int64_t* slot_labels,
+                      void* x_c, cudaStream_t stream);
+int launch_mlm_scatter(const void* dx_c, const int* slot_of_row, long long rows, int H,
+                       void* dhidden, cudaStream_t stream);
+
 // ---------------------------------------------------------------------------------------------
 // Optimizer / parameter maintenance
 // ---------------------------------------------------------------------------------------------

@@ -990,6 +990,78 @@ vocab_ce_finalize_kernel(const double* __restrict__ row_loss, const int* __restr
 }
 
 // ------------------------------------------------------------------------------------------
+// Sparse masked-language-model decoding: the rows the head decodes are the labelled positions.
+//   mlm_gather_kernel   1 CTA per sequence: scans the S labels in position order (warp ballot +
+//                       popc prefix), writes slot_of_row / slot_labels and copies the selected
+//                       hidden rows into the slots (zero rows for empty slots)
+//   mlm_scatter_kernel  grid-stride over dhidden: row r gets dx_c[slot_of_row[r]] or zeros
+// Integer scans and pure copies: bit-identical on every call and replay.
+// ------------------------------------------------------------------------------------------
+constexpr int kMlmThreads = 256;
+constexpr int kMlmWarps = kMlmThreads / 32;
+
+__global__ void __launch_bounds__(kMlmThreads)
+mlm_gather_kernel(const uint4* __restrict__ hidden, const int64_t* __restrict__ labels, int S,
+                  int H8, int P, long long ignore_index, long long sentinel,
+                  int* __restrict__ slot_of_row, int64_t* __restrict__ slot_labels,
+                  uint4* __restrict__ x_c) {
+  extern __shared__ int mlm_row_of_slot[];  // [P]: position of the slot's labelled token
+  __shared__ int warp_cnt[kMlmWarps];
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int64_t* lab = labels + static_cast<long long>(b) * S;
+  int* sor = slot_of_row + static_cast<long long>(b) * S;
+  int n = 0;  // labelled positions in front of the current chunk
+  for (int base = 0; base < S; base += kMlmThreads) {
+    const int pos = base + tid;
+    const bool on = pos < S && lab[pos] != ignore_index;
+    const unsigned m = __ballot_sync(0xffffffffu, on);
+    if (lane == 0) warp_cnt[warp] = __popc(m);
+    __syncthreads();
+    int before = 0, chunk = 0;
+#pragma unroll
+    for (int w = 0; w < kMlmWarps; ++w) {
+      before += w < warp ? warp_cnt[w] : 0;
+      chunk += warp_cnt[w];
+    }
+    const int rank = n + before + __popc(m & ((1u << lane) - 1u));
+    if (pos < S) {
+      const bool kept = on && rank < P;
+      sor[pos] = kept ? b * P + rank : -1;
+      if (kept) mlm_row_of_slot[rank] = pos;
+    }
+    n += chunk;
+    __syncthreads();  // warp_cnt is rewritten by the next chunk; the slot map is read below
+  }
+  const int filled = n < P ? n : P;
+  int64_t* sl = slot_labels + static_cast<long long>(b) * P;
+  for (int r = tid; r < P; r += kMlmThreads) {
+    long long v = r < filled ? lab[mlm_row_of_slot[r]] : ignore_index;
+    if (n > P && r == P - 1) v = sentinel;  // overflow: never silent
+    sl[r] = v;
+  }
+  const long long src0 = static_cast<long long>(b) * S;
+  uint4* dst = x_c + static_cast<long long>(b) * P * H8;
+  const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
+  for (int i = tid; i < P * H8; i += kMlmThreads) {
+    const int r = i / H8, c = i - r * H8;
+    dst[i] = r < filled ? hidden[(src0 + mlm_row_of_slot[r]) * H8 + c] : zero;
+  }
+}
+
+__global__ void __launch_bounds__(kMlmThreads)
+mlm_scatter_kernel(const uint4* __restrict__ dx_c, const int* __restrict__ slot_of_row,
+                   long long rows, int H8, uint4* __restrict__ dhidden) {
+  const long long total = rows * H8;
+  const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long r = i / H8;
+    const int s = slot_of_row[r];
+    dhidden[i] = s >= 0 ? dx_c[static_cast<long long>(s) * H8 + (i - r * H8)] : zero;
+  }
+}
+
+// ------------------------------------------------------------------------------------------
 // Optimizer
 // ------------------------------------------------------------------------------------------
 // kScalars: lr and the clip coefficient come from the device-side OptimScalars (schedule / global
@@ -1582,6 +1654,36 @@ int launch_vocab_ce(const VocabCeArgs& a, cudaStream_t stream) {
   if (eval && a.M == 0) return 0;
   vocab_ce_finalize_kernel<<<1, kVceFinThreads, 0, stream>>>(
       row_loss, row_flags, a.M, n_valid, a.grad_scale, a.loss_out, a.loss_acc, a.acc);
+  SKY_LAUNCH_CHECK();
+}
+
+namespace {
+bool aligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; }
+}  // namespace
+
+int launch_mlm_gather(const void* hidden, const int64_t* labels, int B, int S, int H, int P,
+                      long long ignore_index, int V, int* slot_of_row, int64_t* slot_labels,
+                      void* x_c, cudaStream_t stream) {
+  if (B < 1 || S < 1 || H < 8 || H % 8 != 0 || P < 1 || P > kMlmMaxPredictions || V < 1)
+    return 960;
+  if (!hidden || !labels || !slot_of_row || !slot_labels || !x_c) return 961;
+  if (!aligned16(hidden) || !aligned16(x_c)) return 962;
+  mlm_gather_kernel<<<B, kMlmThreads, static_cast<size_t>(P) * sizeof(int), stream>>>(
+      static_cast<const uint4*>(hidden), labels, S, H / 8, P, ignore_index, V, slot_of_row,
+      slot_labels, static_cast<uint4*>(x_c));
+  SKY_LAUNCH_CHECK();
+}
+
+int launch_mlm_scatter(const void* dx_c, const int* slot_of_row, long long rows, int H,
+                       void* dhidden, cudaStream_t stream) {
+  if (rows < 1 || H < 8 || H % 8 != 0) return 960;
+  if (!dx_c || !slot_of_row || !dhidden) return 961;
+  if (!aligned16(dx_c) || !aligned16(dhidden)) return 962;
+  const long long vec = rows * (H / 8);
+  long long blocks = (vec + kMlmThreads - 1) / kMlmThreads;
+  if (blocks > num_sms() * 8LL) blocks = num_sms() * 8LL;
+  mlm_scatter_kernel<<<static_cast<unsigned>(blocks), kMlmThreads, 0, stream>>>(
+      static_cast<const uint4*>(dx_c), slot_of_row, rows, H / 8, static_cast<uint4*>(dhidden));
   SKY_LAUNCH_CHECK();
 }
 

@@ -907,6 +907,14 @@ PFN_encodeTiled get_encode_fn() {
     if (e == cudaSuccess && qres == cudaDriverEntryPointSuccess)
       fn = reinterpret_cast<PFN_encodeTiled>(ptr);
   });
+  // the encoder is a driver call and needs a current context.  A thread whose first CUDA call
+  // this is (autograd's device thread when a backward starts with a GEMM) has none yet:
+  // cudaSetDevice makes the device's primary context current, once per thread.
+  thread_local bool ctx_current = false;
+  if (!ctx_current) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) == cudaSuccess && cudaSetDevice(dev) == cudaSuccess) ctx_current = true;
+  }
   return fn;
 }
 

@@ -45,6 +45,9 @@ TINY = os.getenv("TINY", "0") == "1"                          # shrink the geome
 TASK = os.getenv("TASK", "cls")
 if TASK not in ("cls", "mlm"):
     raise ValueError("TASK must be 'cls' or 'mlm', got {!r}".format(TASK))
+# MLM_MAX_PREDICTIONS=P (TASK=mlm): the head decodes only the labelled positions, at most P per
+# sequence (P >= round(0.15 * (SEQ_LEN - 2)): 20 at 128 tokens); unset = every position decoded
+MLM_MAX_PREDICTIONS = int(os.getenv("MLM_MAX_PREDICTIONS")) if os.getenv("MLM_MAX_PREDICTIONS") else None
 
 _config = BertConfig.bert_large()                              # wwm_uncased_L-24_H-1024_A-16 geometry
 if TINY:
@@ -68,6 +71,8 @@ _TAIL = [
 ]
 if TASK == "mlm":
     _TAIL = [dict(layer_type="BertTailForMaskedLM", config=_config.__dict__)]
+    if MLM_MAX_PREDICTIONS is not None:
+        _TAIL[0]["max_predictions"] = MLM_MAX_PREDICTIONS
 
 model_config = [dict(layer_type="BertEmbeddings", config=_config.__dict__)] + _ENCODER + _TAIL
 

@@ -163,6 +163,16 @@ class ModuleWrapper(nn.Module):
         self.in_channel = None          # set by the pipeline engine (fused stage boundary)
         self.out_channel = None
         self.microbatch = 0
+        # the micro-batch's labels, bound by the pipeline engine when the last layer consumes
+        # them (a sparse masked-language-model head).  A binding holds for ONE forward call,
+        # which takes and clears it: a later call without a binding (inference, fill-mask) passes
+        # no labels and gets the dense logits
+        self.labels = None
+        children = list(module.children())
+        for i, layer in enumerate(children[:-1]):
+            if getattr(layer, "consumes_labels", False):
+                raise ValueError("{} (layer {} of {}) consumes labels and must be the model's "
+                                 "last layer".format(type(layer).__name__, i, len(children)))
         # the pipeline engine brackets backward itself (begin_backward/end_backward) because the
         # first stage has no differentiable input to hang the autograd probe on
         self.engine_managed_backward = False
@@ -184,6 +194,12 @@ class ModuleWrapper(nn.Module):
     @property
     def layers(self) -> SequentialWrapper:
         return self._module
+
+    @property
+    def consumes_labels(self) -> bool:
+        """Does the last layer take the labels (``ModuleWrapper.labels``) as an input?"""
+        last = self._module[-1] if len(self._module) else None
+        return bool(getattr(last, "consumes_labels", False))
 
     @property
     def device(self) -> torch.device:
@@ -230,13 +246,18 @@ class ModuleWrapper(nn.Module):
                 i += 1
         return plan
 
-    def _run_layers(self, args):
+    def _run_layers(self, args, labels=None):
         from ..models.bert_layers import BertSpan, _native_enabled
 
         first_tensor = next((a for a in args if torch.is_tensor(a)), None)
         use_native = first_tensor is not None and first_tensor.is_cuda and _native_enabled(first_tensor)
+        with_labels = labels is not None and self.consumes_labels
         if not use_native:
-            return self._module(*args)
+            if not with_labels:
+                return self._module(*args)
+            inputs = self._module[:-1](*args)
+            inputs = inputs if isinstance(inputs, (tuple, list)) else (inputs,)
+            return self._module[-1](*inputs, labels=labels)
         if self._plan is None:
             self._plan = self._build_plan()
         inputs = args
@@ -258,6 +279,8 @@ class ModuleWrapper(nn.Module):
                 else:
                     for layer in step.layers:
                         inputs = layer(*inputs) if isinstance(inputs, (tuple, list)) else layer(inputs)
+            elif with_labels and idx == n - 1:
+                inputs = step(*inputs, labels=labels)
             else:
                 inputs = step(*inputs)
         return inputs
@@ -399,6 +422,7 @@ class ModuleWrapper(nn.Module):
         return t
 
     def forward(self, *args):
+        labels, self.labels = self.labels, None
         args = [self._move_in(a) for a in args]
         need_probe = self._record_forward_time or self._slowdown > 0 or self._logger is not None
         timed = not self._probes_suspended
@@ -413,7 +437,7 @@ class ModuleWrapper(nn.Module):
                     self._device_throttle_begin()
             else:
                 t0 = time.time()
-        out = self._run_layers(args)
+        out = self._run_layers(args, labels)
         if need_probe:
             if cuda:
                 if self._slowdown > 0:

@@ -94,14 +94,22 @@ class Estimator:
             return None
         H, I, A = c["hidden_size"], c["intermediate_size"], c["num_attention_heads"]
         if lt == "BertTailForMaskedLM":
-            # transform dense + decoder; every token is decoded, so the decoder dominates (about
-            # 2.5 encoder blocks at BERT-large with a 30K vocabulary)
             B, S, _ = data[0].shape
             V = c["vocab_size"]
             params = H * H + H + 2 * H + V * H + V
-            outs = 3 * B * S * H + 2 * B * S * V   # dense_act, LayerNorm, transform; decoder, layer
-            mem = (2 * outs + param_scale * params + B * S * H + B * S) * 4 / mb
-            return 2.0 * B * S * H * (H + V), mem, [((B, S, V), f32)]
+            P = layer_cfg.get("max_predictions")
+            if P is None:
+                # transform dense + decoder; every token is decoded, so the decoder dominates
+                # (about 2.5 encoder blocks at BERT-large with a 30K vocabulary)
+                outs = 3 * B * S * H + 2 * B * S * V   # dense_act, LayerNorm, transform; decoder, layer
+                mem = (2 * outs + param_scale * params + B * S * H + B * S) * 4 / mb
+                return 2.0 * B * S * H * (H + V), mem, [((B, S, V), f32)]
+            # sparse head: B*P slots are decoded (a fraction of a block at P = 20, S = 128); the
+            # labels [B, S] are one more input and the slot labels one more output
+            R = B * P
+            outs = 3 * R * H + 2 * R * V + R
+            mem = (2 * outs + param_scale * params + B * S * H + 2 * B * S) * 4 / mb
+            return 2.0 * R * H * (H + V), mem, [((R, V), f32), ((R,), torch.int64)]
         if lt == "BertEmbeddings":
             B, S = data[0].shape
             params = (c["vocab_size"] + c["max_position_embeddings"] + c["type_vocab_size"]) * H + 2 * H

@@ -9,6 +9,8 @@ Registered names and calling conventions are those of scaelum/model/bert_layers.
     BertPooler(config)                (hidden, mask)            -> pooled
     BertTailForClassification(hidden_dropout_prob, hidden_size, num_classes)   pooled -> logits
     BertTailForMaskedLM(config)       (hidden, mask)            -> logits [B, S, vocab]
+    BertTailForMaskedLM(config, max_predictions=P)
+                                      (hidden, mask, labels)    -> (logits [B*P, vocab], slot_labels [B*P])
 
 Parameter names match the reference (``attention.self.query.weight`` ...), so layer-indexed
 checkpoints interchange.  Every layer has two execution paths behind the same class:
@@ -501,15 +503,40 @@ class BertPredictionHeadTransform(nn.Module):
 class BertTailForMaskedLM(nn.Module):
     """Masked-language-model head (HF ``BertLMPredictionHead``): dense + activation + LayerNorm,
     then a decoder to vocabulary logits.  ``(hidden [B,S,H], mask) -> logits [B,S,V]``; every
-    token is decoded (the layer does not see which positions are masked).
+    token is decoded unless ``max_predictions`` is set (below).
 
     The decoder weight is a parameter of its own, not tied to the word embeddings.  The native
     path needs ``H % 8 == 0`` and ``V % 8 == 0`` (GEMM output widths), which is why BERT configs
-    pad the vocabulary (30522 -> 30528); other shapes run the eager path."""
+    pad the vocabulary (30522 -> 30528); other shapes run the eager path.
 
-    def __init__(self, config):
+    ``max_predictions=P`` makes the head label-consuming (``consumes_labels``): in a pipeline the
+    stage passes the micro-batch's labels ``[B, S]`` and the head decodes only the labelled
+    positions, at most P per sequence, returning ``(logits [B*P, V], slot_labels [B*P])`` (slot
+    layout and overflow rule: ``ops.functions.mlm_slots_ref``).  It is a data contract: choose
+    ``P >= round(mask_prob * (S - 2))``, the labelled count of the BERT masking (19 at S = 128
+    and 15 %).  Without labels the head decodes every position, as the dense head does; the
+    parameters are the same in both modes, so checkpoints interchange.
+
+    P is at most ``max_position_embeddings`` and at most ``MAX_PREDICTIONS_LIMIT`` (the
+    ``mlm_gather`` kernel keeps a sequence's slot map in shared memory), on every backend, so that
+    a config that constructs also runs on the GPU.  ``ignore_index`` must be the loss's: the head
+    marks empty slots with it, and a loss with another value counts them as invalid labels."""
+
+    MAX_PREDICTIONS_LIMIT = 8192   # csrc/kernels/api.h: kMlmMaxPredictions
+
+    def __init__(self, config, max_predictions=None, ignore_index: int = -100):
         super().__init__()
         config = BertConfig.from_dict(config) if isinstance(config, dict) else config
+        bound = min(config.max_position_embeddings, self.MAX_PREDICTIONS_LIMIT)
+        if max_predictions is not None and (
+                isinstance(max_predictions, bool) or not isinstance(max_predictions, int)
+                or not 1 <= max_predictions <= bound):
+            raise ValueError("max_predictions must be None or an int in [1, {}] (the sequence "
+                             "length bound, at most {} slots per sequence), got {!r}".format(
+                                 bound, self.MAX_PREDICTIONS_LIMIT, max_predictions))
+        self.max_predictions = max_predictions
+        self.ignore_index = int(ignore_index)
+        self.consumes_labels = max_predictions is not None
         self.transform = BertPredictionHeadTransform(config)
         self.decoder = nn.Linear(config.hidden_size, config.vocab_size)
         self._native = None
@@ -526,16 +553,28 @@ class BertTailForMaskedLM(nn.Module):
         return (hidden.dim() == 3 and H % 8 == 0 and V % 8 == 0 and H <= 2048
                 and self.transform.dense_act.act_name in ("gelu", "bias_gelu"))
 
-    def forward(self, hidden_states, attention_mask=None):
+    def forward(self, hidden_states, attention_mask=None, labels=None):
+        if labels is not None and not self.consumes_labels:
+            raise ValueError("labels reach a BertTailForMaskedLM without max_predictions")
+        if labels is not None:
+            labels = labels.to(torch.int64).reshape(hidden_states.shape[0], -1)
         if _native_enabled(hidden_states) and self._supports(hidden_states):
             from ..ops.functions import MaskedLMHeadFn
 
             hp = self._native_params()
             x = hidden_states.to(torch.bfloat16)
             if not self.training and not torch.is_grad_enabled():
-                return MaskedLMHeadFn.infer(hp, x)
-            return MaskedLMHeadFn.apply(hp, x, *hp.all_params())
-        return self.decoder(self.transform(hidden_states.float()))
+                return MaskedLMHeadFn.infer(hp, x, labels)
+            return MaskedLMHeadFn.apply(hp, x, labels, *hp.all_params())
+        if labels is None:
+            return self.decoder(self.transform(hidden_states.float()))
+        from ..ops.functions import mlm_slots_ref
+
+        row, _, slot_labels = mlm_slots_ref(labels, self.max_predictions, self.ignore_index,
+                                            self.decoder.out_features)
+        flat = hidden_states.float().reshape(-1, hidden_states.shape[-1])
+        x = torch.where((row >= 0).unsqueeze(1), flat.index_select(0, row.clamp(min=0)), 0.0)
+        return self.decoder(self.transform(x)), slot_labels
 
 
 def native_param_banks(module: nn.Module):

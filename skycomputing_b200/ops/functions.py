@@ -686,8 +686,37 @@ class SmallLinearParams:
         return [p for b in self.banks for p in b.params]
 
 
+def mlm_slots_ref(labels: torch.Tensor, P: int, ignore_index: int = -100, V: int = 0):
+    """The slot layout of a sparse masked-language-model head, in plain torch (the eager path and
+    the reference of the ``mlm_gather`` / ``mlm_scatter`` kernels).
+
+    ``labels`` [B, S].  Sequence b owns slots [b*P, (b+1)*P); its labelled positions (label !=
+    ``ignore_index``), in position order, fill them from the front.  Returns ``(row_of_slot [B*P],
+    slot_of_row [B*S], slot_labels [B*P])``, all int64: the flat row (b*S + position) decoded in a
+    slot or -1 for an empty slot, the slot of a row or -1 for a row that is not decoded, and the
+    label of each slot (``ignore_index`` when empty).  A sequence with more than P labelled
+    positions drops the extra ones and gets the out-of-range label ``V`` in its last slot, so that
+    the overflow is never silent."""
+    B, S = labels.shape
+    dev = labels.device
+    keep = labels != ignore_index
+    rank = keep.long().cumsum(1) - 1
+    fit = keep & (rank < P)
+    slot = (torch.arange(B, device=dev).unsqueeze(1) * P + rank)[fit]
+    rows = torch.arange(B * S, device=dev).view(B, S)[fit]
+    row_of_slot = torch.full((B * P,), -1, dtype=torch.int64, device=dev)
+    slot_of_row = torch.full((B * S,), -1, dtype=torch.int64, device=dev)
+    slot_labels = torch.full((B * P,), int(ignore_index), dtype=torch.int64, device=dev)
+    row_of_slot[slot] = rows
+    slot_of_row[rows] = slot
+    slot_labels[slot] = labels[fit].to(torch.int64)
+    slot_labels.view(B, P)[keep.sum(1) > P, P - 1] = int(V)
+    return row_of_slot, slot_of_row, slot_labels
+
+
 class MaskedLMHeadParams:
-    """Parameter banks of ``BertTailForMaskedLM``: transform dense (+ GELU), LayerNorm, decoder."""
+    """Parameter banks of ``BertTailForMaskedLM``: transform dense (+ GELU), LayerNorm, decoder;
+    and the head's slot contract (``max_predictions``, ``ignore_index``)."""
 
     def __init__(self, mod):
         tr = mod.transform
@@ -699,6 +728,8 @@ class MaskedLMHeadParams:
         self.b_dec = ParamBank([mod.decoder.bias], False)
         self.banks = [self.w_t, self.b_t, self.gamma, self.beta, self.w_dec, self.b_dec]
         self.eps = float(tr.LayerNorm.eps)
+        self.max_predictions = mod.max_predictions
+        self.ignore_index = mod.ignore_index
 
     def all_params(self):
         return [p for b in self.banks for p in b.params]
@@ -709,32 +740,49 @@ class MaskedLMHeadFn(torch.autograd.Function):
     pre-activation kept for backward), LayerNorm, decoder GEMM with bias to bf16 logits.
     Backward: decoder dgrad GEMM, LayerNorm backward, GELU derivative, transform dgrad GEMM;
     the weight / bias / LayerNorm parameter gradients go straight into the fp32 bank gradients
-    and follow the same deferral / side-stream policy as the encoder's."""
+    and follow the same deferral / side-stream policy as the encoder's.
+
+    With ``labels`` (a sparse head, ``hp.max_predictions`` = P) the ``mlm_gather`` kernel first
+    compacts the labelled rows into B*P slots, the same chain runs on them and the result is
+    ``(logits [B*P, V], slot_labels [B*P])``; backward ends with ``mlm_scatter`` into the
+    [B, S, H] input gradient."""
 
     @staticmethod
-    def _run(hp: MaskedLMHeadParams, hidden: torch.Tensor, keep: bool):
+    def _run(hp: MaskedLMHeadParams, hidden: torch.Tensor, keep: bool, labels=None):
         B, S, H = hidden.shape
         x = hidden.contiguous().view(B * S, H)
+        slots = None
+        if labels is not None:
+            x, slot_of_row, slot_labels = nat.mlm_gather(
+                x, labels, hp.max_predictions, hp.w_dec.master().shape[0], hp.ignore_index)
+            slots = (slot_of_row, slot_labels)
         h1 = torch.empty_like(x) if keep else None
         t = nat.gemm(x, hp.w_t.shadow(), bias=hp.b_t.master(), act=nat.ACT_GELU, out2=h1)
         y, mean, rstd = _ln_fwd(t, hp.gamma.master(), hp.beta.master(), hp.eps)
         logits = nat.gemm(y, hp.w_dec.shadow(), bias=hp.b_dec.master())
-        return logits.view(B, S, -1), (x, h1, t, mean, rstd, y)
+        if slots is None:
+            logits = logits.view(B, S, -1)
+        return logits, (x, h1, t, mean, rstd, y), slots
 
     @staticmethod
-    def infer(hp: MaskedLMHeadParams, hidden: torch.Tensor) -> torch.Tensor:
-        """Eval-mode forward without autograd: the same logits, nothing kept for backward."""
-        return MaskedLMHeadFn._run(hp, hidden, False)[0]
+    def infer(hp: MaskedLMHeadParams, hidden: torch.Tensor, labels=None):
+        """Eval-mode forward without autograd: the same outputs, nothing kept for backward."""
+        logits, _, slots = MaskedLMHeadFn._run(hp, hidden, False, labels)
+        return logits if slots is None else (logits, slots[1])
 
     @staticmethod
-    def forward(ctx, hp, hidden, *params):
-        logits, saved = MaskedLMHeadFn._run(hp, hidden, True)
+    def forward(ctx, hp, hidden, labels, *params):
+        logits, saved, slots = MaskedLMHeadFn._run(hp, hidden, True, labels)
         ctx.hp, ctx.saved, ctx.shape3 = hp, saved, tuple(hidden.shape)
+        ctx.slot_of_row = None if slots is None else slots[0]
         ctx.n_params = len(params)
-        return logits
+        if slots is None:
+            return logits
+        ctx.mark_non_differentiable(slots[1])
+        return logits, slots[1]
 
     @staticmethod
-    def backward(ctx, dlogits):
+    def backward(ctx, dlogits, *_dslot_labels):
         hp = ctx.hp
         x, h1, t, mean, rstd, y = ctx.saved
         B, S, H = ctx.shape3
@@ -751,8 +799,10 @@ class MaskedLMHeadFn(torch.autograd.Function):
                             torch.cuda.current_stream().cuda_stream)
         _wgrad(dh1, x, hp.w_t, hp.b_t)
         dx = nat.gemm(dh1, hp.w_t.shadow(), b_mn=True)
-        ctx.saved = None
-        return (None, dx.view(B, S, H), *([None] * ctx.n_params))
+        if ctx.slot_of_row is not None:
+            dx = nat.mlm_scatter(dx, ctx.slot_of_row)
+        ctx.saved = ctx.slot_of_row = None
+        return (None, dx.view(B, S, H), None, *([None] * ctx.n_params))
 
 
 class SoftmaxCrossEntropyFn(torch.autograd.Function):

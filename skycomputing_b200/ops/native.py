@@ -38,7 +38,7 @@ _KERNELS_PER_CALL = {
     "gemm": 1, "layernorm_fwd": 1, "layernorm_bwd": 1, "ln_param_grad": 1, "colsum": 1, "dgelu_mul": 1,
     "attention_fwd": 1, "attention_bwd": 1, "embed_fwd": 1, "embed_bwd": 1,
     "small_linear_fwd": 1, "small_linear_bwd": 2, "softmax_ce": 1, "classify_eval": 1,
-    "vocab_ce": -1,
+    "vocab_ce": -1, "mlm_gather": 1, "mlm_scatter": 1,
     "sgd_multi": 1, "adam_multi": 1,
     "grad_sumsq_multi": 1, "optim_finalize": 1,
     "cast_f32_to_bf16": 1, "cast_bf16_to_f32": 1, "advance_counter": 1, "advance_epoch": 1,
@@ -447,6 +447,43 @@ def vocab_ce(logits: torch.Tensor, labels: torch.Tensor, grad_scale: float = 1.0
                    grad_scale=float(grad_scale), loss_out=loss.data_ptr(),
                    loss_acc=_ptr(loss_acc), workspace=ws.data_ptr(), stream=_stream())
     return loss, dlogits
+
+
+def mlm_gather(hidden: torch.Tensor, labels: torch.Tensor, P: int, V: int,
+               ignore_index: int = -100):
+    """The rows a sparse masked-language-model head decodes (slot layout: ``functions.
+    mlm_slots_ref``).  ``hidden`` [B*S, H] bf16, ``labels`` [B, S] int64.  Returns ``(x_c
+    [B*P, H] bf16, slot_of_row [B*S] int32, slot_labels [B*P] int64)``; one launch."""
+    _check(hidden, torch.bfloat16, "hidden")
+    if not labels.is_cuda or labels.dtype != torch.int64 or labels.dim() != 2:
+        raise ValueError("labels must be a CUDA int64 [B, S] tensor")
+    B, S = labels.shape
+    H = hidden.shape[-1]
+    if hidden.dim() != 2 or hidden.shape[0] != B * S or not hidden.is_contiguous():
+        raise ValueError("hidden must be a contiguous [B*S, H] tensor")
+    dev = hidden.device
+    x_c = torch.empty((B * P, H), dtype=torch.bfloat16, device=dev)
+    slot_of_row = torch.empty(B * S, dtype=torch.int32, device=dev)
+    slot_labels = torch.empty(B * P, dtype=torch.int64, device=dev)
+    ext().mlm_gather(hidden=hidden.data_ptr(), labels=labels.contiguous().data_ptr(), B=B, S=S,
+                     H=H, P=int(P), ignore_index=int(ignore_index), V=int(V),
+                     slot_of_row=slot_of_row.data_ptr(), slot_labels=slot_labels.data_ptr(),
+                     x_c=x_c.data_ptr(), stream=_stream())
+    return x_c, slot_of_row, slot_labels
+
+
+def mlm_scatter(dx_c: torch.Tensor, slot_of_row: torch.Tensor) -> torch.Tensor:
+    """The input gradient of a sparse head: ``dhidden[r] = dx_c[slot_of_row[r]]`` for a decoded
+    row, zeros otherwise; ``dhidden`` [len(slot_of_row), H] bf16, every row written once."""
+    _check(dx_c, torch.bfloat16, "dx_c")
+    if slot_of_row.dtype != torch.int32 or not slot_of_row.is_cuda:
+        raise ValueError("slot_of_row must be a CUDA int32 tensor")
+    dx_c = dx_c.contiguous()
+    H = dx_c.shape[-1]
+    dhidden = torch.empty((slot_of_row.numel(), H), dtype=torch.bfloat16, device=dx_c.device)
+    ext().mlm_scatter(dx_c=dx_c.data_ptr(), slot_of_row=slot_of_row.data_ptr(),
+                      rows=slot_of_row.numel(), H=H, dhidden=dhidden.data_ptr(), stream=_stream())
+    return dhidden
 
 
 class TokenEvalAccumulator:

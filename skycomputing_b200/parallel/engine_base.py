@@ -202,8 +202,28 @@ class EngineBase:
         label_chunks = labels.chunk(self.m, dim=0) if (self.is_last and labels is not None) else None
         return chunks, label_chunks
 
-    def _last_stage_loss(self, logits, labels):
+    # ------------------------------------------------------------------ labels of the last layer
+    @staticmethod
+    def _bind_labels(st, label_chunks, j: int) -> None:
+        """Before stage ``st`` runs micro-batch ``j``: its labels when the stage's last layer
+        consumes them (a sparse masked-language-model head), none otherwise.  Inside a captured
+        step the chunks are views of the static label buffer."""
+        consumes = getattr(st, "consumes_labels", False)
+        st.labels = label_chunks[j] if (label_chunks is not None and consumes) else None
+
+    @staticmethod
+    def _head_outputs(st, outs, labels):
+        """(logits, labels) that the loss / the evaluation accumulator read from the last stage's
+        outputs: a label-consuming last layer returns its own labels, one per decoded row, as
+        ``outs[1]`` (viewed as [sequences, rows per sequence]); backward still starts at
+        ``outs[0]``."""
+        if getattr(st, "consumes_labels", False):
+            return outs[0], outs[1].view(labels.shape[0], -1)
+        return outs[0], labels
+
+    def _last_stage_loss(self, st, outs, labels):
         """The loss of one micro-batch on the last stage, added into ``_loss_acc``."""
+        logits, labels = self._head_outputs(st, outs, labels)
         if hasattr(self.loss_fn, "fused") and logits.is_cuda and self._loss_acc.dtype == torch.float32:
             # (dlogits,) instead of a scalar loss: see _NativeCrossEntropy.fused
             return (self.loss_fn.fused(logits, labels, 1.0 / self.m, self._loss_acc.view(1)),)
@@ -303,11 +323,11 @@ class EngineBase:
         self._eval_body(inputs, labels, accum, m)
 
     def _eval_body(self, inputs, labels, accum, m: int) -> None:
-        res = self.forward_only(inputs, micro_batches=m)
+        res = self.forward_only(inputs, micro_batches=m, labels=labels if self.is_last else None)
         if self.is_last:
             res = [res] if m == 1 else res
             for outs, lab in zip(res, labels.chunk(m, dim=0)):
-                accum.add(outs[0], lab)
+                accum.add(*self._head_outputs(self.stages[-1], outs, lab))
 
     # ------------------------------------------------------------------ global gradient norm
     def _norm_info(self) -> tuple:

@@ -138,6 +138,7 @@ class PipelineEngine(EngineBase):
     def _forward(self, j: int, args, labels_chunks):
         st = self.stage
         st.microbatch = j
+        self._bind_labels(st, labels_chunks, j)
         st.in_channel = self.fused.prev if self.in_fused else None
         st.out_channel = self.fused.next if self.out_fused else None
         if self.out_fused and not self.is_first:
@@ -148,7 +149,7 @@ class PipelineEngine(EngineBase):
         self._mark(("F", j, "end"))
         if self.out_fused and self.is_first:
             self.fused.next.send_mask(outs[-1], j)  # produced by the embeddings of this stage
-        loss = self._last_stage_loss(outs[0], labels_chunks[j]) if self.is_last else None
+        loss = self._last_stage_loss(st, outs, labels_chunks[j]) if self.is_last else None
         return outs, loss
 
     def _backward(self, j: int, outs, loss, grads, args):
@@ -265,23 +266,30 @@ class PipelineEngine(EngineBase):
         return self._eval_comm_obj
 
     @torch.no_grad()
-    def forward_only(self, inputs: Optional[Sequence[torch.Tensor]] = None, micro_batches: int = 1):
+    def forward_only(self, inputs: Optional[Sequence[torch.Tensor]] = None, micro_batches: int = 1,
+                     labels: Optional[torch.Tensor] = None):
         """Forward through the pipeline without gradients.  The batch is split into
         ``micro_batches`` chunks; sends are asynchronous and waited for at the end of the pass, so
-        stage s runs chunk j + 1 while stage s + 1 runs chunk j.  Returns on the last stage the
-        stage outputs (``micro_batches == 1``) or the list of per-chunk outputs, None elsewhere."""
+        stage s runs chunk j + 1 while stage s + 1 runs chunk j.  ``labels`` (last stage) reach a
+        label-consuming last layer.  Returns on the last stage the stage outputs
+        (``micro_batches == 1``) or the list of per-chunk outputs, None elsewhere."""
         m = int(micro_batches)
         st = self.stage
         st.in_channel = st.out_channel = None
         chunks = [t.chunk(m, dim=0) for t in inputs] if self.is_first else None
+        label_chunks = labels.chunk(m, dim=0) if (self.is_last and labels is not None) else None
         if self.P == 1:
-            results = [st(*(c[j] for c in chunks)) for j in range(m)]
+            results = []
+            for j in range(m):
+                self._bind_labels(st, label_chunks, j)
+                results.append(st(*(c[j] for c in chunks)))
             return results[0] if m == 1 else results
         comm = self._eval_comm()
         comm.forget("eval")   # every pass announces its own shapes
         results, pending, keep = [], [], []
         for j in range(m):
             st.microbatch = j
+            self._bind_labels(st, label_chunks, j)
             if self.is_first:
                 args = tuple(c[j] for c in chunks)
             else:

@@ -143,12 +143,13 @@ class LoopedPipelineEngine(EngineBase):
                 args = tuple(t[j] for t in chunks_in) if first_stage else self._fused_inputs(slot)
                 if not last_stage and not first_stage:
                     self.fused.next.send_mask(args[-1], out_slot)   # the mask travels with the slot
+                self._bind_labels(st, label_chunks if last_stage else None, j)
                 self._mark(("F", slot, "begin"))
                 outs = st(*args)
                 self._mark(("F", slot, "end"))
                 if not last_stage and first_stage:
                     self.fused.next.send_mask(outs[-1], out_slot)   # produced by the embeddings here
-                loss = self._last_stage_loss(outs[0], label_chunks[j]) if last_stage else None
+                loss = self._last_stage_loss(st, outs, label_chunks[j]) if last_stage else None
                 saved[(c, j)] = (outs, loss)
             else:
                 outs, loss = saved.pop((c, j))
@@ -189,10 +190,11 @@ class LoopedPipelineEngine(EngineBase):
                     got, reqs = self.comm.recv(self.prev_rank, f"fwd{c}")
                     self.comm.wait(reqs)
                     args = self._prep_inputs(got)
+                self._bind_labels(st, label_chunks if last_stage else None, j)
                 outs = st(*args)
                 loss = None
                 if last_stage:
-                    loss = self.loss_fn(outs[0], label_chunks[j]) / self.m
+                    loss = self.loss_fn(*self._head_outputs(st, outs, label_chunks[j])) / self.m
                     self._loss_acc += loss.detach().float()
                 else:
                     self._pending_sends += self.comm.send(
@@ -226,13 +228,16 @@ class LoopedPipelineEngine(EngineBase):
 
     # ------------------------------------------------------------------ plain forward (eval)
     @torch.no_grad()
-    def forward_only(self, inputs: Optional[Sequence[torch.Tensor]] = None, micro_batches: int = 1):
+    def forward_only(self, inputs: Optional[Sequence[torch.Tensor]] = None, micro_batches: int = 1,
+                     labels: Optional[torch.Tensor] = None):
         """Breadth-first forward of every (chunk, micro-batch) without gradients; sends are
-        asynchronous and waited for at the end of the pass.  Returns on the rank that owns the last
+        asynchronous and waited for at the end of the pass.  ``labels`` (rank of the last virtual
+        stage) reach a label-consuming last layer.  Returns on the rank that owns the last
         virtual stage its outputs (``micro_batches == 1``) or the list of per-chunk outputs."""
         m = int(micro_batches)
         comm = self.comm
         chunks_in = [t.chunk(m, dim=0) for t in inputs] if self.is_first else None
+        label_chunks = labels.chunk(m, dim=0) if (self.is_last and labels is not None) else None
         results, pending, keep = [], [], []
         for c, st in enumerate(self.stages):
             comm.forget(f"eval{c}")
@@ -240,6 +245,7 @@ class LoopedPipelineEngine(EngineBase):
             st.in_channel = st.out_channel = None
             for j in range(m):
                 st.microbatch = c * m + j
+                self._bind_labels(st, label_chunks if k == self.total - 1 else None, j)
                 if k == 0:
                     args = tuple(t[j] for t in chunks_in)
                 else:

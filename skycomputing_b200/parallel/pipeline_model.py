@@ -138,6 +138,11 @@ class RpcModel(nn.Module):
                 module = LocalModule(rank=worker.rank, model_cfg=model_cfg,
                                      sequential_wrapper_cfg=cfg, device_rank=dev,
                                      layer_range=layer_range)
+                if module.module.consumes_labels and k != D * self.virtual_stages - 1:
+                    # only the last stage receives the labels
+                    raise ValueError("pipeline stage {} of {} ends with a layer that consumes "
+                                     "labels; it must be the model's last layer".format(
+                                         k, D * self.virtual_stages))
             else:
                 module = RemoteModule(rank=worker.rank, model_cfg=model_cfg,
                                       sequential_wrapper_cfg=cfg, device_rank=dev,

@@ -403,6 +403,10 @@ class Runner:
                 payload = dict(classification_metrics(totals["confusion"], totals["loss_sum"],
                                                       totals["count"]),
                                invalid=totals["invalid"], classes=len(totals["confusion"]))
+            if payload is not None:
+                last = eng.stages[-1]
+                payload["max_predictions"] = (getattr(last.layers[-1], "max_predictions", None)
+                                              if getattr(last, "consumes_labels", False) else None)
             if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
                 box = [payload]
                 dist.broadcast_object_list(box, src=self.model.stage_to_rank[-1])
@@ -411,9 +415,16 @@ class Runner:
             self.model.train(was_training)
             torch.random.set_rng_state(cpu_rng)
         invalid, classes = payload.pop("invalid"), payload.pop("classes")
+        max_predictions = payload.pop("max_predictions")
         if invalid:
-            raise ValueError("evaluation {}: {} labels are outside [0, {}) and not ignore_index "
-                             "({})".format(name, invalid, classes, ignore_index))
+            msg = "evaluation {}: {} labels are outside [0, {}) and not ignore_index ({})".format(
+                name, invalid, classes, ignore_index)
+            if max_predictions is not None:
+                msg += ("; the sparse masked-language-model head decodes at most max_predictions = "
+                        "{} labelled positions per sequence, and a sequence with more gets the "
+                        "out-of-range label {} in its last slot: raise max_predictions or label "
+                        "fewer positions".format(max_predictions, classes))
+            raise ValueError(msg)
         self._call_hook("after_val_epoch")
         self._log("eval {}: {}".format(name, format_metrics(payload)))
         if self._metrics_path is not None:

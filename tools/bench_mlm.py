@@ -1,7 +1,8 @@
 """Masked-language-model pretraining cost on one GPU, at the geometry of ``bench.py --gpus 1``
 (BERT-large, 24 blocks, 32 sequences of 128 tokens, one CUDA graph per step).
 
-    python tools/bench_mlm.py [--steps 20] [--rounds 5] [--layers 24] [--out FILE]
+    python tools/bench_mlm.py [--steps 20] [--rounds 5] [--layers 24] [--max-predictions P]
+                              [--out FILE]
 
 Reports, after the card's name and power limit (read in the same run):
 * ms/step of training with the BertTailForMaskedLM head + MaskedLMLoss against the pooler +
@@ -12,6 +13,12 @@ Reports, after the card's name and power limit (read in the same run):
   not read rows whose label is ignore_index, so with the 15 % MLM labelling it moves less than
   that floor; both label densities are timed;
 * the decoder GEMM ([4096, 1024] x [30528, 1024]^T + bias, bf16 out) in TFLOP/s.
+With ``--max-predictions P`` the sparse head (``BertTailForMaskedLM(max_predictions=P)``, only the
+labelled positions decoded) joins the alternating windows as a third arm, each arm's peak memory
+(weights, optimizer state, activations and graph pool, measured from its construction through its
+warm-up) is reported, and the mlm_gather / mlm_scatter kernels are timed against their byte
+floors at the benchmark's geometry with the dataset's 15 % labelling (graph replays: the
+wrappers' host time exceeds these kernels' device time).
 Kernel times are CUDA-event means over 50 launches after 5 warm-up launches.
 """
 from __future__ import annotations
@@ -42,14 +49,17 @@ def card() -> dict:
     return dict(name=name, power_limit=power, max_sm_clock=clock)
 
 
-def build_runner(layers: int, mlm: bool):
+def build_runner(layers: int, mlm: bool, max_predictions=None):
     cfg = sky.BertConfig.bert_large()
     if mlm:
         cfg.vocab_size = V
     enc = [dict(layer_type="BertLayer_Head", config=cfg.__dict__),
            dict(layer_type="BertLayer_Body", config=cfg.__dict__),
            dict(layer_type="BertLayer_Tail", config=cfg.__dict__)] * layers
-    tail = ([dict(layer_type="BertTailForMaskedLM", config=cfg.__dict__)] if mlm else
+    head = dict(layer_type="BertTailForMaskedLM", config=cfg.__dict__)
+    if max_predictions is not None:
+        head["max_predictions"] = max_predictions
+    tail = ([head] if mlm else
             [dict(layer_type="BertPooler", config=cfg.__dict__),
              dict(layer_type="BertTailForClassification", hidden_dropout_prob=0.1,
                   hidden_size=cfg.hidden_size, num_classes=3)])
@@ -102,12 +112,62 @@ def kernel_ms(fn, iters: int = 50, warmup: int = 5) -> float:
     return e0.elapsed_time(e1) / iters
 
 
+def graph_kernel_ms(fn, iters: int = 50, replays: int = 20) -> float:
+    """Device time of a call whose host side (allocations, argument checks) takes longer than its
+    kernel: ``iters`` calls captured in one CUDA graph, mean over ``replays`` replays."""
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        fn()
+    torch.cuda.current_stream().wait_stream(s)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        for _ in range(iters):
+            fn()
+    g.replay()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(replays):
+        g.replay()
+    e1.record()
+    e1.synchronize()
+    return e0.elapsed_time(e1) / (replays * iters)
+
+
+def slot_kernels(P: int) -> dict:
+    """mlm_gather / mlm_scatter at the benchmark's geometry against their byte floors."""
+    H = 1024
+    ds = sky.SynthMLMDataset(num_samples=B, max_seq_length=S, vocab_size=V, seed=0)
+    _, labels = next(iter(torch.utils.data.DataLoader(ds, batch_size=B)))
+    labels = labels.cuda()
+    g = torch.Generator(device="cuda").manual_seed(1)
+    hidden = torch.randn(B * S, H, generator=g, device="cuda").to(torch.bfloat16)
+    x_c, slot_of_row, _ = nat.mlm_gather(hidden, labels, P, V)
+    dx_c = torch.randn(B * P, H, generator=g, device="cuda").to(torch.bfloat16)
+    decoded = min(int((labels != -100).sum()), B * P)
+    # gather: labels read, the decoded rows read, the slots written, the two maps written
+    gather_bytes = B * S * 8 + decoded * H * 2 + B * P * H * 2 + B * S * 4 + B * P * 8
+    # scatter: the slot map read, the decoded slots read, every row of dhidden written
+    scatter_bytes = B * S * 4 + decoded * H * 2 + B * S * H * 2
+    out = {}
+    for name, fn, nbytes in (
+            ("mlm_gather", lambda: nat.mlm_gather(hidden, labels, P, V), gather_bytes),
+            ("mlm_scatter", lambda: nat.mlm_scatter(dx_c, slot_of_row), scatter_bytes)):
+        t = graph_kernel_ms(fn)
+        floor_ms = nbytes / HBM_BYTES_PER_S * 1e3
+        out[name] = dict(ms=t, bytes=nbytes, byte_floor_ms=floor_ms, floor_over_time=floor_ms / t)
+        print("{} B={} S={} H={} P={}: {:.1f} us, byte floor {:.2f} us ({:.2f} of the floor's "
+              "time)".format(name, B, S, H, P, t * 1e3, floor_ms * 1e3, floor_ms / t), flush=True)
+    return out
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--layers", type=int, default=24)
+    ap.add_argument("--max-predictions", type=int, default=None)
     ap.add_argument("--out", type=str, default=None)
     args = ap.parse_args()
     if not (torch.cuda.is_available() and nat.available()):
@@ -119,12 +179,21 @@ def main() -> None:
           flush=True)
 
     # --- whole steps, alternating windows ---
-    runs = {name: build_runner(args.layers, name == "mlm") for name in ("cls", "mlm")}
-    for name, (runner, inputs, labels) in runs.items():
+    P = args.max_predictions
+    runs, peak_mib = {}, {}
+    for name in ("cls", "mlm") + (("mlm_sparse",) if P else ()):
+        if P:
+            torch.cuda.synchronize()
+            base = torch.cuda.memory_allocated()
+            torch.cuda.reset_peak_memory_stats()
+        runs[name] = build_runner(args.layers, name != "cls", P if name == "mlm_sparse" else None)
+        runner, inputs, labels = runs[name]
         for _ in range(args.warmup):
             runner.engine.train_step(inputs, labels)
         torch.cuda.synchronize()
         assert runner.engine._graph is not None, name
+        if P:
+            peak_mib[name] = (torch.cuda.max_memory_allocated() - base) / 2 ** 20
     times = {name: [] for name in runs}
     for _ in range(args.rounds):
         for name, (runner, inputs, labels) in runs.items():
@@ -140,6 +209,16 @@ def main() -> None:
     print("step ms (median of {} windows x {} steps): cls {:.3f}, mlm {:.3f} ({:.2f}x)".format(
         args.rounds, args.steps, steps["cls"]["median_ms"], steps["mlm"]["median_ms"],
         steps["mlm_over_cls"]), flush=True)
+    if P:
+        steps["mlm_sparse_over_cls"] = steps["mlm_sparse"]["median_ms"] / steps["cls"]["median_ms"]
+        res["step"].update(mlm_sparse_over_cls=steps["mlm_sparse_over_cls"], max_predictions=P)
+        res["peak_mib"] = peak_mib
+        print("sparse head (P = {}): mlm_sparse {:.3f} ms ({:.2f}x), {:.3f} ms less than the dense "
+              "head".format(P, steps["mlm_sparse"]["median_ms"], steps["mlm_sparse_over_cls"],
+                            steps["mlm"]["median_ms"] - steps["mlm_sparse"]["median_ms"]), flush=True)
+        print("peak MiB: " + ", ".join("{} {:.0f}".format(k, v) for k, v in peak_mib.items()),
+              flush=True)
+        res["mlm_slots"] = slot_kernels(P)
 
     # --- vocab_ce kernel ---
     M = B * S

@@ -7,6 +7,9 @@ pipelines cut at different places can be compared (dropout off => the same math 
                    stage boundary is fused (peer-memory slots, one CUDA graph per step)
     --cut head     the last stage is the head alone: the cut sits directly in front of it, and the
                    boundary runs over torch.distributed p2p (the head does not consume a fused slot)
+    --max-predictions P
+                   the sparse head: only the labelled positions (at most P per sequence) are
+                   decoded; the labels reach the head on the last stage
 """
 import argparse
 import json
@@ -30,6 +33,7 @@ def main():
     ap.add_argument("--layers", type=int, default=4)
     ap.add_argument("--steps", type=int, default=6)
     ap.add_argument("--batch", type=int, default=16)
+    ap.add_argument("--max-predictions", type=int, default=None)
     a = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -45,8 +49,10 @@ def main():
     enc = [dict(layer_type="BertLayer_Head", config=cfg.__dict__),
            dict(layer_type="BertLayer_Body", config=cfg.__dict__),
            dict(layer_type="BertLayer_Tail", config=cfg.__dict__)] * a.layers
-    model_config = ([dict(layer_type="BertEmbeddings", config=cfg.__dict__)] + enc
-                    + [dict(layer_type="BertTailForMaskedLM", config=cfg.__dict__)])
+    head = dict(layer_type="BertTailForMaskedLM", config=cfg.__dict__)
+    if a.max_predictions is not None:
+        head["max_predictions"] = a.max_predictions
+    model_config = [dict(layer_type="BertEmbeddings", config=cfg.__dict__)] + enc + [head]
     workers = [dict(name=f"gpu-{i}", server_config={}, device=i,
                     extra_config=dict(module_to_cuda=True, cuda_device=local, slowdown=0,
                                       mem_limit=-1, timer_config=dict(root="/tmp/sky_check_mlm")))

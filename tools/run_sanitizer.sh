@@ -8,6 +8,8 @@
 #         layers   embeddings + block + pooler + classifier through the layer classes (embed_fwd /
 #                  embed_bwd / small_linear kernels) and the flag handshake (peer_copy_signal,
 #                  wait_flags, flag-gated GEMM) on one GPU
+#         mlm      the sparse masked-language-model slot kernels (mlm_gather / mlm_scatter) over
+#                  the shape grid, and one graph replayed with different label counts
 #         all      everything above (default)
 # Runs on ONE GPU; reports land in bench_out/sanitizer_<tool>_<suite>.log.  The sanitizer slows
 # kernels 10-100x: the 4 s flag-wait timeouts are only meaningful under memcheck / synccheck.
@@ -31,6 +33,9 @@ case "$SUITE" in rows|all)
 esac
 case "$SUITE" in attn|all)
   run attn tests/test_kernels_gpu.py -k "attention" ;;
+esac
+case "$SUITE" in mlm|all)
+  run mlm tests/test_mlm_sparse_gpu.py -k "gather_and_scatter or different_label_counts" ;;
 esac
 case "$SUITE" in layers|all)
   run layers tests/test_layers_gpu.py tests/test_kernels_gpu.py -k "embeddings_pooler_classifier or handshake or signals_panels" ;;
