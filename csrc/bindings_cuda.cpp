@@ -338,6 +338,56 @@ void adam_multi(uintptr_t d_tensors, int n, long long max_numel, float lr, float
                                zero_grad, S(stream), P<const sky::OptimScalars>(scalars)),
         "adam_multi");
 }
+// segments: list of (p, g, m, v, p_bf16, numel, weight_decay, use_ratio, skip_zero) -> (packed
+// LambSegment bytes, packed int32 chunk -> segment table, n_chunks, [vec flag per segment])
+py::tuple pack_lamb_segments(
+    const std::vector<std::tuple<uintptr_t, uintptr_t, uintptr_t, uintptr_t, uintptr_t, long long,
+                                 float, int, int>>& ts) {
+  std::vector<sky::LambSegment> v(ts.size());
+  long long cap = 0;
+  for (size_t i = 0; i < ts.size(); ++i) {
+    sky::LambSegment& s = v[i];
+    s.p = P<float>(std::get<0>(ts[i]));
+    s.g = P<float>(std::get<1>(ts[i]));
+    s.m = P<float>(std::get<2>(ts[i]));
+    s.v = P<float>(std::get<3>(ts[i]));
+    s.p_bf16 = P<void>(std::get<4>(ts[i]));
+    s.numel = std::get<5>(ts[i]);
+    s.weight_decay = std::get<6>(ts[i]);
+    s.use_ratio = std::get<7>(ts[i]);
+    s.skip_zero = std::get<8>(ts[i]);
+    s.vec = s.chunk0 = s.n_chunks = 0;
+    if (s.numel > 0) cap += sky::lamb_chunks(s.numel);
+  }
+  std::vector<int> chunk_seg(static_cast<size_t>(cap));
+  int n_chunks = 0;
+  check(sky::lamb_prepare(v.data(), static_cast<int>(v.size()), chunk_seg.data(), cap, &n_chunks),
+        "pack_lamb_segments");
+  py::list vec;
+  for (const auto& s : v) vec.append(s.vec != 0);
+  return py::make_tuple(
+      py::bytes(reinterpret_cast<const char*>(v.data()), v.size() * sizeof(sky::LambSegment)),
+      py::bytes(reinterpret_cast<const char*>(chunk_seg.data()), chunk_seg.size() * sizeof(int)),
+      n_chunks, vec);
+}
+void lamb_moments(uintptr_t segs, uintptr_t chunk_seg, int n_chunks, float beta1, float beta2,
+                  float eps, uintptr_t step, float grad_scale, uintptr_t partials, uintptr_t stream,
+                  uintptr_t scalars) {
+  check(sky::launch_lamb_moments(P<const sky::LambSegment>(segs), P<const int>(chunk_seg),
+                                 n_chunks, beta1, beta2, eps, P<const uint64_t>(step), grad_scale,
+                                 P<float2>(partials), S(stream),
+                                 P<const sky::OptimScalars>(scalars)),
+        "lamb_moments");
+}
+void lamb_update(uintptr_t segs, uintptr_t chunk_seg, int n_chunks, float lr, float beta1,
+                 float beta2, float eps, uintptr_t step, uintptr_t partials, uintptr_t ratios,
+                 uintptr_t stream, uintptr_t scalars) {
+  check(sky::launch_lamb_update(P<const sky::LambSegment>(segs), P<const int>(chunk_seg), n_chunks,
+                                lr, beta1, beta2, eps, P<const uint64_t>(step),
+                                P<const float2>(partials), P<float>(ratios), S(stream),
+                                P<const sky::OptimScalars>(scalars)),
+        "lamb_update");
+}
 void grad_sumsq_multi(uintptr_t d_tensors, int n, int blocks, float grad_scale, uintptr_t partials,
                       uintptr_t stream) {
   check(sky::launch_grad_sumsq_multi(P<const sky::SgdTensor>(d_tensors), n, blocks, grad_scale,
@@ -540,6 +590,15 @@ PYBIND11_MODULE(_cuda, m) {
         py::arg("weight_decay") = 0.f, py::arg("decoupled") = false, py::arg("step") = 0,
         py::arg("grad_scale") = 1.f, py::arg("zero_grad") = true, py::arg("stream") = 0,
         py::arg("scalars") = 0);
+  m.def("pack_lamb_segments", &pack_lamb_segments);
+  m.attr("LAMB_CHUNK") = sky::kLambChunk;
+  m.def("lamb_moments", &lamb_moments, py::arg("segs"), py::arg("chunk_seg"), py::arg("n_chunks"),
+        py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("step"),
+        py::arg("grad_scale") = 1.f, py::arg("partials"), py::arg("stream") = 0,
+        py::arg("scalars") = 0);
+  m.def("lamb_update", &lamb_update, py::arg("segs"), py::arg("chunk_seg"), py::arg("n_chunks"),
+        py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("step"),
+        py::arg("partials"), py::arg("ratios"), py::arg("stream") = 0, py::arg("scalars") = 0);
   m.def("grad_sumsq_blocks", &sky::grad_sumsq_blocks, py::arg("max_numel"));
   m.def("grad_sumsq_multi", &grad_sumsq_multi, py::arg("d_tensors"), py::arg("n"),
         py::arg("blocks"), py::arg("grad_scale") = 1.f, py::arg("partials"), py::arg("stream") = 0);

@@ -335,6 +335,48 @@ int launch_adam_multi(const SgdTensor* d_tensors, int n_tensors, long long max_n
 int grad_sumsq_blocks(long long max_numel);
 int launch_grad_sumsq_multi(const SgdTensor* d_tensors, int n_tensors, int blocks,
                             float grad_scale, float* partials, cudaStream_t stream);
+// LAMB (You et al. 2019, apex FusedLAMB defaults: adam_w_mode, grad averaging, bias correction,
+// no NVLAMB).  One segment per nn.Parameter inside the flat banks, each with its own trust ratio:
+//   g = grad * grad_scale * clip_coef,  m = b1 m + (1-b1) g,  v = b2 v + (1-b2) g^2,
+//   u = (m / (1-b1^t)) / (sqrt(v / (1-b2^t)) + eps) + wd p,
+//   r = ||p|| / ||u|| if use_ratio and both norms > 0, else 1,   p -= lr r u.
+// Work is handed out in kLambChunk-element chunks of the segments (chunk c belongs to segment
+// chunk_seg[c]); each block takes a contiguous range of chunks.
+constexpr int kLambChunk = 16384;
+struct LambSegment {
+  float* p;           // fp32 master (the segment's first element)
+  float* g;           // fp32 gradient
+  float* m;           // first moment
+  float* v;           // second moment
+  void* p_bf16;       // bf16 shadow, may be null
+  long long numel;
+  float weight_decay; // lambda (0 for a tensor excluded from weight decay)
+  int use_ratio;      // apply the trust ratio (lambda != 0)
+  int skip_zero;      // leave g as it is: the next step's first wgrad overwrites it
+  int vec;            // float4 path (p, g, m, v 16-byte, p_bf16 8-byte aligned); set by lamb_prepare
+  int chunk0;         // index of the segment's first chunk
+  int n_chunks;
+};
+// Host side, once per table: checks the segments, sets vec / chunk0 / n_chunks and fills
+// chunk_seg[0 .. *n_chunks) (capacity `cap`).  Errors: 970 null pointer, numel < 1, a fp32 pointer
+// not 4-byte aligned or more than `cap` / INT_MAX chunks; 972 a bf16 shadow not 2-byte aligned.
+int lamb_prepare(LambSegment* segs, int n_segments, int* chunk_seg, long long cap, int* n_chunks);
+long long lamb_chunks(long long numel);
+// Pass 1: m and v, and the fp32 partials {sum p^2, sum u^2} of every chunk into partials[c]
+// (fixed slots, fixed in-block order: bit-identical on every call); zeroes g unless skip_zero.
+// Pass 2: r from the segment's partials (summed in fp64 in a fixed order), p -= lr r u (u
+// recomputed from the new m, v and the old p), the bf16 shadow from the new p; the block holding a
+// segment's first chunk writes its r to ratios[segment].  `step` is the device step counter
+// (1-based, advanced before pass 1); with `scalars` lr and clip_coef come from the device.
+// Errors: 970 bad table / null buffer, 971 null step counter.
+int launch_lamb_moments(const LambSegment* segs, const int* chunk_seg, int n_chunks, float beta1,
+                        float beta2, float eps, const uint64_t* step, float grad_scale,
+                        float2* partials, cudaStream_t stream,
+                        const OptimScalars* scalars = nullptr);
+int launch_lamb_update(const LambSegment* segs, const int* chunk_seg, int n_chunks, float lr,
+                       float beta1, float beta2, float eps, const uint64_t* step,
+                       const float2* partials, float* ratios, cudaStream_t stream,
+                       const OptimScalars* scalars = nullptr);
 // Learning-rate schedules f(k) of launch_optim_finalize (lr = base_lr * f(k)).
 enum LrScheduleType : int { kLrNone = 0, kLrConstant = 1, kLrLinear = 2, kLrCosine = 3 };
 // Cross-rank exchange of the local sums of squares through peer memory (CUDA IPC).  Every rank

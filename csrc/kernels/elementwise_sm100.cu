@@ -12,6 +12,8 @@
 //   nn.CrossEntropyLoss      scaelum/runner/runner.py:51-52,131     -> softmax_ce
 //   optim.SGD step           experiment/launch.py:152-155           -> sgd_multi
 //   time.sleep slowdown      scaelum/builder/module_wrapper.py:124-126,265-266 -> spin_* kernels
+#include <algorithm>
+
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -1310,6 +1312,183 @@ optim_finalize_kernel(const float* __restrict__ partials, int n_partials,
   out->local_sumsq = local_f;
 }
 
+// LAMB, two passes over the segment / chunk table (api.h).  Block b takes the contiguous chunk
+// range [b * n / G, (b + 1) * n / G): every chunk is at most kLambChunk elements, so the blocks
+// carry equal work whether a segment is a 1K bias or the 31M-element word-embedding table, and a
+// block meets only the few segments its range crosses.  A chunk's partials depend only on the
+// chunk, never on G or on which block ran it.
+struct LambBias {
+  float inv_bc1, inv_bc2;
+};
+__device__ __forceinline__ LambBias lamb_bias(const uint64_t* step, float beta1, float beta2) {
+  const double t = static_cast<double>(*step);
+  return {static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(beta1), t))),
+          static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(beta2), t)))};
+}
+// the Adam-style update plus decay; both passes call this one function on the same m, v, p
+__device__ __forceinline__ float lamb_u(float m, float v, float p, LambBias bc, float eps,
+                                        float wd) {
+  return (m * bc.inv_bc1) / (sqrtf(v * bc.inv_bc2) + eps) + wd * p;
+}
+__device__ __forceinline__ void lamb_chunk_range(int n_chunks, int& c0, int& c1) {
+  c0 = static_cast<int>(static_cast<long long>(blockIdx.x) * n_chunks / gridDim.x);
+  c1 = static_cast<int>(static_cast<long long>(blockIdx.x + 1) * n_chunks / gridDim.x);
+}
+
+template <bool kScalars>
+__global__ void __launch_bounds__(256)
+lamb_moments_kernel(const LambSegment* __restrict__ segs, const int* __restrict__ chunk_seg,
+                    int n_chunks, float beta1, float beta2, float eps,
+                    const uint64_t* __restrict__ step, float grad_scale,
+                    const OptimScalars* __restrict__ sc, float2* __restrict__ partials) {
+  const float clip = kScalars ? sc->clip_coef : 1.f;
+  const LambBias bc = lamb_bias(step, beta1, beta2);
+  __shared__ float red[2][8];
+  int c0, c1;
+  lamb_chunk_range(n_chunks, c0, c1);
+  for (int c = c0; c < c1; ++c) {
+    const LambSegment s = segs[chunk_seg[c]];
+    const long long base = static_cast<long long>(c - s.chunk0) * kLambChunk;
+    const int len = static_cast<int>(min(static_cast<long long>(kLambChunk), s.numel - base));
+    const float wd = s.weight_decay;
+    float w2 = 0.f, u2 = 0.f;
+    auto one = [&](float p, float gi, float& m, float& v) {
+      const float g = scaled_grad<kScalars>(gi, grad_scale, clip);
+      m = beta1 * m + (1.f - beta1) * g;
+      v = beta2 * v + (1.f - beta2) * g * g;
+      const float u = lamb_u(m, v, p, bc, eps, wd);
+      w2 += p * p;
+      u2 += u * u;
+    };
+    float* p = s.p + base;
+    float* g = s.g + base;
+    float* m = s.m + base;
+    float* v = s.v + base;
+    int scalar_from = 0;
+    if (s.vec) {
+      const int n4 = len >> 2;
+      for (int i = threadIdx.x; i < n4; i += blockDim.x) {
+        const float4 pp = reinterpret_cast<const float4*>(p)[i];
+        const float4 gg = reinterpret_cast<const float4*>(g)[i];
+        float4 mm = reinterpret_cast<const float4*>(m)[i];
+        float4 vv = reinterpret_cast<const float4*>(v)[i];
+        one(pp.x, gg.x, mm.x, vv.x);
+        one(pp.y, gg.y, mm.y, vv.y);
+        one(pp.z, gg.z, mm.z, vv.z);
+        one(pp.w, gg.w, mm.w, vv.w);
+        reinterpret_cast<float4*>(m)[i] = mm;
+        reinterpret_cast<float4*>(v)[i] = vv;
+        if (!s.skip_zero) reinterpret_cast<float4*>(g)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      scalar_from = n4 << 2;
+    }
+    for (int i = scalar_from + threadIdx.x; i < len; i += blockDim.x) {
+      float mi = m[i], vi = v[i];
+      one(p[i], g[i], mi, vi);
+      m[i] = mi;
+      v[i] = vi;
+      if (!s.skip_zero) g[i] = 0.f;
+    }
+    w2 = warp_sum(w2);
+    u2 = warp_sum(u2);
+    if ((threadIdx.x & 31) == 0) {
+      red[0][threadIdx.x >> 5] = w2;
+      red[1][threadIdx.x >> 5] = u2;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float a = 0.f, b = 0.f;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) {
+        a += red[0][w];
+        b += red[1][w];
+      }
+      partials[c] = make_float2(a, b);
+    }
+    __syncthreads();
+  }
+}
+
+template <bool kScalars>
+__global__ void __launch_bounds__(256)
+lamb_update_kernel(const LambSegment* __restrict__ segs, const int* __restrict__ chunk_seg,
+                   int n_chunks, float lr, float beta1, float beta2, float eps,
+                   const uint64_t* __restrict__ step, const OptimScalars* __restrict__ sc,
+                   const float2* __restrict__ partials, float* __restrict__ ratios) {
+  if constexpr (kScalars) lr = sc->lr;
+  const LambBias bc = lamb_bias(step, beta1, beta2);
+  __shared__ double red[2][256];
+  __shared__ float ratio_s;
+  int c0, c1;
+  lamb_chunk_range(n_chunks, c0, c1);
+  int cur = -1;
+  float r = 1.f;
+  for (int c = c0; c < c1; ++c) {
+    const int si = chunk_seg[c];
+    const LambSegment s = segs[si];
+    if (si != cur) {   // block-uniform: the trust ratio of a segment this block enters
+      cur = si;
+      r = 1.f;
+      if (s.use_ratio) {
+        double a = 0.0, b = 0.0;
+        for (int k = threadIdx.x; k < s.n_chunks; k += blockDim.x) {
+          const float2 q = partials[s.chunk0 + k];
+          a += q.x;
+          b += q.y;
+        }
+        red[0][threadIdx.x] = a;
+        red[1][threadIdx.x] = b;
+        __syncthreads();
+        for (int h = 128; h > 0; h >>= 1) {
+          if (threadIdx.x < h) {
+            red[0][threadIdx.x] += red[0][threadIdx.x + h];
+            red[1][threadIdx.x] += red[1][threadIdx.x + h];
+          }
+          __syncthreads();
+        }
+        if (threadIdx.x == 0) {
+          const double wn = sqrt(red[0][0]), un = sqrt(red[1][0]);
+          ratio_s = (wn > 0.0 && un > 0.0) ? static_cast<float>(wn / un) : 1.f;
+        }
+        __syncthreads();
+        r = ratio_s;
+      }
+    }
+    if (c == s.chunk0 && threadIdx.x == 0) ratios[si] = r;
+    const long long base = static_cast<long long>(c - s.chunk0) * kLambChunk;
+    const int len = static_cast<int>(min(static_cast<long long>(kLambChunk), s.numel - base));
+    const float wd = s.weight_decay;
+    const float step_lr = lr * r;
+    float* p = s.p + base;
+    const float* m = s.m + base;
+    const float* v = s.v + base;
+    int scalar_from = 0;
+    if (s.vec) {
+      const int n4 = len >> 2;
+      uint2* b4 = s.p_bf16 ? reinterpret_cast<uint2*>(static_cast<__nv_bfloat16*>(s.p_bf16) + base)
+                           : nullptr;
+      for (int i = threadIdx.x; i < n4; i += blockDim.x) {
+        float4 pp = reinterpret_cast<const float4*>(p)[i];
+        const float4 mm = reinterpret_cast<const float4*>(m)[i];
+        const float4 vv = reinterpret_cast<const float4*>(v)[i];
+        pp.x -= step_lr * lamb_u(mm.x, vv.x, pp.x, bc, eps, wd);
+        pp.y -= step_lr * lamb_u(mm.y, vv.y, pp.y, bc, eps, wd);
+        pp.z -= step_lr * lamb_u(mm.z, vv.z, pp.z, bc, eps, wd);
+        pp.w -= step_lr * lamb_u(mm.w, vv.w, pp.w, bc, eps, wd);
+        reinterpret_cast<float4*>(p)[i] = pp;
+        if (b4 != nullptr) b4[i] = make_uint2(pack_bf16x2(pp.x, pp.y), pack_bf16x2(pp.z, pp.w));
+      }
+      scalar_from = n4 << 2;
+    }
+    __nv_bfloat16* b = s.p_bf16 ? static_cast<__nv_bfloat16*>(s.p_bf16) + base : nullptr;
+    for (int i = scalar_from + threadIdx.x; i < len; i += blockDim.x) {
+      const float pi = p[i] - step_lr * lamb_u(m[i], v[i], p[i], bc, eps, wd);
+      p[i] = pi;
+      if (b != nullptr) b[i] = __float2bfloat16(pi);
+    }
+  }
+}
+
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ s, __nv_bfloat16* __restrict__ d,
                                      long long n) {
   const long long n4 = n >> 2;
@@ -1751,6 +1930,82 @@ int launch_optim_finalize(const float* partials, int n_partials, const float* ex
     return 909;
   optim_finalize_kernel<<<1, 256, 0, stream>>>(partials, n_partials, extra_sumsq, ex, step,
                                                step_offset, schedule, warmup, total, base_lr, max_norm, out);
+  SKY_LAUNCH_CHECK();
+}
+
+long long lamb_chunks(long long numel) { return (numel + kLambChunk - 1) / kLambChunk; }
+
+int lamb_prepare(LambSegment* segs, int n_segments, int* chunk_seg, long long cap, int* n_chunks) {
+  if (n_segments < 0 || (n_segments > 0 && segs == nullptr) || n_chunks == nullptr) return 970;
+  auto al = [](const void* q, uintptr_t a) { return reinterpret_cast<uintptr_t>(q) % a == 0; };
+  long long total = 0;
+  for (int i = 0; i < n_segments; ++i) {
+    LambSegment& s = segs[i];
+    if (!s.p || !s.g || !s.m || !s.v || s.numel < 1) return 970;
+    if (!al(s.p, 4) || !al(s.g, 4) || !al(s.m, 4) || !al(s.v, 4)) return 970;
+    if (s.p_bf16 != nullptr && !al(s.p_bf16, 2)) return 972;
+    s.vec = al(s.p, 16) && al(s.g, 16) && al(s.m, 16) && al(s.v, 16) &&
+            (s.p_bf16 == nullptr || al(s.p_bf16, 8));
+    const long long c = lamb_chunks(s.numel);
+    if (total + c > cap || total + c > 0x7fffffffLL) return 970;
+    s.chunk0 = static_cast<int>(total);
+    s.n_chunks = static_cast<int>(c);
+    for (long long k = 0; k < c; ++k) chunk_seg[total + k] = i;
+    total += c;
+  }
+  *n_chunks = static_cast<int>(total);
+  return 0;
+}
+
+namespace {
+// resident blocks of `kernel` (256 threads) on the whole device: the grid of both LAMB passes,
+// so that the contiguous chunk ranges run in one wave
+template <typename K>
+int lamb_grid(K kernel, int n_chunks) {
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 256, 0) != cudaSuccess ||
+      per_sm < 1)
+    per_sm = 1;
+  return n_chunks < per_sm * num_sms() ? n_chunks : per_sm * num_sms();
+}
+}  // namespace
+
+int launch_lamb_moments(const LambSegment* segs, const int* chunk_seg, int n_chunks, float beta1,
+                        float beta2, float eps, const uint64_t* step, float grad_scale,
+                        float2* partials, cudaStream_t stream, const OptimScalars* scalars) {
+  if (n_chunks == 0) return 0;
+  if (n_chunks < 0 || segs == nullptr || chunk_seg == nullptr || partials == nullptr) return 970;
+  if (step == nullptr) return 971;
+  if (scalars != nullptr) {
+    static const int grid = lamb_grid(lamb_moments_kernel<true>, 1 << 30);
+    lamb_moments_kernel<true><<<std::min(grid, n_chunks), 256, 0, stream>>>(
+        segs, chunk_seg, n_chunks, beta1, beta2, eps, step, grad_scale, scalars, partials);
+  } else {
+    static const int grid = lamb_grid(lamb_moments_kernel<false>, 1 << 30);
+    lamb_moments_kernel<false><<<std::min(grid, n_chunks), 256, 0, stream>>>(
+        segs, chunk_seg, n_chunks, beta1, beta2, eps, step, grad_scale, nullptr, partials);
+  }
+  SKY_LAUNCH_CHECK();
+}
+
+int launch_lamb_update(const LambSegment* segs, const int* chunk_seg, int n_chunks, float lr,
+                       float beta1, float beta2, float eps, const uint64_t* step,
+                       const float2* partials, float* ratios, cudaStream_t stream,
+                       const OptimScalars* scalars) {
+  if (n_chunks == 0) return 0;
+  if (n_chunks < 0 || segs == nullptr || chunk_seg == nullptr || partials == nullptr ||
+      ratios == nullptr)
+    return 970;
+  if (step == nullptr) return 971;
+  if (scalars != nullptr) {
+    static const int grid = lamb_grid(lamb_update_kernel<true>, 1 << 30);
+    lamb_update_kernel<true><<<std::min(grid, n_chunks), 256, 0, stream>>>(
+        segs, chunk_seg, n_chunks, lr, beta1, beta2, eps, step, scalars, partials, ratios);
+  } else {
+    static const int grid = lamb_grid(lamb_update_kernel<false>, 1 << 30);
+    lamb_update_kernel<false><<<std::min(grid, n_chunks), 256, 0, stream>>>(
+        segs, chunk_seg, n_chunks, lr, beta1, beta2, eps, step, nullptr, partials, ratios);
+  }
   SKY_LAUNCH_CHECK();
 }
 

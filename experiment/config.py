@@ -49,6 +49,14 @@ if TASK not in ("cls", "mlm"):
 # sequence (P >= round(0.15 * (SEQ_LEN - 2)): 20 at 128 tokens); unset = every position decoded
 MLM_MAX_PREDICTIONS = int(os.getenv("MLM_MAX_PREDICTIONS")) if os.getenv("MLM_MAX_PREDICTIONS") else None
 
+# OPTIM=sgd|adam|adamw|lamb and LR: the optimizer (LAMB with BERT's weight-decay exclusion of
+# biases and LayerNorm parameters, skycomputing_b200.parallel.optim); unset = SGD, lr 0.001
+OPTIM = os.getenv("OPTIM", "sgd").lower()
+LR = float(os.getenv("LR", "0.001"))
+_OPTIM_TYPES = dict(sgd="SGD", adam="Adam", adamw="AdamW", lamb="LAMB")
+if OPTIM not in _OPTIM_TYPES:
+    raise ValueError("OPTIM must be one of {}, got {!r}".format(sorted(_OPTIM_TYPES), OPTIM))
+
 _config = BertConfig.bert_large()                              # wwm_uncased_L-24_H-1024_A-16 geometry
 if TINY:
     _config = BertConfig(1000, hidden_size=64, num_hidden_layers=LAYER_NUM, num_attention_heads=4,
@@ -151,7 +159,7 @@ allocator_config = dict(
 )
 
 train_config = dict(
-    optim_cfg=dict(optim_type="SGD", lr=0.001),
+    optim_cfg=dict(optim_type=_OPTIM_TYPES[OPTIM], lr=LR),
     lr_schedule_cfg=(dict(type=LR_SCHEDULE, warmup_steps=WARMUP_STEPS, total_steps=TOTAL_STEPS)
                      if LR_SCHEDULE else None),
     grad_clip_cfg=dict(max_norm=MAX_GRAD_NORM) if MAX_GRAD_NORM is not None else None,

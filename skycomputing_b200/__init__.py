@@ -44,8 +44,8 @@ from .dataset import *  # noqa: F401,F403
 from .dynamics import *  # noqa: F401,F403
 from .logger import *  # noqa: F401,F403
 from .models import *  # noqa: F401,F403
-from .parallel import (BaseModule, FusedAdam, FusedSGD, LocalModule, PipelineEngine, RemoteModule,  # noqa: F401
-                       RpcModel, build_optimizer)
+from .parallel import (BaseModule, FusedAdam, FusedLamb, FusedSGD, Lamb, LocalModule,  # noqa: F401
+                       PipelineEngine, RemoteModule, RpcModel, build_optimizer)
 from .registry import *  # noqa: F401,F403
 from .runner import *  # noqa: F401,F403
 from .stimulator import Stimulator  # noqa: F401

@@ -39,7 +39,7 @@ _KERNELS_PER_CALL = {
     "attention_fwd": 1, "attention_bwd": 1, "embed_fwd": 1, "embed_bwd": 1,
     "small_linear_fwd": 1, "small_linear_bwd": 2, "softmax_ce": 1, "classify_eval": 1,
     "vocab_ce": -1, "mlm_gather": 1, "mlm_scatter": 1,
-    "sgd_multi": 1, "adam_multi": 1,
+    "sgd_multi": 1, "adam_multi": 1, "lamb_moments": 1, "lamb_update": 1,
     "grad_sumsq_multi": 1, "optim_finalize": 1,
     "cast_f32_to_bf16": 1, "cast_bf16_to_f32": 1, "advance_counter": 1, "advance_epoch": 1,
     "signal_flags": 1, "wait_flags": 1, "spin_ns": 1, "record_time": 1, "spin_factor": 1,

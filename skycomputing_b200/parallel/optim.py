@@ -11,12 +11,17 @@ moments, master, shadow and gradient zeroing in one pass, the step count lives i
 the update replays correctly inside the whole-step CUDA graph.
 
 ``build_optimizer`` keeps the reference's config contract (``optim_cfg = {optim_type: <any
-torch.optim class name>, **kwargs}``, experiment/launch.py:152-155): SGD / Adam / AdamW on the
-native path map to the fused classes, everything else (or options the fused kernels do not cover:
+torch.optim class name or "LAMB">, **kwargs}``, experiment/launch.py:152-155): SGD / Adam / AdamW /
+LAMB on the native path map to the fused classes, everything else (or options the fused kernels do not cover:
 nesterov, dampening, amsgrad, maximize) to the named ``torch.optim`` class over the fp32 masters
 (the bf16 shadows are then refreshed lazily by version counter; such a step is NOT graph-safe and
 the engines run it eagerly).  Optimizer state lives with the stage, as with the reference's
 DistributedOptimizer.
+
+``FusedLamb`` - LAMB (apex ``FusedLAMB`` semantics) in two launches per step over a per-parameter
+segment table inside the banks (``lamb_moments`` / ``lamb_update``): a trust ratio per
+``nn.Parameter``, weight decay off for names containing ``exclude_from_weight_decay``.  ``Lamb`` is
+its torch counterpart (``backend="torch"``, CPU, and parameters outside the banks).
 
 Learning-rate schedules and global-norm gradient clipping (``build_optimizer(..., lr_schedule=,
 grad_clip=)``, both opt-in).  The fused optimizers keep them on the device so that a captured step
@@ -384,6 +389,238 @@ class FusedAdam(FusedSGD):
                 v.copy_(s_)
 
 
+LAMB_DEFAULTS = dict(lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.01,
+                     exclude_from_weight_decay=("bias", "LayerNorm"))
+
+
+def check_lamb_cfg(cfg: dict) -> dict:
+    """LAMB options (``optim_cfg`` without ``optim_type``) completed with LAMB_DEFAULTS;
+    ValueError for unknown keys or values outside their range."""
+    cfg = dict(cfg)
+    unknown = sorted(set(cfg) - set(LAMB_DEFAULTS))
+    if unknown:
+        raise ValueError(f"unknown LAMB options {unknown}; allowed: {sorted(LAMB_DEFAULTS)}")
+    out = dict(LAMB_DEFAULTS, **cfg)
+    lr, eps, wd = float(out["lr"]), float(out["eps"]), float(out["weight_decay"])
+    try:
+        b1, b2 = (float(b) for b in out["betas"])
+    except (TypeError, ValueError):
+        raise ValueError(f"LAMB betas must be two numbers, got {out['betas']!r}") from None
+    if not (0.0 <= b1 < 1.0 and 0.0 <= b2 < 1.0):
+        raise ValueError(f"LAMB betas must lie in [0, 1), got {(b1, b2)}")
+    if not eps > 0.0:
+        raise ValueError(f"LAMB eps must be > 0, got {eps}")
+    if not wd >= 0.0:
+        raise ValueError(f"LAMB weight_decay must be >= 0, got {wd}")
+    if not lr >= 0.0:
+        raise ValueError(f"LAMB lr must be >= 0, got {lr}")
+    excl = out["exclude_from_weight_decay"]
+    if isinstance(excl, str) or not all(isinstance(s, str) and s for s in excl):
+        raise ValueError("LAMB exclude_from_weight_decay must be a sequence of non-empty "
+                         f"strings, got {excl!r}")
+    return dict(lr=lr, betas=(b1, b2), eps=eps, weight_decay=wd,
+                exclude_from_weight_decay=tuple(excl))
+
+
+def lamb_weight_decay(name: str, weight_decay: float, exclude) -> float:
+    """λ of the parameter called ``name``: 0 when the name contains one of ``exclude``."""
+    return 0.0 if any(s in name for s in exclude) else weight_decay
+
+
+def lamb_param_groups(module: nn.Module, weight_decay: float, exclude, params=None) -> list:
+    """Parameter groups of ``module`` (or of its ``params`` subset) by weight decay, named as in
+    ``module.named_parameters()``: the decayed ones first, then the excluded ones."""
+    keep = None if params is None else {id(p) for p in params}
+    groups = {}
+    for name, p in module.named_parameters():
+        if not p.requires_grad or (keep is not None and id(p) not in keep):
+            continue
+        wd = lamb_weight_decay(name, weight_decay, exclude)
+        g = groups.setdefault(wd, dict(params=[], names=[], weight_decay=wd))
+        g["params"].append(p)
+        g["names"].append(name)
+    return sorted(groups.values(), key=lambda g: -g["weight_decay"])
+
+
+class Lamb(torch.optim.Optimizer):
+    """LAMB (You et al. 2019) with apex ``FusedLAMB``'s defaults: decoupled weight decay inside
+    the update, bias correction, no NVLAMB.  Per tensor W with weight decay λ, at step t::
+
+        m = β1 m + (1-β1) g,   v = β2 v + (1-β2) g²
+        u = (m / (1-β1^t)) / (sqrt(v / (1-β2^t)) + eps) + λ W
+        r = ||W|| / ||u||  if λ != 0 and both norms > 0, else 1
+        W ← W - lr · r · u
+
+    The torch path of ``optim_type="LAMB"`` and the reference of the fused kernels.  No host
+    synchronisation: r stays a device tensor (``state[p]["trust_ratio"]``)."""
+
+    def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-6,
+                 weight_decay: float = 0.0):
+        chk = check_lamb_cfg(dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
+        chk.pop("exclude_from_weight_decay")
+        super().__init__(params, chk)
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            b1, b2 = group["betas"]
+            lr, eps, wd = group["lr"], group["eps"], group["weight_decay"]
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                st = self.state[p]
+                if not st:
+                    st["step"] = 0
+                    st["exp_avg"] = torch.zeros_like(p)
+                    st["exp_avg_sq"] = torch.zeros_like(p)
+                st["step"] += 1
+                t = st["step"]
+                g = p.grad
+                m, v = st["exp_avg"], st["exp_avg_sq"]
+                m.mul_(b1).add_(g, alpha=1.0 - b1)
+                v.mul_(b2).addcmul_(g, g, value=1.0 - b2)
+                u = (m / (1.0 - b1 ** t)) / ((v / (1.0 - b2 ** t)).sqrt() + eps)
+                if wd != 0.0:
+                    u.add_(p, alpha=wd)
+                    wn, un = torch.linalg.vector_norm(p), torch.linalg.vector_norm(u)
+                    r = torch.where((wn > 0) & (un > 0), wn / un, torch.ones_like(wn))
+                else:
+                    r = torch.ones((), dtype=p.dtype, device=p.device)
+                st["trust_ratio"] = r
+                p.sub_(u * (r * lr))
+        return loss
+
+
+class FusedLamb(FusedAdam):
+    """LAMB (see ``Lamb``) over the stage's flat parameter banks in two launches per step.
+
+    Every ``nn.Parameter`` inside a bank is one segment with its own λ and trust ratio (``wqkv``
+    holds three).  ``lamb_moments`` updates m and v and writes fp32 partials of ||W||² and ||u||²
+    per fixed-size chunk; ``lamb_update`` sums a segment's partials in fp64 in a fixed order, forms
+    r and applies the update with the bf16 shadow refresh.  No host sync, no per-step host-to-device
+    copy: graph-safe like ``FusedAdam``, whose moments, step counter, schedule / clipping path and
+    state_dict it shares.  Parameters outside the banks are stepped by ``Lamb``."""
+
+    def __init__(self, module: nn.Module, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-6,
+                 weight_decay: float = 0.01, exclude_from_weight_decay=("bias", "LayerNorm"),
+                 banks: Optional[list] = None):
+        chk = check_lamb_cfg(dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
+                                  exclude_from_weight_decay=exclude_from_weight_decay))
+        super().__init__(module, lr=chk["lr"], betas=chk["betas"], eps=chk["eps"],
+                         weight_decay=chk["weight_decay"], decoupled=True, banks=banks)
+        self.exclude = chk["exclude_from_weight_decay"]
+        self._names = {id(p): n for n, p in module.named_parameters()}
+        if self._rest_opt is not None:
+            rest = [p for g in self._rest_opt.param_groups for p in g["params"]]
+            self._rest_opt = Lamb(lamb_param_groups(module, self.weight_decay, self.exclude, rest),
+                                  lr=self.lr, betas=self.betas, eps=self.eps)
+        self.param_groups[0]["exclude_from_weight_decay"] = self.exclude
+        self._lamb = None          # (segments, chunk table, n_chunks) on the device, built once
+        self._seg_info: list = []
+
+    def segments(self) -> list:
+        """The segment table as dicts: name, bank (index into ``banks``), offset and numel in the
+        bank's flat buffer, weight_decay, use_ratio, skip_zero, aligned (float4 path)."""
+        if self._lamb is None:
+            return lamb_segments(self.banks, self._names, self.weight_decay, self.exclude)
+        return [dict(s) for s in self._seg_info]
+
+    def _lamb_table(self):
+        if self._lamb is None:
+            self._descriptors()          # decides overwrite_first (skip_zero) for every bank
+            ext = self._nat.ext()
+            info = lamb_segments(self.banks, self._names, self.weight_decay, self.exclude)
+            rows = []
+            for s in info:
+                b = self.banks[s["bank"]]
+                i, off = s["bank"], s["offset"]
+                shadow = b.shadow().data_ptr() + 2 * off if b.need_shadow else 0
+                rows.append((b.master().data_ptr() + 4 * off, b.grad().data_ptr() + 4 * off,
+                             self._mom[i].data_ptr() + 4 * off, self._mom2[i].data_ptr() + 4 * off,
+                             shadow, s["numel"], s["weight_decay"], int(s["use_ratio"]),
+                             int(s["skip_zero"])))
+            seg_raw, chunk_raw, n_chunks, vec = ext.pack_lamb_segments(rows)
+            for s, a in zip(info, vec):
+                s["aligned"] = bool(a)
+            dev = self._device
+            segs = torch.frombuffer(bytearray(seg_raw), dtype=torch.uint8).to(dev)
+            chunks = torch.frombuffer(bytearray(chunk_raw), dtype=torch.uint8).to(dev)
+            self._lamb_partials = torch.zeros(2 * max(1, n_chunks), dtype=torch.float32, device=dev)
+            self._ratios = torch.ones(max(1, len(info)), dtype=torch.float32, device=dev)
+            self._lamb = (segs, chunks, n_chunks)
+            self._seg_info = info
+        return self._lamb
+
+    def step(self, grad_scale: float = 1.0) -> None:
+        sc = 0
+        stream = torch.cuda.current_stream().cuda_stream if self.banks else 0
+        if self._scalars is not None:
+            stream = torch.cuda.current_stream().cuda_stream
+            self._compute_scalars(grad_scale, stream)
+            sc = self._scalars.data_ptr()
+            self._stepped = True
+        if self.banks:
+            segs, chunks, n_chunks = self._lamb_table()
+            ext = self._nat.ext()
+            ext.advance_counter(self._step.data_ptr(), 1, stream)
+            b1, b2 = self.betas
+            ext.lamb_moments(segs.data_ptr(), chunks.data_ptr(), n_chunks, b1, b2, float(self.eps),
+                             self._step.data_ptr(), float(grad_scale),
+                             self._lamb_partials.data_ptr(), stream, sc)
+            ext.lamb_update(segs.data_ptr(), chunks.data_ptr(), n_chunks,
+                            float(self.param_groups[0]["lr"]), b1, b2, float(self.eps),
+                            self._step.data_ptr(), self._lamb_partials.data_ptr(),
+                            self._ratios.data_ptr(), stream, sc)
+            for b in self.banks:
+                if b.overwrite_first:
+                    b.fresh = True
+            self._lamb_stepped = True
+        elif self._scalars is not None:
+            self._nat.ext().advance_counter(self._step.data_ptr(), 1, stream)
+        if self._rest_opt is not None:
+            self._rest_step()
+
+    _lamb_stepped = False
+
+    def trust_ratios(self) -> dict:
+        """{parameter name: r} of the last step (one device-to-host copy; {} before the first
+        step).  Parameters outside the banks report the ratio ``Lamb`` used for them."""
+        out = {}
+        if self._lamb_stepped:
+            out.update(zip((s["name"] for s in self._seg_info), self._ratios.tolist()))
+        if self._rest_opt is not None:
+            for g in self._rest_opt.param_groups:
+                for name, p in zip(g["names"], g["params"]):
+                    r = self._rest_opt.state.get(p, {}).get("trust_ratio")
+                    if r is not None:
+                        out[name] = float(r)
+        return out
+
+
+def lamb_segments(banks: list, names: dict, weight_decay: float, exclude) -> list:
+    """One segment per ``nn.Parameter`` of ``banks``, in bank order: dict(name, bank, offset,
+    numel, weight_decay, use_ratio, skip_zero, aligned).  ``names`` maps id(param) to its name in
+    the stage (``named_parameters()``); offsets are in elements of the bank's flat buffer and
+    ``aligned`` (float4 path) holds when the offset is a multiple of 4 elements."""
+    out = []
+    for i, b in enumerate(banks):
+        flat = b.master()
+        for p in b.params:
+            off = (p.data_ptr() - flat.data_ptr()) // flat.element_size()
+            name = names.get(id(p), f"<bank {i}>.{len(out)}")
+            wd = lamb_weight_decay(name, weight_decay, exclude)
+            if p.numel() == 0:
+                continue
+            out.append(dict(name=name, bank=i, offset=int(off), numel=p.numel(), weight_decay=wd,
+                            use_ratio=wd != 0.0, skip_zero=bool(b.overwrite_first),
+                            aligned=off % 4 == 0))
+    return out
+
+
 class TorchOptimizerAdapter:
     """Any ``torch.optim`` class over the stage's parameters; same step()/zero_grad() surface."""
 
@@ -500,6 +737,19 @@ def _build_optimizer(module: nn.Module, optim_cfg: dict, prefer_fused: bool):
     optim_type = cfg.pop("optim_type", "SGD")
     params = [p for p in module.parameters() if p.requires_grad]
     on_cuda = any(p.is_cuda for p in params)
+    if optim_type == "LAMB":
+        # no torch.optim class to fall back to: every option is checked here, on every backend
+        cfg = check_lamb_cfg(cfg)
+        if prefer_fused and on_cuda:
+            from ..models.bert_layers import get_backend
+            from ..ops import native as nat
+
+            if get_backend() != "torch" and nat.available():
+                return FusedLamb(module, **cfg)
+        if params:
+            excl = cfg.pop("exclude_from_weight_decay")
+            return TorchOptimizerAdapter(
+                Lamb(lamb_param_groups(module, cfg["weight_decay"], excl), **cfg))
     if optim_type in ("SGD", "Adam", "AdamW") and prefer_fused and on_cuda:
         from ..models.bert_layers import get_backend
         from ..ops import native as nat

@@ -34,6 +34,8 @@ def main():
     # every rank then reports its grad_norm per step, which must be the same on all of them
     ap.add_argument("--max-grad-norm", type=float, default=None)
     ap.add_argument("--lr-schedule", default=None, choices=["constant", "linear", "cosine"])
+    # the optimizer of every stage (lamb: per-tensor trust ratios, stage-local)
+    ap.add_argument("--optim", default="sgd", choices=["sgd", "adamw", "lamb"])
     a = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -79,7 +81,10 @@ def main():
         lr_schedule=(dict(type=a.lr_schedule, warmup_steps=2, total_steps=a.steps)
                      if a.lr_schedule else None),
         grad_clip=dict(max_norm=a.max_grad_norm) if a.max_grad_norm is not None else None)
-    opt = sky.build_optimizer(model.optim_module, dict(optim_type="SGD", lr=0.01), **step_cfg)
+    optim_cfg = dict(sgd=dict(optim_type="SGD", lr=0.01),
+                     adamw=dict(optim_type="AdamW", lr=1e-3, weight_decay=0.01),
+                     lamb=dict(optim_type="LAMB", lr=1e-3, weight_decay=0.01))[a.optim]
+    opt = sky.build_optimizer(model.optim_module, optim_cfg, **step_cfg)
     runner = sky.Runner(model=model, parameter_server=None, worker_manager=wm, optimizer=opt,
                         max_epochs=1, max_iters=10 ** 9, loss_cfg=dict(type="CrossEntropyLoss"),
                         timer_cfg=dict(root="/tmp/sky_check"), logging_cfg=None,
