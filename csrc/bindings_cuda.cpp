@@ -503,6 +503,15 @@ PYBIND11_MODULE(_cuda, m) {
   m.def("gemm_ln_tiles_per_panel", &sky::gemm_ln_tiles_per_panel, py::arg("M"), py::arg("N"),
         py::arg("force") = false);
   m.def("gemm_pick_block_n", &sky::gemm_pick_block_n);
+  m.def(
+      "gemm_ln_max_active_clusters",
+      [](int N, int block_n) {
+        int cluster = 0;
+        const int n = sky::gemm_ln_max_active_clusters(N, block_n, &cluster);
+        return py::make_tuple(n, cluster);
+      },
+      py::arg("N"), py::arg("block_n"),
+      "(clusters resident at once, CTAs per cluster) of the GEMM + LayerNorm kernel");
   m.def("gemm_tiles_per_panel", &sky::gemm_tiles_per_panel);
   m.def("layernorm_fwd", &layernorm_fwd, py::arg("z"), py::arg("y"), py::arg("mean"),
         py::arg("rstd"), py::arg("gamma"), py::arg("beta"), py::arg("M"), py::arg("H"),

@@ -48,8 +48,9 @@ struct GemmArgs {
   int* error_flag = nullptr;  // set to non-zero on flag-wait timeout
   // LayerNorm epilogue (ln_gamma != nullptr): out = LN(dropout(A B^T + bias) + aux) * gamma + beta,
   // out2 = the pre-LN sum (bf16, saved for backward), ln_mean / ln_rstd = row statistics.  The
-  // N / BLOCK_N CTAs of a 128-row panel form a thread-block cluster (row statistics through
-  // DSMEM); `out` may be peer memory, signal_flags[panel] then receives N / BLOCK_N signals.
+  // N / BLOCK_N CTAs of a 128-row panel (at N = 1024 and BLOCK_N = 256: the CTA pairs of its two
+  // 64-row halves) form thread-block clusters (row statistics through DSMEM); `out` may be peer
+  // memory, signal_flags[panel] then receives N / BLOCK_N signals.
   const float* ln_gamma = nullptr;
   const float* ln_beta = nullptr;
   float* ln_mean = nullptr;
@@ -73,6 +74,9 @@ int launch_gemm_ln(const GemmArgs& args, cudaStream_t stream);
 int gemm_ln_block_n(int M, int N, bool force = false);
 int gemm_ln_tiles_per_panel(int M, int N, bool force = false);
 int gemm_tiles_per_panel(int N, int block_n);  // number of signals per 128-row panel
+// clusters of the GEMM + LayerNorm kernel for width N and tile width block_n that the device can
+// hold at once (cudaOccupancyMaxActiveClusters); *cluster = CTAs per cluster; < 0 on error
+int gemm_ln_max_active_clusters(int N, int block_n, int* cluster);
 int gemm_pick_block_n(int M, int N);
 
 // ---------------------------------------------------------------------------------------------

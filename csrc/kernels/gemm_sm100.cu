@@ -241,12 +241,12 @@ struct Operands {
 
 // Prologue of both kernels, before their cluster / CTA sync: warp 0 prefetches the tensor maps,
 // lane 0 of warp 1 initialises the ring barriers.  A stage is free again after `empty_count`
-// arrivals: one per consumer warpgroup of every CTA that loads into it.
-template <int BLOCK_N>
+// arrivals: one per consumer warpgroup of every CTA that loads into it.  C = the ring's layout
+// (kStages, kABytes, kOffBars).
+template <int BLOCK_N, class C = Cfg<BLOCK_N>>
 __device__ __forceinline__ Operands ring_prologue(uint8_t* smem_raw, const CUtensorMap* tmap_a,
                                                   const CUtensorMap* tmap_b, int warp_idx,
                                                   int lane, uint32_t empty_count) {
-  using C = Cfg<BLOCK_N>;
   Operands op;
   op.base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                        ~static_cast<uintptr_t>(1023));
@@ -361,12 +361,12 @@ __device__ __forceinline__ void release_stage(uint64_t* empty_bar) {
 
 // Main loop of one consumer warpgroup over k-blocks [kb0, kb1): acc (+)= A[64 rows] * B^T.
 // One wgmma group stays in flight; a stage is released once the group that read it has retired.
-template <int BLOCK_N, bool A_MN, bool B_MN, int CL, int kStages>
+// C = the ring's layout (stage strides kABytes, kBBytes).
+template <int BLOCK_N, bool A_MN, bool B_MN, int CL, int kStages, class C = Cfg<BLOCK_N>>
 __device__ __forceinline__ void consumer_mainloop(float (&acc)[BLOCK_N / 2], int kb0, int kb1,
                                                   uint32_t a_base, uint32_t b_base,
                                                   const Operands& op, Ring<kStages>& ring,
                                                   bool elected, bool skip_mma) {
-  using C = Cfg<BLOCK_N>;
   // K-major  SW128: 8-row atoms 1024B apart (SBO), LBO unused (1); K advance = 32B per MMA_K
   // MN-major SW128: 64-element MN chunks BLOCK_K*128B apart (LBO), 8-k-row groups 1024B apart
   //                 (SBO); K advance = 16 rows * 128B = 2048B per MMA_K
@@ -679,19 +679,32 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
 //
 //     y = LayerNorm( dropout(A W^T + bias) + residual ) * gamma + beta        z = the pre-LN sum
 //
-// A LayerNorm row spans all N columns, a CTA's accumulator only BLOCK_N of them, so the N / BLOCK_N
-// CTAs that own the column tiles of one 128-row panel form a THREAD-BLOCK CLUSTER (2..8 CTAs) and
-// exchange per-row partial sums through distributed shared memory.  The prologue, the producer,
-// the main loop and the epilogue steps of pass 1 are those of gemm_wgmma_kernel:
+// A LayerNorm row spans all N columns, a warpgroup's accumulator only 256 (or 128) of them, so the
+// CTAs that own the columns of one row panel form a THREAD-BLOCK CLUSTER and exchange per-row
+// partial sums through distributed shared memory.  Two layouts (L below) share one body:
+//
+//   wide  (LnCfg<BLOCK_N>)  128-row panels; the N / BLOCK_N CTAs of a panel form a 2..8-CTA cluster,
+//                           each CTA owns 128 x BLOCK_N (warpgroup: 64 rows x BLOCK_N)
+//   pair  (LnPairCfg)       N = 1024 only: 64-row panels, one CTA pair per panel, each CTA owns
+//                           64 x 512 (warpgroup: the same 64 rows x 256 columns).  A 4-CTA
+//                           cluster needs four free SMs in one GPC: an H100 SXM (132 SMs) holds
+//                           30 such clusters of this kernel at once, so the 32 clusters of a
+//                           4096-token wide launch ran in two waves; it holds 66 pairs, and the
+//                           64 pairs of that launch run in one.
+//
+// The prologue, the producer (wide), the main loop and the epilogue steps of pass 1 are those of
+// gemm_wgmma_kernel:
 //
 //   pass 1  on the accumulator fragments: + bias, dropout, + residual; store z (bf16, saved for
 //           backward); accumulate row sum / sum of squares (the quad that holds a row combines
 //           them with two shuffles); the fp32 sums stay in the accumulator registers
-//   DSMEM   one thread per row stores the row's (sum, sumsq) into ALL CTAs of the cluster
-//           (st.shared::cluster) and arrives on their mbarriers (release.cluster)
+//   DSMEM   one thread per row and warpgroup stores the row's (sum, sumsq) into ALL CTAs of the
+//           cluster (st.shared::cluster) and arrives on their mbarriers (release.cluster); each
+//           CTA adds the partials in column order, so both layouts give the same statistics
 //   pass 2  on the fragments again: normalise with the cluster-wide statistics,
 //           gamma / beta, store y - straight into the NEXT PIPELINE STAGE's HBM when y is a peer
-//           pointer, then one red.release.sys per CTA on the panel flag.
+//           pointer, then one red.release.sys per CTA on the 128-row panel's flag (N / 256 per
+//           panel at N = 1024 in both layouts).
 //
 // This is the forward stage boundary of the north star: the last GEMM of stage i stores its
 // output tiles into stage i+1's HBM from inside the GEMM kernel; no separate LayerNorm launch.
@@ -707,13 +720,17 @@ struct GemmLnDev : GemmCommon {
   float* mean;
   float* rstd;
   float eps;
+  int debug;  // 1 = main loop only: the epilogue discards the tile (see GemmArgs::debug)
 };
 
 constexpr int kLnMaxCluster = 8;
 
 template <int BLOCK_N>
 struct LnCfg {
-  using C = Cfg<BLOCK_N>;
+  using C = Cfg<BLOCK_N>;  // the operand ring
+  static constexpr bool kPair = false;
+  static constexpr int kRows = BLOCK_M;  // rows of a panel (= of a CTA tile)
+  static constexpr int kCols = BLOCK_N;  // columns of a CTA tile
   static constexpr int kVecBytes = 3 * BLOCK_N * 4;                 // bias, gamma, beta
   static constexpr int kStatsBytes = kLnMaxCluster * BLOCK_M * 8;   // float2 per (cta, row)
   static constexpr int kOffVec = C::kOffBars + 256;
@@ -723,29 +740,80 @@ struct LnCfg {
   static_assert(kSmemBytes <= kMaxSmemBytes, "GEMM + LayerNorm shared memory over the per-block limit");
 };
 
-template <int BLOCK_N>
-__global__ void __launch_bounds__(kNumThreads, 1)
-gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                     const __grid_constant__ CUtensorMap tmap_b, const GemmLnDev p) {
-  using L = LnCfg<BLOCK_N>;
-  constexpr int kStages = L::C::kStages;
-  const uint32_t cln = cluster_nctarank();     // CTAs per cluster == column tiles per row panel
-  const uint32_t n_blk = cluster_ctarank();    // this CTA's column tile
-  const int m_blk = static_cast<int>(blockIdx.x / cln);
+// The pair layout: its own operand ring (64 A rows, 512 B rows per stage) and, since a stage is
+// 72 KB, only three stages; the epilogue's staging buffers reuse the ring once the main loop is
+// done.  The statistics stay outside the ring: the peer writes them while we may still compute.
+struct LnPairCfg {
+  using C = LnPairCfg;
+  static constexpr bool kPair = true;
+  static constexpr int kRows = 64;
+  static constexpr int kCols = 512;
+  static constexpr int kStages = 3;
+  static constexpr int kABytes = kRows * BLOCK_K * 2;
+  static constexpr int kBBytes = kCols * BLOCK_K * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kOffBars = kStages * kStageBytes;
+  static constexpr int kVecBytes = 3 * kCols * 4;   // bias, gamma, beta
+  static constexpr int kStatsBytes = 4 * kRows * 8;  // float2 per (warpgroup of the pair, row)
+  static constexpr int kOffVec = kOffBars + 256;
+  static constexpr int kOffOut = 0;
+  static constexpr int kOffStats = kOffVec + kVecBytes;
+  static constexpr int kSmemBytes = kOffStats + kStatsBytes + 1024 /*align slack*/;
+  static_assert(kSmemBytes <= kMaxSmemBytes, "GEMM + LayerNorm shared memory over the per-block limit");
+  static_assert(8 * kWarpStageBytes <= kOffBars, "epilogue staging does not fit the operand ring");
+};
+
+// Producer of the pair layout: k-block kb of the CTA's tile into ring stage `stage`, whose empty
+// barrier the caller has waited on.  A: the panel's 64 rows from a_row0; B: the CTA's 512 rows as
+// two boxes.  A is not multicast inside the pair: with three stages, a stage that both CTAs must
+// release before either can refill it stalled the main loop (measured on H100: 1.9x the plain
+// GEMM's time at K = 4096, against 1.07x without multicast).
+__device__ __forceinline__ void load_k_block_ln_pair(const Operands& op, int stage,
+                                                     const CUtensorMap* tmap_a,
+                                                     const CUtensorMap* tmap_b, int kb, int a_row0,
+                                                     uint32_t cta) {
+  using C = LnPairCfg;
+  if (elect_one_sync()) {
+    uint64_t* full = &op.full_bar[stage];
+    mbar_expect_tx(full, C::kStageBytes);
+    uint8_t* sa = op.a + stage * C::kABytes;
+    uint8_t* sb = op.b + stage * C::kBBytes;
+    tma_load_2d(sa, tmap_a, full, kb * BLOCK_K, a_row0);
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      tma_load_2d(sb + h * (C::kBBytes / 2), tmap_b, full, kb * BLOCK_K,
+                  static_cast<int>(cta) * C::kCols + h * (C::kCols / 2));
+  }
+  __syncwarp();
+}
+
+template <int BLOCK_N, class L>
+__device__ __forceinline__ void gemm_ln_body(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b,
+                                             const GemmLnDev& p) {
+  using C = typename L::C;
+  constexpr int kStages = C::kStages;
+  constexpr bool kPair = L::kPair;
+  const uint32_t cln = cluster_nctarank();  // CTAs per cluster (wide: column tiles per panel)
+  const uint32_t cta = cluster_ctarank();   // this CTA's column tile
+  const int m_blk = static_cast<int>(blockIdx.x / cln);  // panel of L::kRows rows
+  const int panel128 = kPair ? m_blk / 2 : m_blk;         // the flags count 128-row panels
+  // contributors of row statistics: wide: one per CTA, pair: one per warpgroup
+  const uint32_t ncontrib = kPair ? 2 * cln : cln;
 
   extern __shared__ uint8_t smem_raw[];
   const int warp_idx = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
   const int num_k_blks = (p.K + BLOCK_K - 1) / BLOCK_K;
 
-  const Operands op = ring_prologue<BLOCK_N>(smem_raw, &tmap_a, &tmap_b, warp_idx, lane, 2);
+  const Operands op =
+      ring_prologue<BLOCK_N, C>(smem_raw, tmap_a, tmap_b, warp_idx, lane, 2);
   uint64_t* stats_bar = op.empty_bar + kStages;
   float* s_bias = reinterpret_cast<float*>(op.base + L::kOffVec);
-  float* s_gamma = s_bias + BLOCK_N;
-  float* s_beta = s_gamma + BLOCK_N;
-  float2* s_stats = reinterpret_cast<float2*>(op.base + L::kOffStats);   // [cln][128]
+  float* s_gamma = s_bias + L::kCols;
+  float* s_beta = s_gamma + L::kCols;
+  float2* s_stats = reinterpret_cast<float2*>(op.base + L::kOffStats);   // [ncontrib][kRows]
   if (warp_idx == 1 && lane == 0) {
-    mbar_init(stats_bar, cln * BLOCK_M);   // one arrival per row-owner thread of every CTA
+    mbar_init(stats_bar, ncontrib * L::kRows);   // one arrival per row-owner thread of every CTA
     fence_barrier_init();
   }
   __syncwarp();
@@ -758,23 +826,31 @@ gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
     if (warp_idx == 0) {
       // ===================================== TMA producer =====================================
       Ring<kStages> ring;
-      if (p.wait_flags != nullptr) wait_inbound_panel(p, m_blk);
+      if (p.wait_flags != nullptr) wait_inbound_panel(p, panel128);
       for (int kb = 0; kb < num_k_blks; ++kb, ring.advance()) {
         mbar_wait(&op.empty_bar[ring.stage], ring.phase ^ 1);
-        load_k_block<BLOCK_N, false, false, 1>(op, ring.stage, &tmap_a, &tmap_b, kb,
-                                               m_blk * BLOCK_M, static_cast<int>(n_blk) * BLOCK_N,
-                                               0u, false);
+        if constexpr (kPair) {
+          load_k_block_ln_pair(op, ring.stage, tmap_a, tmap_b, kb, m_blk * L::kRows, cta);
+        } else {
+          load_k_block<BLOCK_N, false, false, 1>(op, ring.stage, tmap_a, tmap_b, kb,
+                                                 m_blk * BLOCK_M, static_cast<int>(cta) * BLOCK_N,
+                                                 0u, false);
+        }
       }
     }
   } else {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     // ============================ consumers: wgmma main loop + epilogue ============================
     const Consumer c = consumer_of(warp_idx, lane, op.base + L::kOffOut, p);
-    const long long warp_row0 = static_cast<long long>(m_blk) * BLOCK_M + c.warp_row;
+    // the warp's first row inside the CTA tile, the warpgroup's first column inside it
+    const int warp_row = kPair ? c.warp_row - 64 * c.wg : c.warp_row;
+    const int wg_col = kPair ? c.wg * BLOCK_N : 0;
+    const int tile_col0 = static_cast<int>(cta) * L::kCols;
+    const long long warp_row0 = static_cast<long long>(m_blk) * L::kRows + warp_row;
     const long long row_a = warp_row0 + c.fr;  // and row_a + 8
     const bool has_aux = p.aux != nullptr;
-    for (int i = c.epi_tid; i < BLOCK_N; i += 256) {
-      const int gc = static_cast<int>(n_blk) * BLOCK_N + i;
+    for (int i = c.epi_tid; i < L::kCols; i += 256) {
+      const int gc = tile_col0 + i;
       s_bias[i] = p.bias != nullptr ? __ldg(p.bias + gc) : 0.f;
       s_gamma[i] = __ldg(p.gamma + gc);
       s_beta[i] = __ldg(p.beta + gc);
@@ -783,109 +859,129 @@ gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
     float acc[BLOCK_N / 2];
     {
       Ring<kStages> ring;
-      consumer_mainloop<BLOCK_N, false, false, 1>(acc, 0, num_k_blks, smem_u32(op.a) + c.wg * 8192,
-                                                  smem_u32(op.b), op, ring, c.elected, false);
+      const uint32_t a_base = smem_u32(op.a) + (kPair ? 0 : c.wg * 8192);
+      const uint32_t b_base = smem_u32(op.b) + (kPair ? c.wg * (C::kBBytes / 2) : 0);
+      consumer_mainloop<BLOCK_N, false, false, 1, kStages, C>(
+          acc, 0, num_k_blks, a_base, b_base, op, ring, c.elected, false);
     }
-    asm volatile("bar.sync 1, 256;" ::: "memory");   // bias / gamma / beta staged
+    // bias / gamma / beta staged; (pair) no warpgroup reads the ring any more
+    asm volatile("bar.sync 1, 256;" ::: "memory");
 
-    // ---------------- pass 1: z = dropout(acc + bias) + residual; row statistics ----------------
-    // the fp32 sums stay in the accumulator registers for pass 2
-    float s1a = 0.f, s2a = 0.f, s1b = 0.f, s2b = 0.f;   // rows fr / fr + 8
+    if (p.debug != 1) {
+      // -------------- pass 1: z = dropout(acc + bias) + residual; row statistics --------------
+      // the fp32 sums stay in the accumulator registers for pass 2
+      float s1a = 0.f, s2a = 0.f, s1b = 0.f, s2b = 0.f;   // rows fr / fr + 8
 #pragma unroll
-    for (int g = 0; g < BLOCK_N / 64; ++g) {
-      const int ct = g * 64;
-      const int col0 = static_cast<int>(n_blk) * BLOCK_N + ct;
-      uint4 ax[4];
-      if (has_aux) aux_load(ax, p.aux, p.ldaux, warp_row0, p.M, col0, p.N, lane);
-      float f[32];
+      for (int g = 0; g < BLOCK_N / 64; ++g) {
+        const int ct = wg_col + g * 64;  // first column of the group inside the CTA tile
+        const int col0 = tile_col0 + ct;
+        uint4 ax[4];
+        if (has_aux) aux_load(ax, p.aux, p.ldaux, warp_row0, p.M, col0, p.N, lane);
+        float f[32];
 #pragma unroll
-      for (int i = 0; i < 32; ++i) f[i] = acc[g * 32 + i];
-      frag_add_bias(f, s_bias, ct, c.fc);
-      if (c.dr.on) frag_dropout(f, c.dr.seed, c.dr.thr16, c.dr.scale, row_a, col0, p.N, lane);
-      if (has_aux) frag_apply_aux(f, ax, c.stage, lane, false, true);
+        for (int i = 0; i < 32; ++i) f[i] = acc[g * 32 + i];
+        frag_add_bias(f, s_bias, ct, c.fc);
+        if (c.dr.on) frag_dropout(f, c.dr.seed, c.dr.thr16, c.dr.scale, row_a, col0, p.N, lane);
+        if (has_aux) frag_apply_aux(f, ax, c.stage, lane, false, true);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        s1a += f[4 * j] + f[4 * j + 1];
-        s2a = fmaf(f[4 * j], f[4 * j], fmaf(f[4 * j + 1], f[4 * j + 1], s2a));
-        s1b += f[4 * j + 2] + f[4 * j + 3];
-        s2b = fmaf(f[4 * j + 2], f[4 * j + 2], fmaf(f[4 * j + 3], f[4 * j + 3], s2b));
+        for (int j = 0; j < 8; ++j) {
+          s1a += f[4 * j] + f[4 * j + 1];
+          s2a = fmaf(f[4 * j], f[4 * j], fmaf(f[4 * j + 1], f[4 * j + 1], s2a));
+          s1b += f[4 * j + 2] + f[4 * j + 3];
+          s2b = fmaf(f[4 * j + 2], f[4 * j + 2], fmaf(f[4 * j + 3], f[4 * j + 3], s2b));
+        }
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[g * 32 + i] = f[i];
+        if (p.z != nullptr)
+          frag_store_bf16(f, c.stage, lane, reinterpret_cast<__nv_bfloat16*>(p.z), p.ldz,
+                          warp_row0, p.M, col0, p.N);
       }
+      // -------------- cluster-wide row statistics through distributed shared memory --------------
+      // a row of the warpgroup's BLOCK_N columns lives in one quad: two shuffles give its sums,
+      // then lane 0 (row fr) and lane 1 (row fr + 8) of the quad publish them to every CTA of
+      // the cluster, in the slot of the warpgroup's column range
 #pragma unroll
-      for (int i = 0; i < 32; ++i) acc[g * 32 + i] = f[i];
-      if (p.z != nullptr)
-        frag_store_bf16(f, c.stage, lane, reinterpret_cast<__nv_bfloat16*>(p.z), p.ldz, warp_row0,
+      for (int o = 1; o <= 2; o <<= 1) {
+        s1a += __shfl_xor_sync(0xffffffffu, s1a, o);
+        s2a += __shfl_xor_sync(0xffffffffu, s2a, o);
+        s1b += __shfl_xor_sync(0xffffffffu, s1b, o);
+        s2b += __shfl_xor_sync(0xffffffffu, s2b, o);
+      }
+      const int contrib = kPair ? static_cast<int>(2 * cta) + c.wg : static_cast<int>(cta);
+      const int row_a_in_tile = warp_row + c.fr;
+      if ((lane & 3) < 2) {
+        const int hb = lane & 1;
+        const uint32_t slot = smem_u32(&s_stats[contrib * L::kRows + row_a_in_tile + 8 * hb]);
+        const uint32_t bar = smem_u32(stats_bar);
+        const float v1 = hb ? s1b : s1a;
+        const float v2 = hb ? s2b : s2a;
+        for (uint32_t r = 0; r < cln; ++r) {
+          st_cluster_v2_f32(mapa_shared(slot, r), v1, v2);
+          mbar_arrive_cluster(mapa_shared(bar, r));
+        }
+      }
+      mbar_wait_cluster(stats_bar, 0);
+      float t1a = 0.f, t2a = 0.f, t1b = 0.f, t2b = 0.f;
+      for (uint32_t r = 0; r < ncontrib; ++r) {
+        const float2 oa = s_stats[r * L::kRows + row_a_in_tile];
+        const float2 ob = s_stats[r * L::kRows + row_a_in_tile + 8];
+        t1a += oa.x;
+        t2a += oa.y;
+        t1b += ob.x;
+        t2b += ob.y;
+      }
+      const float inv_n = 1.f / static_cast<float>(p.N);
+      const float mean_a = t1a * inv_n;
+      const float rstd_a = rsqrtf(fmaxf(fmaf(-mean_a, mean_a, t2a * inv_n), 0.f) + p.eps);
+      const float mean_b = t1b * inv_n;
+      const float rstd_b = rsqrtf(fmaxf(fmaf(-mean_b, mean_b, t2b * inv_n), 0.f) + p.eps);
+      if (contrib == 0 && (lane & 3) < 2) {
+        const int hb = lane & 1;
+        const long long row = row_a + 8 * hb;
+        if (row < p.M) {
+          p.mean[row] = hb ? mean_b : mean_a;
+          p.rstd[row] = hb ? rstd_b : rstd_a;
+        }
+      }
+      // ------------ pass 2: normalise, gamma / beta, store y (possibly into a peer GPU) ------------
+#pragma unroll
+      for (int g = 0; g < BLOCK_N / 64; ++g) {
+        const int ct = wg_col + g * 64;
+        const int col0 = tile_col0 + ct;
+        float f[32];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float2 gm = *reinterpret_cast<const float2*>(s_gamma + ct + j * 8 + c.fc);
+          const float2 bt = *reinterpret_cast<const float2*>(s_beta + ct + j * 8 + c.fc);
+          f[4 * j] = fmaf((acc[g * 32 + 4 * j] - mean_a) * rstd_a, gm.x, bt.x);
+          f[4 * j + 1] = fmaf((acc[g * 32 + 4 * j + 1] - mean_a) * rstd_a, gm.y, bt.y);
+          f[4 * j + 2] = fmaf((acc[g * 32 + 4 * j + 2] - mean_b) * rstd_b, gm.x, bt.x);
+          f[4 * j + 3] = fmaf((acc[g * 32 + 4 * j + 3] - mean_b) * rstd_b, gm.y, bt.y);
+        }
+        frag_store_bf16(f, c.stage, lane, reinterpret_cast<__nv_bfloat16*>(p.y), p.ldy, warp_row0,
                         p.M, col0, p.N);
-    }
-    // ---------------- cluster-wide row statistics through distributed shared memory ----------------
-    // a row of this CTA's BLOCK_N columns lives in one quad: two shuffles give its sums, then lane
-    // 0 (row fr) and lane 1 (row fr + 8) of the quad publish them to every CTA of the cluster
-#pragma unroll
-    for (int o = 1; o <= 2; o <<= 1) {
-      s1a += __shfl_xor_sync(0xffffffffu, s1a, o);
-      s2a += __shfl_xor_sync(0xffffffffu, s2a, o);
-      s1b += __shfl_xor_sync(0xffffffffu, s1b, o);
-      s2b += __shfl_xor_sync(0xffffffffu, s2b, o);
-    }
-    const int row_a_in_tile = c.warp_row + c.fr;
-    if ((lane & 3) < 2) {
-      const int hb = lane & 1;
-      const uint32_t slot = smem_u32(&s_stats[n_blk * BLOCK_M + row_a_in_tile + 8 * hb]);
-      const uint32_t bar = smem_u32(stats_bar);
-      const float v1 = hb ? s1b : s1a;
-      const float v2 = hb ? s2b : s2a;
-      for (uint32_t r = 0; r < cln; ++r) {
-        st_cluster_v2_f32(mapa_shared(slot, r), v1, v2);
-        mbar_arrive_cluster(mapa_shared(bar, r));
       }
+      // publish this CTA's tile of the 128-row panel; the consumer waits for epoch x
+      // (N / BLOCK_N) signals per panel
+      if (p.signal_flags != nullptr) publish_panel(p.signal_flags, panel128, c.epi_tid);
     }
-    mbar_wait_cluster(stats_bar, 0);
-    float t1a = 0.f, t2a = 0.f, t1b = 0.f, t2b = 0.f;
-    for (uint32_t r = 0; r < cln; ++r) {
-      const float2 oa = s_stats[r * BLOCK_M + row_a_in_tile];
-      const float2 ob = s_stats[r * BLOCK_M + row_a_in_tile + 8];
-      t1a += oa.x;
-      t2a += oa.y;
-      t1b += ob.x;
-      t2b += ob.y;
-    }
-    const float inv_n = 1.f / static_cast<float>(p.N);
-    const float mean_a = t1a * inv_n;
-    const float rstd_a = rsqrtf(fmaxf(fmaf(-mean_a, mean_a, t2a * inv_n), 0.f) + p.eps);
-    const float mean_b = t1b * inv_n;
-    const float rstd_b = rsqrtf(fmaxf(fmaf(-mean_b, mean_b, t2b * inv_n), 0.f) + p.eps);
-    if (n_blk == 0 && (lane & 3) < 2) {
-      const int hb = lane & 1;
-      const long long row = row_a + 8 * hb;
-      if (row < p.M) {
-        p.mean[row] = hb ? mean_b : mean_a;
-        p.rstd[row] = hb ? rstd_b : rstd_a;
-      }
-    }
-    // ---------------- pass 2: normalise, gamma / beta, store y (possibly into a peer GPU) ----------------
-#pragma unroll
-    for (int g = 0; g < BLOCK_N / 64; ++g) {
-      const int ct = g * 64;
-      const int col0 = static_cast<int>(n_blk) * BLOCK_N + ct;
-      float f[32];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float2 gm = *reinterpret_cast<const float2*>(s_gamma + ct + j * 8 + c.fc);
-        const float2 bt = *reinterpret_cast<const float2*>(s_beta + ct + j * 8 + c.fc);
-        f[4 * j] = fmaf((acc[g * 32 + 4 * j] - mean_a) * rstd_a, gm.x, bt.x);
-        f[4 * j + 1] = fmaf((acc[g * 32 + 4 * j + 1] - mean_a) * rstd_a, gm.y, bt.y);
-        f[4 * j + 2] = fmaf((acc[g * 32 + 4 * j + 2] - mean_b) * rstd_b, gm.x, bt.x);
-        f[4 * j + 3] = fmaf((acc[g * 32 + 4 * j + 3] - mean_b) * rstd_b, gm.y, bt.y);
-      }
-      frag_store_bf16(f, c.stage, lane, reinterpret_cast<__nv_bfloat16*>(p.y), p.ldy, warp_row0,
-                      p.M, col0, p.N);
-    }
-    // publish this CTA's 128 x BLOCK_N tile of the panel; the consumer waits for epoch x
-    // (N / BLOCK_N) signals per panel
-    if (p.signal_flags != nullptr) publish_panel(p.signal_flags, m_blk, c.epi_tid);
   }
 
   __syncwarp();
   cluster_sync_all();   // nobody leaves while a peer may still write its statistics into us
+}
+
+template <int BLOCK_N>
+__global__ void __launch_bounds__(kNumThreads, 1)
+gemm_ln_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                     const __grid_constant__ CUtensorMap tmap_b, const GemmLnDev p) {
+  gemm_ln_body<BLOCK_N, LnCfg<BLOCK_N>>(&tmap_a, &tmap_b, p);
+}
+
+__global__ void __launch_bounds__(kNumThreads, 1)
+gemm_ln_pair_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                    const __grid_constant__ CUtensorMap tmap_b, const GemmLnDev p) {
+  gemm_ln_body<256, LnPairCfg>(&tmap_a, &tmap_b, p);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1189,6 +1285,22 @@ int launch_ln_inst(const GemmArgs& a, const GemmLnDev& d, cudaStream_t stream) {
   return launch<gemm_ln_wgmma_kernel<BLOCK_N>>(panels * cln, cln, LnCfg<BLOCK_N>::kSmemBytes,
                                                stream, tma, tmb, d);
 }
+
+// the pair layout runs N = 1024 with 256-wide warpgroup tiles
+bool ln_pair_layout(int N, int block_n) { return block_n == 256 && N == 2 * LnPairCfg::kCols; }
+
+int launch_ln_pair(const GemmArgs& a, const GemmLnDev& d, cudaStream_t stream) {
+  using L = LnPairCfg;
+  CUtensorMap tma, tmb;
+  int rc = make_tmap_bf16_2d(&tma, a.A, a.K, a.M, a.lda, BLOCK_K, L::kRows);
+  if (rc) return rc;
+  rc = make_tmap_bf16_2d(&tmb, a.B, a.K, a.N, a.ldb, BLOCK_K, L::kCols / 2);
+  if (rc) return rc;
+  // whole 128-row panels, so that every panel's flag receives its 4 signals even when M is ragged
+  // (the rows of a pair past M are loaded as zeros and never stored)
+  const int pairs = 2 * ((a.M + BLOCK_M - 1) / BLOCK_M);
+  return launch<gemm_ln_pair_kernel>(2 * pairs, 2, L::kSmemBytes, stream, tma, tmb, d);
+}
 }  // namespace
 
 int launch_gemm_ln(const GemmArgs& a, cudaStream_t stream) {
@@ -1212,9 +1324,49 @@ int launch_gemm_ln(const GemmArgs& a, cudaStream_t stream) {
   d.mean = a.ln_mean;
   d.rstd = a.ln_rstd;
   d.eps = a.ln_eps;
+  d.debug = a.debug;
+  if (ln_pair_layout(a.N, bn)) return launch_ln_pair(a, d, stream);
   if (bn == 256) return launch_ln_inst<256>(a, d, stream);
   if (bn == 128) return launch_ln_inst<128>(a, d, stream);
   return 905;
+}
+
+namespace {
+// clusters of `cluster` CTAs of `kern` with `smem` bytes of dynamic shared memory each that the
+// device can hold at once; < 0: minus the CUDA error
+template <class Kern>
+int max_active_clusters(Kern kern, int smem, int cluster) {
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e != cudaSuccess) return -static_cast<int>(e);
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(cluster * 64);
+  cfg.blockDim = dim3(kNumThreads);
+  cfg.dynamicSmemBytes = smem;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = static_cast<unsigned>(cluster);
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  int n = 0;
+  e = cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
+  return e == cudaSuccess ? n : -static_cast<int>(e);
+}
+}  // namespace
+
+int gemm_ln_max_active_clusters(int N, int block_n, int* cluster) {
+  *cluster = 0;
+  if ((block_n != 128 && block_n != 256) || N % block_n != 0 || N / block_n > kLnMaxCluster)
+    return -907;
+  if (ln_pair_layout(N, block_n)) {
+    *cluster = 2;
+    return max_active_clusters(gemm_ln_pair_kernel, LnPairCfg::kSmemBytes, 2);
+  }
+  *cluster = N / block_n;
+  if (block_n == 256)
+    return max_active_clusters(gemm_ln_wgmma_kernel<256>, LnCfg<256>::kSmemBytes, *cluster);
+  return max_active_clusters(gemm_ln_wgmma_kernel<128>, LnCfg<128>::kSmemBytes, *cluster);
 }
 
 int launch_gemm(const GemmArgs& a, cudaStream_t stream) {

@@ -239,13 +239,15 @@ def gemm_ln(a: torch.Tensor, b: torch.Tensor, gamma: torch.Tensor, beta: torch.T
             residual: Optional[torch.Tensor] = None, dropout_p: float = 0.0,
             rng: Optional[RngState] = None, rng_stream: int = 0, save_z: bool = True,
             y_ptr: int = 0, y_ld: int = 0, signal_flags: int = 0, wait_flags: int = 0,
-            wait_epoch: int = 0, wait_mult: int = 0, error_flag: int = 0, block_n: int = 0):
+            wait_epoch: int = 0, wait_mult: int = 0, error_flag: int = 0, block_n: int = 0,
+            debug: int = 0):
     """y = LayerNorm(dropout(a b^T + bias) + residual) * gamma + beta in ONE wgmma kernel
     (cluster-wide row statistics through DSMEM, see csrc/kernels/gemm_sm100.cu).
 
     Returns ``(y, z, mean, rstd)``: ``z`` is the bf16 pre-LayerNorm sum saved for backward (None
     when ``save_z`` is False), ``y`` is None when ``y_ptr`` redirects the store to raw (peer)
-    memory; ``signal_flags`` then receives ``gemm_ln_tiles_per_panel`` signals per 128-row panel."""
+    memory; ``signal_flags`` then receives ``gemm_ln_tiles_per_panel`` signals per 128-row panel.
+    ``debug=1`` (timing only) runs the main loop and skips the epilogue: nothing is written."""
     _check(a, torch.bfloat16, "a")
     _check(b, torch.bfloat16, "b")
     _check(gamma, torch.float32, "gamma")
@@ -275,7 +277,7 @@ def gemm_ln(a: torch.Tensor, b: torch.Tensor, gamma: torch.Tensor, beta: torch.T
         add_aux=residual is not None, dropout_p=float(dropout_p),
         rng_state=0 if rng is None else rng.ptr, rng_stream=rng_stream,
         signal_flags=signal_flags, wait_flags=wait_flags, wait_epoch=wait_epoch,
-        wait_mult=wait_mult, error_flag=error_flag, block_n=block_n,
+        wait_mult=wait_mult, error_flag=error_flag, block_n=block_n, debug=debug,
         ln_gamma=gamma.data_ptr(), ln_beta=beta.data_ptr(), ln_mean=mean.data_ptr(),
         ln_rstd=rstd.data_ptr(), ln_eps=float(eps), stream=_stream(),
     )
