@@ -13,6 +13,7 @@
 //   optim.SGD step           experiment/launch.py:152-155           -> sgd_multi
 //   time.sleep slowdown      scaelum/builder/module_wrapper.py:124-126,265-266 -> spin_* kernels
 #include <algorithm>
+#include <type_traits>
 
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -1075,6 +1076,48 @@ __device__ __forceinline__ float scaled_grad(float g, float grad_scale, float cl
   return g * grad_scale;
 }
 
+// One bank of a multi-tensor update (blockIdx.y picks the bank): a grid-stride float4 body and a
+// scalar tail in block 0.  upd(p, g, m, v) updates one element's master p in place from its raw
+// gradient g, with m / v the element's momentum / second moment, loaded and stored only when the
+// update uses them (has_mom / has_mom2).  The bf16 shadow refresh and the gradient zeroing
+// follow every element's update.
+template <typename Update>
+__device__ __forceinline__ void multi_tensor_update(const SgdTensor& t, int zero_grad, bool has_mom,
+                                                    bool has_mom2, Update upd) {
+  const long long n4 = t.numel >> 2;
+  float4* p4 = reinterpret_cast<float4*>(t.p);
+  float4* g4 = reinterpret_cast<float4*>(t.g);
+  float4* m4 = reinterpret_cast<float4*>(t.mom);
+  float4* v4 = reinterpret_cast<float4*>(t.mom2);
+  uint2* b4 = reinterpret_cast<uint2*>(t.p_bf16);
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n4;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float4 p = p4[i], m = has_mom ? m4[i] : float4{}, v = has_mom2 ? v4[i] : float4{};
+    const float4 g = g4[i];
+    upd(p.x, g.x, m.x, v.x);
+    upd(p.y, g.y, m.y, v.y);
+    upd(p.z, g.z, m.z, v.z);
+    upd(p.w, g.w, m.w, v.w);
+    p4[i] = p;
+    if (has_mom) m4[i] = m;
+    if (has_mom2) v4[i] = v;
+    if (b4 != nullptr) b4[i] = make_uint2(pack_bf16x2(p.x, p.y), pack_bf16x2(p.z, p.w));
+    if (zero_grad && !t.skip_zero) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  if (blockIdx.x == 0) {
+    for (long long i = (n4 << 2) + threadIdx.x; i < t.numel; i += blockDim.x) {
+      float p = t.p[i], m = has_mom ? t.mom[i] : 0.f, v = has_mom2 ? t.mom2[i] : 0.f;
+      upd(p, t.g[i], m, v);
+      t.p[i] = p;
+      if (has_mom) t.mom[i] = m;
+      if (has_mom2) t.mom2[i] = v;
+      if (t.p_bf16 != nullptr) reinterpret_cast<__nv_bfloat16*>(t.p_bf16)[i] = __float2bfloat16(p);
+      // zeroed even under skip_zero: harmless, the next step's first wgrad overwrites it anyway
+      if (zero_grad) t.g[i] = 0.f;
+    }
+  }
+}
+
 template <bool kScalars>
 __global__ void __launch_bounds__(256)
 sgd_multi_kernel(const SgdTensor* __restrict__ tensors, float lr, float momentum,
@@ -1086,52 +1129,15 @@ sgd_multi_kernel(const SgdTensor* __restrict__ tensors, float lr, float momentum
     lr = sc->lr;
     clip = sc->clip_coef;
   }
-  const long long n4 = t.numel >> 2;
-  float4* p4 = reinterpret_cast<float4*>(t.p);
-  float4* g4 = reinterpret_cast<float4*>(t.g);
-  float4* m4 = reinterpret_cast<float4*>(t.mom);
-  uint2* b4 = reinterpret_cast<uint2*>(t.p_bf16);
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n4;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    float4 p = p4[i];
-    float4 g = g4[i];
-    g.x = scaled_grad<kScalars>(g.x, grad_scale, clip) + weight_decay * p.x;
-    g.y = scaled_grad<kScalars>(g.y, grad_scale, clip) + weight_decay * p.y;
-    g.z = scaled_grad<kScalars>(g.z, grad_scale, clip) + weight_decay * p.z;
-    g.w = scaled_grad<kScalars>(g.w, grad_scale, clip) + weight_decay * p.w;
-    if (m4 != nullptr) {
-      float4 m = m4[i];
-      m.x = momentum * m.x + g.x;
-      m.y = momentum * m.y + g.y;
-      m.z = momentum * m.z + g.z;
-      m.w = momentum * m.w + g.w;
-      m4[i] = m;
+  const bool has_mom = t.mom != nullptr;
+  multi_tensor_update(t, zero_grad, has_mom, false, [&](float& p, float gi, float& m, float&) {
+    float g = scaled_grad<kScalars>(gi, grad_scale, clip) + weight_decay * p;
+    if (has_mom) {
+      m = momentum * m + g;
       g = m;
     }
-    p.x -= lr * g.x;
-    p.y -= lr * g.y;
-    p.z -= lr * g.z;
-    p.w -= lr * g.w;
-    p4[i] = p;
-    if (b4 != nullptr) b4[i] = make_uint2(pack_bf16x2(p.x, p.y), pack_bf16x2(p.z, p.w));
-    if (zero_grad && !t.skip_zero) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-  // scalar tail
-  if (blockIdx.x == 0) {
-    for (long long i = (n4 << 2) + threadIdx.x; i < t.numel; i += blockDim.x) {
-      float p = t.p[i];
-      float g = scaled_grad<kScalars>(t.g[i], grad_scale, clip) + weight_decay * p;
-      if (t.mom != nullptr) {
-        const float m = momentum * t.mom[i] + g;
-        t.mom[i] = m;
-        g = m;
-      }
-      p -= lr * g;
-      t.p[i] = p;
-      if (t.p_bf16 != nullptr) reinterpret_cast<__nv_bfloat16*>(t.p_bf16)[i] = __float2bfloat16(p);
-      if (zero_grad) t.g[i] = 0.f;
-    }
-  }
+    p -= lr * g;
+  });
 }
 
 // Adam / AdamW over the same descriptors (torch.optim.Adam semantics, experiment/launch.py:152-155
@@ -1155,44 +1161,13 @@ adam_multi_kernel(const SgdTensor* __restrict__ tensors, float lr, float beta1, 
   const float step_size = lr / bc1;
   const float decay = decoupled ? 1.f - lr * weight_decay : 1.f;
   const float l2 = decoupled ? 0.f : weight_decay;
-  auto upd = [&](float& p, float gi, float& m, float& v) {
+  multi_tensor_update(t, zero_grad, true, true, [&](float& p, float gi, float& m, float& v) {
     p *= decay;
     const float g = scaled_grad<kScalars>(gi, grad_scale, clip) + l2 * p;
     m = beta1 * m + (1.f - beta1) * g;
     v = beta2 * v + (1.f - beta2) * g * g;
     p -= step_size * m / (sqrtf(v) * bc2_rsqrt + eps);
-  };
-  const long long n4 = t.numel >> 2;
-  float4* p4 = reinterpret_cast<float4*>(t.p);
-  float4* g4 = reinterpret_cast<float4*>(t.g);
-  float4* m4 = reinterpret_cast<float4*>(t.mom);
-  float4* v4 = reinterpret_cast<float4*>(t.mom2);
-  uint2* b4 = reinterpret_cast<uint2*>(t.p_bf16);
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n4;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    float4 p = p4[i], m = m4[i], v = v4[i];
-    const float4 g = g4[i];
-    upd(p.x, g.x, m.x, v.x);
-    upd(p.y, g.y, m.y, v.y);
-    upd(p.z, g.z, m.z, v.z);
-    upd(p.w, g.w, m.w, v.w);
-    p4[i] = p;
-    m4[i] = m;
-    v4[i] = v;
-    if (b4 != nullptr) b4[i] = make_uint2(pack_bf16x2(p.x, p.y), pack_bf16x2(p.z, p.w));
-    if (zero_grad && !t.skip_zero) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-  if (blockIdx.x == 0) {
-    for (long long i = (n4 << 2) + threadIdx.x; i < t.numel; i += blockDim.x) {
-      float p = t.p[i], m = t.mom[i], v = t.mom2[i];
-      upd(p, t.g[i], m, v);
-      t.p[i] = p;
-      t.mom[i] = m;
-      t.mom2[i] = v;
-      if (t.p_bf16 != nullptr) reinterpret_cast<__nv_bfloat16*>(t.p_bf16)[i] = __float2bfloat16(p);
-      if (zero_grad) t.g[i] = 0.f;
-    }
-  }
+  });
 }
 
 // Global-norm clipping, step 1: per-block sums of squares of g * grad_scale over the same
@@ -1866,20 +1841,36 @@ int launch_mlm_scatter(const void* dx_c, const int* slot_of_row, long long rows,
   SKY_LAUNCH_CHECK();
 }
 
+namespace {
+// blocks per bank of sgd_multi / adam_multi / grad_sumsq_multi: one float4 per thread over the
+// largest bank, at most two per SM
+int multi_tensor_blocks(long long max_numel) {
+  long long blocks = (max_numel / 4 + 255) / 256;
+  if (blocks > num_sms() * 2) blocks = num_sms() * 2;
+  if (blocks < 1) blocks = 1;
+  return static_cast<int>(blocks);
+}
+
+// launch(std::true_type{}) when the device-side OptimScalars are given, launch(std::false_type{})
+// otherwise: the kScalars instantiation of an optimizer kernel
+template <typename Launch>
+void dispatch_scalars(const OptimScalars* scalars, Launch launch) {
+  if (scalars != nullptr)
+    launch(std::true_type{});
+  else
+    launch(std::false_type{});
+}
+}  // namespace
+
 int launch_sgd_multi(const SgdTensor* d_tensors, int n_tensors, long long max_numel, float lr,
                      float momentum, float weight_decay, float grad_scale, bool zero_grad,
                      cudaStream_t stream, const OptimScalars* scalars) {
   if (n_tensors <= 0) return 0;
-  long long blocks = (max_numel / 4 + 255) / 256;
-  if (blocks > num_sms() * 2) blocks = num_sms() * 2;
-  if (blocks < 1) blocks = 1;
-  dim3 grid(static_cast<unsigned>(blocks), n_tensors);
-  if (scalars != nullptr)
-    sgd_multi_kernel<true><<<grid, 256, 0, stream>>>(d_tensors, lr, momentum, weight_decay,
-                                                     grad_scale, zero_grad ? 1 : 0, scalars);
-  else
-    sgd_multi_kernel<false><<<grid, 256, 0, stream>>>(d_tensors, lr, momentum, weight_decay,
-                                                      grad_scale, zero_grad ? 1 : 0, nullptr);
+  dim3 grid(static_cast<unsigned>(multi_tensor_blocks(max_numel)), n_tensors);
+  dispatch_scalars(scalars, [&](auto k) {
+    sgd_multi_kernel<decltype(k)::value><<<grid, 256, 0, stream>>>(
+        d_tensors, lr, momentum, weight_decay, grad_scale, zero_grad ? 1 : 0, scalars);
+  });
   SKY_LAUNCH_CHECK();
 }
 
@@ -1889,27 +1880,16 @@ int launch_adam_multi(const SgdTensor* d_tensors, int n_tensors, long long max_n
                       const OptimScalars* scalars) {
   if (n_tensors <= 0) return 0;
   if (step == nullptr) return 906;
-  long long blocks = (max_numel / 4 + 255) / 256;
-  if (blocks > num_sms() * 2) blocks = num_sms() * 2;
-  if (blocks < 1) blocks = 1;
-  dim3 grid(static_cast<unsigned>(blocks), n_tensors);
-  if (scalars != nullptr)
-    adam_multi_kernel<true><<<grid, 256, 0, stream>>>(d_tensors, lr, beta1, beta2, eps,
-                                                      weight_decay, decoupled ? 1 : 0, step,
-                                                      grad_scale, zero_grad ? 1 : 0, scalars);
-  else
-    adam_multi_kernel<false><<<grid, 256, 0, stream>>>(d_tensors, lr, beta1, beta2, eps,
-                                                       weight_decay, decoupled ? 1 : 0, step,
-                                                       grad_scale, zero_grad ? 1 : 0, nullptr);
+  dim3 grid(static_cast<unsigned>(multi_tensor_blocks(max_numel)), n_tensors);
+  dispatch_scalars(scalars, [&](auto k) {
+    adam_multi_kernel<decltype(k)::value><<<grid, 256, 0, stream>>>(
+        d_tensors, lr, beta1, beta2, eps, weight_decay, decoupled ? 1 : 0, step, grad_scale,
+        zero_grad ? 1 : 0, scalars);
+  });
   SKY_LAUNCH_CHECK();
 }
 
-int grad_sumsq_blocks(long long max_numel) {
-  long long blocks = (max_numel / 4 + 255) / 256;
-  if (blocks > num_sms() * 2) blocks = num_sms() * 2;
-  if (blocks < 1) blocks = 1;
-  return static_cast<int>(blocks);
-}
+int grad_sumsq_blocks(long long max_numel) { return multi_tensor_blocks(max_numel); }
 
 int launch_grad_sumsq_multi(const SgdTensor* d_tensors, int n_tensors, int blocks,
                             float grad_scale, float* partials, cudaStream_t stream) {
@@ -1976,15 +1956,12 @@ int launch_lamb_moments(const LambSegment* segs, const int* chunk_seg, int n_chu
   if (n_chunks == 0) return 0;
   if (n_chunks < 0 || segs == nullptr || chunk_seg == nullptr || partials == nullptr) return 970;
   if (step == nullptr) return 971;
-  if (scalars != nullptr) {
-    static const int grid = lamb_grid(lamb_moments_kernel<true>, 1 << 30);
-    lamb_moments_kernel<true><<<std::min(grid, n_chunks), 256, 0, stream>>>(
+  dispatch_scalars(scalars, [&](auto k) {
+    constexpr bool kScalars = decltype(k)::value;
+    static const int grid = lamb_grid(lamb_moments_kernel<kScalars>, 1 << 30);
+    lamb_moments_kernel<kScalars><<<std::min(grid, n_chunks), 256, 0, stream>>>(
         segs, chunk_seg, n_chunks, beta1, beta2, eps, step, grad_scale, scalars, partials);
-  } else {
-    static const int grid = lamb_grid(lamb_moments_kernel<false>, 1 << 30);
-    lamb_moments_kernel<false><<<std::min(grid, n_chunks), 256, 0, stream>>>(
-        segs, chunk_seg, n_chunks, beta1, beta2, eps, step, grad_scale, nullptr, partials);
-  }
+  });
   SKY_LAUNCH_CHECK();
 }
 
@@ -1997,15 +1974,12 @@ int launch_lamb_update(const LambSegment* segs, const int* chunk_seg, int n_chun
       ratios == nullptr)
     return 970;
   if (step == nullptr) return 971;
-  if (scalars != nullptr) {
-    static const int grid = lamb_grid(lamb_update_kernel<true>, 1 << 30);
-    lamb_update_kernel<true><<<std::min(grid, n_chunks), 256, 0, stream>>>(
+  dispatch_scalars(scalars, [&](auto k) {
+    constexpr bool kScalars = decltype(k)::value;
+    static const int grid = lamb_grid(lamb_update_kernel<kScalars>, 1 << 30);
+    lamb_update_kernel<kScalars><<<std::min(grid, n_chunks), 256, 0, stream>>>(
         segs, chunk_seg, n_chunks, lr, beta1, beta2, eps, step, scalars, partials, ratios);
-  } else {
-    static const int grid = lamb_grid(lamb_update_kernel<false>, 1 << 30);
-    lamb_update_kernel<false><<<std::min(grid, n_chunks), 256, 0, stream>>>(
-        segs, chunk_seg, n_chunks, lr, beta1, beta2, eps, step, nullptr, partials, ratios);
-  }
+  });
   SKY_LAUNCH_CHECK();
 }
 

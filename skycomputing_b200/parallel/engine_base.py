@@ -333,10 +333,10 @@ class EngineBase:
     def _norm_info(self) -> tuple:
         """(needs the global gradient norm, can reduce it through peer memory): gathered with the
         other setup flags so that every rank picks the same reduction."""
-        from .optim import FusedSGD
+        from .optim import FusedOptimizer
 
         needs = bool(getattr(self.optimizer, "needs_global_norm", False))
-        return needs, needs and isinstance(self.optimizer, FusedSGD)
+        return needs, needs and isinstance(self.optimizer, FusedOptimizer)
 
     def _setup_grad_norm(self, position: int, num_positions: int, rank_of_position,
                          infos) -> None:

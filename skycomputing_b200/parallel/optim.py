@@ -33,9 +33,9 @@ with k = optimizer steps already taken, read from a device-side counter.
 """
 from __future__ import annotations
 
-from typing import Optional
-
 import math
+import os
+from typing import Optional
 
 import torch
 import torch.nn as nn
@@ -103,60 +103,60 @@ def check_grad_clip(cfg: Optional[dict]) -> Optional[float]:
     return max_norm
 
 
-class FusedSGD:
-    def __init__(self, module: nn.Module, lr: float = 1e-3, momentum: float = 0.0,
-                 weight_decay: float = 0.0, dampening: float = 0.0, nesterov: bool = False,
-                 banks: Optional[list] = None):
+# index of local_sumsq, this rank's share of grad_norm^2, in OptimScalars {lr, clip_coef,
+# grad_norm, local_sumsq} (csrc/kernels/api.h)
+_LOCAL_SUMSQ = 3
+
+
+class FusedOptimizer:
+    """What the fused optimizers share: the stage's de-duplicated parameter banks, a torch
+    optimizer for the parameters outside them, the device-side step counter, learning-rate
+    schedule and global-norm clipping, and one ``step()``.  A subclass supplies three things:
+    ``_state_buffers()`` ({state_dict key: one buffer or None per bank}), ``_fallback(module,
+    params)`` (the torch optimizer class and its parameter groups for the parameters outside the
+    banks) and ``_update(stream, grad_scale, scalars)``, which launches the update of every bank
+    (``scalars``: the device OptimScalars pointer, or 0)."""
+
+    def __init__(self, module: nn.Module, banks: Optional[list], defaults: dict, counter: bool):
         from ..models.bert_layers import native_param_banks
         from ..ops import native as nat
 
-        if dampening != 0.0 or nesterov:
-            raise ValueError("FusedSGD supports plain / momentum SGD only")
-        self.lr, self.momentum, self.weight_decay = lr, momentum, weight_decay
         self._nat = nat
-        self.banks = list(banks) if banks is not None else native_param_banks(module)
-        seen = set()
-        uniq = []
-        for b in self.banks:
-            if id(b) not in seen:
-                seen.add(id(b))
-                uniq.append(b)
-        self.banks = uniq
+        banks = native_param_banks(module) if banks is None else banks
+        self.banks = list({id(b): b for b in banks}.values())
         for b in self.banks:
             b.ensure()
-        bank_params = {id(p) for b in self.banks for p in b.params}
-        rest = [p for p in module.parameters() if id(p) not in bank_params and p.requires_grad]
-        self._rest_opt = (torch.optim.SGD(rest, lr=lr, momentum=momentum, weight_decay=weight_decay)
-                          if rest else None)
-        self._mom = ([torch.zeros_like(b.master()) for b in self.banks] if momentum else
-                     [None] * len(self.banks))
-        self._desc_dev: Optional[torch.Tensor] = None
-        self._max_numel = 0
-        import os as _os
-
-        self._overwrite_ok = _os.environ.get("SKY_SGD_OVERWRITE", "1") != "0"
-        self.param_groups = [dict(lr=lr, momentum=momentum, weight_decay=weight_decay)]
+        self.param_groups = [defaults]
         params = list(module.parameters())
         self._device = self.banks[0].master().device if self.banks else (
             params[0].device if params else torch.device("cpu"))
+        bank_params = {id(p) for b in self.banks for p in b.params}
+        rest = [p for p in params if id(p) not in bank_params and p.requires_grad]
+        cls, groups = self._fallback(module, rest) if rest else (None, None)
+        self._rest_opt = cls(groups) if rest else None
+        self._overwrite_ok = os.environ.get("SKY_SGD_OVERWRITE", "1") != "0"
+        self._zeroing_decided = False
+        self._desc_dev: Optional[torch.Tensor] = None
+        self._max_numel = 0
+        # device-side count of steps taken: Adam's bias correction and the learning-rate schedule
+        self._step = torch.zeros(1, dtype=torch.int64, device=self._device) if counter else None
+        self._step_offset = 0                     # schedule steps taken by an earlier optimizer
+        # learning-rate schedule / gradient clipping (configure()); all None = the plain update
+        self._sched: Optional[dict] = None
+        self._max_norm: Optional[float] = None
+        self._scalars: Optional[torch.Tensor] = None      # device OptimScalars
+        self._partials: Optional[torch.Tensor] = None
+        self._sumsq_blocks = 0
+        self._rest_sumsq: Optional[torch.Tensor] = None
+        self._norm_allreduce = False
+        self._norm_group = None
+        self._norm_exchange = None
+        self._stepped = False
 
     @property
     def graph_safe(self) -> bool:
         """True when step() is pure device work with static addresses (CUDA-graph capturable)."""
         return self._rest_opt is None
-
-    _mom2: list = []
-    # learning-rate schedule / gradient clipping (configure()); all None = the plain update
-    _step: Optional[torch.Tensor] = None          # device-side count of steps taken
-    _step_offset = 0                              # schedule steps taken by an earlier optimizer
-    _sched: Optional[dict] = None
-    _max_norm: Optional[float] = None
-    _scalars: Optional[torch.Tensor] = None       # device OptimScalars {lr, clip_coef, norm, local}
-    _partials: Optional[torch.Tensor] = None
-    _norm_allreduce = False
-    _norm_group = None
-    _norm_exchange = None
-    _stepped = False
 
     def configure(self, lr_schedule: Optional[dict] = None, max_norm: Optional[float] = None) -> None:
         """Device-side learning-rate schedule and / or global-norm clipping (validated configs,
@@ -188,7 +188,7 @@ class FusedSGD:
 
     def _compute_scalars(self, grad_scale: float, stream: int) -> None:
         """grad_sumsq_multi + optim_finalize: writes lr / clip_coef / grad_norm for this step,
-        reading k from the step counter before the caller advances it."""
+        reading k from the step counter before step() advances it."""
         ext = self._nat.ext()
         partials, n_part, extra = 0, 0, 0
         if self._max_norm is not None:
@@ -226,8 +226,9 @@ class FusedSGD:
             import torch.distributed as dist
 
             ext.optim_finalize(partials, n_part, extra, **common)    # this rank's share
-            dist.all_reduce(self._scalars[3:4], group=self._norm_group)
-            ext.optim_finalize(0, 0, self._scalars.data_ptr() + 12, **common)
+            local = self._scalars[_LOCAL_SUMSQ:_LOCAL_SUMSQ + 1]
+            dist.all_reduce(local, group=self._norm_group)
+            ext.optim_finalize(0, 0, local.data_ptr(), **common)
         else:
             ext.optim_finalize(partials, n_part, extra, **common)
 
@@ -264,14 +265,22 @@ class FusedSGD:
         restart with the new optimizer."""
         self._step_offset = int(k) - (int(self._step.item()) if self._step is not None else 0)
 
-    def _descriptors(self) -> torch.Tensor:
-        if self._desc_dev is None and self.banks:
-            # banks that received a wgrad GEMM in the first backward pass will receive one in every
-            # step: their gradient need not be zeroed, the next step's first wgrad overwrites it
+    def _decide_zeroing(self) -> None:
+        """Banks that received a wgrad GEMM in the first backward pass will receive one in every
+        step: their gradient need not be zeroed, the next step's first wgrad overwrites it
+        (``overwrite_first``).  Decided once, before the first descriptor or segment table."""
+        if not self._zeroing_decided:
             for b in self.banks:
                 b.overwrite_first = bool(getattr(b, "wgrad_target", False)) and self._overwrite_ok
-            mom2 = self._mom2 or [None] * len(self.banks)
-            descs = [b.sgd_descriptor(m, v) for b, m, v in zip(self.banks, self._mom, mom2)]
+            self._zeroing_decided = True
+
+    def _descriptors(self) -> torch.Tensor:
+        """The SgdTensor table of the banks on the device, built once."""
+        if self._desc_dev is None and self.banks:
+            self._decide_zeroing()
+            bufs = self._state_buffers()
+            mom2 = bufs.get("second_moment", [None] * len(self.banks))
+            descs = [b.sgd_descriptor(m, v) for b, m, v in zip(self.banks, bufs["momentum"], mom2)]
             raw = self._nat.ext().pack_sgd_descriptors(descs)
             host = torch.frombuffer(bytearray(raw), dtype=torch.uint8)
             self._desc_dev = host.to(self.banks[0].master().device)
@@ -279,22 +288,18 @@ class FusedSGD:
         return self._desc_dev
 
     def step(self, grad_scale: float = 1.0) -> None:
+        configured = self._scalars is not None
+        stream = torch.cuda.current_stream().cuda_stream if self.banks or configured else 0
         sc = 0
-        if self._scalars is not None:
-            stream = torch.cuda.current_stream().cuda_stream
+        if configured:
             self._compute_scalars(grad_scale, stream)
-            if self._step is not None:
-                self._nat.ext().advance_counter(self._step.data_ptr(), 1, stream)
             sc = self._scalars.data_ptr()
             self._stepped = True
+        # the counter counts the steps that ran device work, and only those
+        if self._step is not None and (self.banks or configured):
+            self._nat.ext().advance_counter(self._step.data_ptr(), 1, stream)
         if self.banks:
-            d = self._descriptors()
-            self._nat.ext().sgd_multi(d_tensors=d.data_ptr(), n=len(self.banks),
-                                      max_numel=self._max_numel, lr=float(self.param_groups[0]["lr"]),
-                                      momentum=float(self.momentum),
-                                      weight_decay=float(self.weight_decay),
-                                      grad_scale=float(grad_scale), zero_grad=True,
-                                      stream=torch.cuda.current_stream().cuda_stream, scalars=sc)
+            self._update(stream, float(grad_scale), sc)
             for b in self.banks:
                 if b.overwrite_first:
                     b.fresh = True
@@ -309,8 +314,9 @@ class FusedSGD:
             self._rest_opt.zero_grad(set_to_none=False)
 
     def state_dict(self) -> dict:
-        sd = dict(momentum=[None if m is None else m.detach().cpu() for m in self._mom],
-                  rest=None if self._rest_opt is None else self._rest_opt.state_dict(),
+        sd = {k: [None if t is None else t.detach().cpu() for t in bufs]
+              for k, bufs in self._state_buffers().items()}
+        sd.update(rest=None if self._rest_opt is None else self._rest_opt.state_dict(),
                   param_groups=self.param_groups)
         if self._step is not None:
             sd["step"] = int(self._step.item())
@@ -319,9 +325,10 @@ class FusedSGD:
         return sd
 
     def load_state_dict(self, sd: dict) -> None:
-        for m, s in zip(self._mom, sd.get("momentum", [])):
-            if m is not None and s is not None:
-                m.copy_(s)
+        for k, bufs in self._state_buffers().items():
+            for t, s in zip(bufs, sd.get(k, [])):
+                if t is not None and s is not None:
+                    t.copy_(s)
         if self._rest_opt is not None and sd.get("rest") is not None:
             self._rest_opt.load_state_dict(sd["rest"])
         self.param_groups = sd.get("param_groups", self.param_groups)
@@ -331,7 +338,36 @@ class FusedSGD:
             self.set_step_count(int(sd["lr_schedule_step"]))
 
 
-class FusedAdam(FusedSGD):
+class FusedSGD(FusedOptimizer):
+    """``torch.optim.SGD`` (plain or momentum) as one multi-tensor launch per step."""
+
+    def __init__(self, module: nn.Module, lr: float = 1e-3, momentum: float = 0.0,
+                 weight_decay: float = 0.0, dampening: float = 0.0, nesterov: bool = False,
+                 banks: Optional[list] = None):
+        if dampening != 0.0 or nesterov:
+            raise ValueError("FusedSGD supports plain / momentum SGD only")
+        self.lr, self.momentum, self.weight_decay = lr, momentum, weight_decay
+        super().__init__(module, banks, dict(lr=lr, momentum=momentum, weight_decay=weight_decay),
+                         counter=False)
+        self._mom = [torch.zeros_like(b.master()) if momentum else None for b in self.banks]
+
+    def _fallback(self, module, params):
+        return torch.optim.SGD, [dict(params=params, lr=self.lr, momentum=self.momentum,
+                                      weight_decay=self.weight_decay)]
+
+    def _state_buffers(self) -> dict:
+        return dict(momentum=self._mom)
+
+    def _update(self, stream, grad_scale, scalars):
+        d = self._descriptors()
+        self._nat.ext().sgd_multi(
+            d_tensors=d.data_ptr(), n=len(self.banks), max_numel=self._max_numel,
+            lr=float(self.param_groups[0]["lr"]), momentum=float(self.momentum),
+            weight_decay=float(self.weight_decay), grad_scale=grad_scale, zero_grad=True,
+            stream=stream, scalars=scalars)
+
+
+class FusedAdam(FusedOptimizer):
     """``torch.optim.Adam`` / ``AdamW`` (amsgrad=False) as one multi-tensor launch per step."""
 
     def __init__(self, module: nn.Module, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8,
@@ -339,54 +375,29 @@ class FusedAdam(FusedSGD):
                  maximize: bool = False, banks: Optional[list] = None, **unsupported):
         if amsgrad or maximize or unsupported:
             raise ValueError("FusedAdam covers plain Adam / AdamW only")
-        super().__init__(module, lr=lr, momentum=0.0, weight_decay=weight_decay, banks=banks)
+        self.lr, self.weight_decay = lr, weight_decay
         self.betas, self.eps, self.decoupled = (float(betas[0]), float(betas[1])), eps, decoupled
+        super().__init__(module, banks, dict(lr=lr, betas=self.betas, eps=eps,
+                                             weight_decay=weight_decay), counter=True)
         self._mom = [torch.zeros_like(b.master()) for b in self.banks]
         self._mom2 = [torch.zeros_like(b.master()) for b in self.banks]
-        dev = self.banks[0].master().device if self.banks else torch.device("cpu")
-        self._step = torch.zeros(1, dtype=torch.int64, device=dev)   # device-side step count
-        if self._rest_opt is not None:
-            rest = [p for g in self._rest_opt.param_groups for p in g["params"]]
-            cls = torch.optim.AdamW if decoupled else torch.optim.Adam
-            self._rest_opt = cls(rest, lr=lr, betas=self.betas, eps=eps, weight_decay=weight_decay)
-        self.param_groups = [dict(lr=lr, betas=self.betas, eps=eps, weight_decay=weight_decay)]
 
-    def step(self, grad_scale: float = 1.0) -> None:
-        sc = 0
-        if self._scalars is not None:
-            self._compute_scalars(grad_scale, torch.cuda.current_stream().cuda_stream)
-            sc = self._scalars.data_ptr()
-            self._stepped = True
-        if self.banks:
-            d = self._descriptors()
-            ext = self._nat.ext()
-            stream = torch.cuda.current_stream().cuda_stream
-            ext.advance_counter(self._step.data_ptr(), 1, stream)
-            ext.adam_multi(d_tensors=d.data_ptr(), n=len(self.banks), max_numel=self._max_numel,
-                           lr=float(self.param_groups[0]["lr"]), beta1=self.betas[0],
-                           beta2=self.betas[1], eps=float(self.eps),
-                           weight_decay=float(self.weight_decay), decoupled=bool(self.decoupled),
-                           step=self._step.data_ptr(), grad_scale=float(grad_scale),
-                           zero_grad=True, stream=stream, scalars=sc)
-            for b in self.banks:
-                if b.overwrite_first:
-                    b.fresh = True
-        elif self._scalars is not None:
-            self._nat.ext().advance_counter(self._step.data_ptr(), 1,
-                                            torch.cuda.current_stream().cuda_stream)
-        if self._rest_opt is not None:
-            self._rest_step()
+    def _fallback(self, module, params):
+        cls = torch.optim.AdamW if self.decoupled else torch.optim.Adam
+        return cls, [dict(params=params, lr=self.lr, betas=self.betas, eps=self.eps,
+                          weight_decay=self.weight_decay)]
 
-    def state_dict(self) -> dict:
-        sd = super().state_dict()
-        sd["second_moment"] = [v.detach().cpu() for v in self._mom2]
-        return sd
+    def _state_buffers(self) -> dict:
+        return dict(momentum=self._mom, second_moment=self._mom2)
 
-    def load_state_dict(self, sd: dict) -> None:
-        super().load_state_dict(sd)
-        for v, s_ in zip(self._mom2, sd.get("second_moment", [])):
-            if s_ is not None:
-                v.copy_(s_)
+    def _update(self, stream, grad_scale, scalars):
+        d = self._descriptors()
+        self._nat.ext().adam_multi(
+            d_tensors=d.data_ptr(), n=len(self.banks), max_numel=self._max_numel,
+            lr=float(self.param_groups[0]["lr"]), beta1=self.betas[0], beta2=self.betas[1],
+            eps=float(self.eps), weight_decay=float(self.weight_decay),
+            decoupled=bool(self.decoupled), step=self._step.data_ptr(), grad_scale=grad_scale,
+            zero_grad=True, stream=stream, scalars=scalars)
 
 
 LAMB_DEFAULTS = dict(lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.01,
@@ -502,25 +513,27 @@ class FusedLamb(FusedAdam):
     holds three).  ``lamb_moments`` updates m and v and writes fp32 partials of ||W||² and ||u||²
     per fixed-size chunk; ``lamb_update`` sums a segment's partials in fp64 in a fixed order, forms
     r and applies the update with the bf16 shadow refresh.  No host sync, no per-step host-to-device
-    copy: graph-safe like ``FusedAdam``, whose moments, step counter, schedule / clipping path and
-    state_dict it shares.  Parameters outside the banks are stepped by ``Lamb``."""
+    copy: graph-safe like ``FusedAdam``, whose moments and step counter it shares.  Parameters outside the banks are stepped by ``Lamb``."""
 
     def __init__(self, module: nn.Module, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-6,
                  weight_decay: float = 0.01, exclude_from_weight_decay=("bias", "LayerNorm"),
                  banks: Optional[list] = None):
         chk = check_lamb_cfg(dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
                                   exclude_from_weight_decay=exclude_from_weight_decay))
-        super().__init__(module, lr=chk["lr"], betas=chk["betas"], eps=chk["eps"],
-                         weight_decay=chk["weight_decay"], decoupled=True, banks=banks)
         self.exclude = chk["exclude_from_weight_decay"]
         self._names = {id(p): n for n, p in module.named_parameters()}
-        if self._rest_opt is not None:
-            rest = [p for g in self._rest_opt.param_groups for p in g["params"]]
-            self._rest_opt = Lamb(lamb_param_groups(module, self.weight_decay, self.exclude, rest),
-                                  lr=self.lr, betas=self.betas, eps=self.eps)
+        super().__init__(module, lr=chk["lr"], betas=chk["betas"], eps=chk["eps"],
+                         weight_decay=chk["weight_decay"], decoupled=True, banks=banks)
         self.param_groups[0]["exclude_from_weight_decay"] = self.exclude
         self._lamb = None          # (segments, chunk table, n_chunks) on the device, built once
         self._seg_info: list = []
+        self._lamb_partials: Optional[torch.Tensor] = None
+        self._ratios: Optional[torch.Tensor] = None
+        self._lamb_stepped = False
+
+    def _fallback(self, module, params):
+        groups = lamb_param_groups(module, self.weight_decay, self.exclude, params)
+        return Lamb, [dict(g, lr=self.lr, betas=self.betas, eps=self.eps) for g in groups]
 
     def segments(self) -> list:
         """The segment table as dicts: name, bank (index into ``banks``), offset and numel in the
@@ -531,7 +544,7 @@ class FusedLamb(FusedAdam):
 
     def _lamb_table(self):
         if self._lamb is None:
-            self._descriptors()          # decides overwrite_first (skip_zero) for every bank
+            self._decide_zeroing()
             ext = self._nat.ext()
             info = lamb_segments(self.banks, self._names, self.weight_decay, self.exclude)
             rows = []
@@ -555,36 +568,18 @@ class FusedLamb(FusedAdam):
             self._seg_info = info
         return self._lamb
 
-    def step(self, grad_scale: float = 1.0) -> None:
-        sc = 0
-        stream = torch.cuda.current_stream().cuda_stream if self.banks else 0
-        if self._scalars is not None:
-            stream = torch.cuda.current_stream().cuda_stream
-            self._compute_scalars(grad_scale, stream)
-            sc = self._scalars.data_ptr()
-            self._stepped = True
-        if self.banks:
-            segs, chunks, n_chunks = self._lamb_table()
-            ext = self._nat.ext()
-            ext.advance_counter(self._step.data_ptr(), 1, stream)
-            b1, b2 = self.betas
-            ext.lamb_moments(segs.data_ptr(), chunks.data_ptr(), n_chunks, b1, b2, float(self.eps),
-                             self._step.data_ptr(), float(grad_scale),
-                             self._lamb_partials.data_ptr(), stream, sc)
-            ext.lamb_update(segs.data_ptr(), chunks.data_ptr(), n_chunks,
-                            float(self.param_groups[0]["lr"]), b1, b2, float(self.eps),
-                            self._step.data_ptr(), self._lamb_partials.data_ptr(),
-                            self._ratios.data_ptr(), stream, sc)
-            for b in self.banks:
-                if b.overwrite_first:
-                    b.fresh = True
-            self._lamb_stepped = True
-        elif self._scalars is not None:
-            self._nat.ext().advance_counter(self._step.data_ptr(), 1, stream)
-        if self._rest_opt is not None:
-            self._rest_step()
-
-    _lamb_stepped = False
+    def _update(self, stream, grad_scale, scalars):
+        segs, chunks, n_chunks = self._lamb_table()
+        ext = self._nat.ext()
+        b1, b2 = self.betas
+        ext.lamb_moments(segs.data_ptr(), chunks.data_ptr(), n_chunks, b1, b2, float(self.eps),
+                         self._step.data_ptr(), grad_scale, self._lamb_partials.data_ptr(), stream,
+                         scalars)
+        ext.lamb_update(segs.data_ptr(), chunks.data_ptr(), n_chunks,
+                        float(self.param_groups[0]["lr"]), b1, b2, float(self.eps),
+                        self._step.data_ptr(), self._lamb_partials.data_ptr(),
+                        self._ratios.data_ptr(), stream, scalars)
+        self._lamb_stepped = True
 
     def trust_ratios(self) -> dict:
         """{parameter name: r} of the last step (one device-to-host copy; {} before the first
@@ -736,34 +731,31 @@ def _build_optimizer(module: nn.Module, optim_cfg: dict, prefer_fused: bool):
     cfg = dict(optim_cfg)
     optim_type = cfg.pop("optim_type", "SGD")
     params = [p for p in module.parameters() if p.requires_grad]
-    on_cuda = any(p.is_cuda for p in params)
+    fused = False
+    if prefer_fused and any(p.is_cuda for p in params):
+        from ..models.bert_layers import get_backend
+        from ..ops import native as nat
+
+        fused = get_backend() != "torch" and nat.available()
     if optim_type == "LAMB":
         # no torch.optim class to fall back to: every option is checked here, on every backend
         cfg = check_lamb_cfg(cfg)
-        if prefer_fused and on_cuda:
-            from ..models.bert_layers import get_backend
-            from ..ops import native as nat
-
-            if get_backend() != "torch" and nat.available():
-                return FusedLamb(module, **cfg)
+        if fused:
+            return FusedLamb(module, **cfg)
         if params:
             excl = cfg.pop("exclude_from_weight_decay")
             return TorchOptimizerAdapter(
                 Lamb(lamb_param_groups(module, cfg["weight_decay"], excl), **cfg))
-    if optim_type in ("SGD", "Adam", "AdamW") and prefer_fused and on_cuda:
-        from ..models.bert_layers import get_backend
-        from ..ops import native as nat
-
-        if get_backend() != "torch" and nat.available():
-            try:
-                if optim_type == "SGD":
-                    return FusedSGD(module, **cfg)
-                if optim_type == "AdamW":
-                    cfg.setdefault("weight_decay", 1e-2)   # torch.optim.AdamW's default
-                return FusedAdam(module, decoupled=optim_type == "AdamW", **cfg)
-            except (ValueError, TypeError):
-                cfg = dict(optim_cfg)
-                cfg.pop("optim_type", None)
+    if optim_type in ("SGD", "Adam", "AdamW") and fused:
+        try:
+            if optim_type == "SGD":
+                return FusedSGD(module, **cfg)
+            if optim_type == "AdamW":
+                cfg.setdefault("weight_decay", 1e-2)   # torch.optim.AdamW's default
+            return FusedAdam(module, decoupled=optim_type == "AdamW", **cfg)
+        except (ValueError, TypeError):
+            cfg = dict(optim_cfg)
+            cfg.pop("optim_type", None)
     if not params:
         return TorchOptimizerAdapter(torch.optim.SGD([torch.nn.Parameter(torch.zeros(1))], lr=0.0))
     return TorchOptimizerAdapter(getattr(torch.optim, optim_type)(params, **cfg))

@@ -78,22 +78,12 @@ def test_fused_sgd_marks_only_wgrad_targets(monkeypatch):
         def sgd_multi(self, **kw):
             self.stepped = kw
 
-    class FakeNat:
-        def __init__(self):
-            self._e = FakeExt()
-
-        def ext(self):
-            return self._e
-
+    fake = FakeExt()
+    monkeypatch.setattr(F.nat, "ext", lambda: fake)
+    monkeypatch.delenv("SKY_SGD_OVERWRITE", raising=False)
     w, b = _bank(4, 3), _bank(4)
     w.wgrad_target = True
-    opt = optim.FusedSGD.__new__(optim.FusedSGD)
-    opt.lr, opt.momentum, opt.weight_decay = 0.1, 0.0, 0.0
-    opt._nat = FakeNat()
-    opt.banks, opt._mom = [w, b], [None, None]
-    opt._rest_opt, opt._desc_dev, opt._max_numel = None, None, 0
-    opt._overwrite_ok = True
-    opt.param_groups = [dict(lr=0.1, momentum=0.0, weight_decay=0.0)]
+    opt = optim.FusedSGD(torch.nn.Module(), lr=0.1, banks=[w, b])
     monkeypatch.setattr(torch.cuda, "current_stream", lambda *a, **k: type("S", (), {"cuda_stream": 0})())
     opt.step()
     assert [d[5] for d in opt._nat.ext().descs] == [1, 0]
