@@ -44,9 +44,14 @@ void gemm(uintptr_t A, uintptr_t B, int M, int N, int K, int lda, int ldb, bool 
           uintptr_t rng_state, uint32_t rng_stream, uintptr_t signal_flags, uintptr_t wait_flags,
           uintptr_t wait_epoch, uint32_t wait_mult, uintptr_t error_flag, int block_n, int pair, int stream_k, int max_ctas,
           int debug, uintptr_t ln_gamma, uintptr_t ln_beta, uintptr_t ln_mean, uintptr_t ln_rstd,
-          float ln_eps,
-          uintptr_t stream) {
+          float ln_eps, uintptr_t sgd_master, uintptr_t sgd_shadow, float sgd_lr,
+          float sgd_weight_decay, float sgd_grad_scale, uintptr_t stream) {
   GemmArgs a;
+  a.sgd_master = P<float>(sgd_master);
+  a.sgd_shadow = P<void>(sgd_shadow);
+  a.sgd_lr = sgd_lr;
+  a.sgd_weight_decay = sgd_weight_decay;
+  a.sgd_grad_scale = sgd_grad_scale;
   a.ln_gamma = P<const float>(ln_gamma);
   a.ln_beta = P<const float>(ln_beta);
   a.ln_mean = P<float>(ln_mean);
@@ -496,7 +501,9 @@ PYBIND11_MODULE(_cuda, m) {
         py::arg("wait_mult") = 0, py::arg("error_flag") = 0, py::arg("block_n") = 0, py::arg("pair") = -1, py::arg("stream_k") = -1,
         py::arg("max_ctas") = 0, py::arg("debug") = 0, py::arg("ln_gamma") = 0,
         py::arg("ln_beta") = 0, py::arg("ln_mean") = 0, py::arg("ln_rstd") = 0,
-        py::arg("ln_eps") = 1e-12f, py::arg("stream") = 0);
+        py::arg("ln_eps") = 1e-12f, py::arg("sgd_master") = 0, py::arg("sgd_shadow") = 0,
+        py::arg("sgd_lr") = 0.f, py::arg("sgd_weight_decay") = 0.f,
+        py::arg("sgd_grad_scale") = 1.f, py::arg("stream") = 0);
   m.def("attention_supported", &sky::attention_supported, py::arg("S"), py::arg("head_dim"));
   m.def("gemm_ln_block_n", &sky::gemm_ln_block_n, py::arg("M"), py::arg("N"),
         py::arg("force") = false);

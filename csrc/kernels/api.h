@@ -64,6 +64,16 @@ struct GemmArgs {
   // loads only (no MMAs), no epilogue.  With clusters (pair != 0), 3 and 4 only drop the epilogue.
   int debug = 0;
   int max_ctas = 0;           // 0 = all SMs
+  // SGD update in the epilogue of a weight gradient (sgd_master != nullptr).  The fp32 result g (or
+  // out + g when accumulate) is NOT stored; the epilogue applies sgd_multi's plain update with it,
+  //   sgd_master -= sgd_lr * (g * sgd_grad_scale + sgd_weight_decay * sgd_master),
+  // and writes the new value to the bf16 sgd_shadow, both laid out as `out` ([M, N], row stride
+  // ldo).  Only with out_f32, a_mn and b_mn, and without bias / aux / out2 / act / dropout / flags
+  // or an explicit stream-K or cluster schedule (980); sgd_shadow must be non-null and out,
+  // sgd_master and sgd_shadow 16-byte aligned with ldo % 8 == 0 (981).
+  float* sgd_master = nullptr;
+  void* sgd_shadow = nullptr;
+  float sgd_lr = 0.f, sgd_weight_decay = 0.f, sgd_grad_scale = 1.f;
 };
 
 // Returns 0 on success, a cudaError_t / CUresult-like code otherwise.

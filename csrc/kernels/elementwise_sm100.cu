@@ -1131,12 +1131,12 @@ sgd_multi_kernel(const SgdTensor* __restrict__ tensors, float lr, float momentum
   }
   const bool has_mom = t.mom != nullptr;
   multi_tensor_update(t, zero_grad, has_mom, false, [&](float& p, float gi, float& m, float&) {
-    float g = scaled_grad<kScalars>(gi, grad_scale, clip) + weight_decay * p;
+    float g = sgd_direction<kScalars>(gi, p, grad_scale, clip, weight_decay);
     if (has_mom) {
-      m = momentum * m + g;
+      m = __fmaf_rn(momentum, m, g);
       g = m;
     }
-    p -= lr * g;
+    p = sgd_apply(p, g, lr);
   });
 }
 

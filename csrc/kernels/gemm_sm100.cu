@@ -164,6 +164,10 @@ struct GemmDev : GemmCommon {
   int stream_k;
   float* ws;           // partial accumulators: slot (2 * unit + which) * ctas_per_unit + cta_rank
   uint32_t* counters;  // per CTA tile: [2 * t] arrivals, [2 * t + 1] partials written
+  // SGD update in the epilogue (gemm_wgrad_sgd_kernel only, see GemmArgs::sgd_master)
+  float* sgd_p;
+  __nv_bfloat16* sgd_shadow;
+  float sgd_lr, sgd_weight_decay, sgd_grad_scale;
 };
 
 struct Work {
@@ -431,6 +435,62 @@ __device__ __forceinline__ void publish_panel(uint32_t* signal_flags, int m_blk,
   if (epi_tid == 0) red_release_sys_add(signal_flags + m_blk, 1u);
 }
 
+// ---- SGD update in the weight-gradient epilogue (UPD, see gemm_body) ----
+// The producer pulls a tile's fp32 masters (and, when accumulating, the gradient the epilogue adds
+// to) into L2 this many k-blocks before the tile's main loop ends, so that the epilogue's reads do
+// not wait on HBM.
+constexpr int kSgdPrefetchKBlocks = 8;
+// producer warp: one bulk L2 prefetch per row of the tile (rows >= M skipped); the rows are
+// 16-byte aligned because the launcher checks the pointers and ldo % 8 == 0
+__device__ __forceinline__ void prefetch_update_tile(const GemmDev& p, int row0, int col0,
+                                                     int block_n, int lane) {
+  const int cols = min(block_n, p.N - col0);
+  if (cols <= 0) return;
+  const uint32_t bytes = static_cast<uint32_t>(cols) * 4u;  // a multiple of 32: N % 8 == 0
+  for (int r = lane; r < BLOCK_M && row0 + r < p.M; r += 32) {
+    const long long off = static_cast<long long>(row0 + r) * p.ldo + col0;
+    prefetch_l2_bulk(p.sgd_p + off, bytes);
+    if (p.accumulate) prefetch_l2_bulk(reinterpret_cast<const float*>(p.out) + off, bytes);
+  }
+}
+// f (the group's fp32 fragments of dW) -> the gradient g that the plain fp32 epilogue would leave in
+// p.out (f, or p.out + f when accumulating); the master p is updated with sgd_multi_kernel's
+// arithmetic and f gets the new p for the shadow store.  The gradient itself is not stored.
+__device__ __forceinline__ void frag_sgd_update(float (&f)[32], const GemmDev& p, long long row_a,
+                                                int col0, int fc) {
+  const float* grad = reinterpret_cast<const float*>(p.out);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const long long row = row_a + 8 * h;
+    if (row >= p.M) continue;
+    const long long off = row * p.ldo + col0 + fc;
+    float2 w[8], g0[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {  // every load of the row in flight before the math
+      const bool in = col0 + j * 8 < p.N;  // covers fc, fc + 1 because N % 8 == 0
+      w[j] = in ? *reinterpret_cast<const float2*>(p.sgd_p + off + j * 8) : make_float2(0.f, 0.f);
+      g0[j] = (in && p.accumulate) ? *reinterpret_cast<const float2*>(grad + off + j * 8)
+                                   : make_float2(0.f, 0.f);
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      if (col0 + j * 8 >= p.N) continue;
+      float gx = f[4 * j + 2 * h], gy = f[4 * j + 2 * h + 1];
+      if (p.accumulate) {
+        gx = g0[j].x + gx;
+        gy = g0[j].y + gy;
+      }
+      w[j].x = sgd_apply(w[j].x, sgd_direction<false>(gx, w[j].x, p.sgd_grad_scale, 1.f,
+                                                      p.sgd_weight_decay), p.sgd_lr);
+      w[j].y = sgd_apply(w[j].y, sgd_direction<false>(gy, w[j].y, p.sgd_grad_scale, 1.f,
+                                                      p.sgd_weight_decay), p.sgd_lr);
+      *reinterpret_cast<float2*>(p.sgd_p + off + j * 8) = w[j];
+      f[4 * j + 2 * h] = w[j].x;
+      f[4 * j + 2 * h + 1] = w[j].y;
+    }
+  }
+}
+
 // CL = CTAs per cluster: 1 = independent CTAs; 2 = two CTAs that compute vertically neighbouring
 // tiles (256 rows, the same BLOCK_N columns) and share the B operand: each fetches half of the B
 // tile from L2 and TMA multicasts it to both; 4 = two such pairs on neighbouring N tiles that also
@@ -438,10 +498,15 @@ __device__ __forceinline__ void publish_panel(uint32_t* signal_flags, int m_blk,
 // the other pair that needs the same rows).
 // SK = stream-K schedule compiled in (a separate instantiation: its bookkeeping costs registers in
 // the epilogue, which the classic kernels - the ones every training step runs - must not pay).
-template <int BLOCK_N, bool A_MN, bool B_MN, bool OUT_F32, int CL, bool SK>
-__global__ void __launch_bounds__(kNumThreads, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                  const __grid_constant__ CUtensorMap tmap_b, const GemmDev p) {
+// UPD = the fp32 result is a weight gradient that is not stored: the epilogue applies the SGD
+// update to the master weights and their bf16 shadow instead (gemm_wgrad_sgd_kernel; no bias,
+// activation, dropout or aux input, single CTAs, classic schedule).
+template <int BLOCK_N, bool A_MN, bool B_MN, bool OUT_F32, int CL, bool SK, bool UPD>
+__device__ __forceinline__ void gemm_body(const CUtensorMap* tmap_a_, const CUtensorMap* tmap_b_,
+                                          const GemmDev& p) {
+  static_assert(!UPD || (OUT_F32 && CL == 1 && !SK), "the SGD epilogue needs fp32 single CTAs");
+  const CUtensorMap& tmap_a = *tmap_a_;
+  const CUtensorMap& tmap_b = *tmap_b_;
   constexpr bool PAIR = CL >= 2;
   constexpr bool MC = CL == 4;
   using C = Cfg<BLOCK_N>;
@@ -495,6 +560,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
         const int b_row0 = n_blk * BLOCK_N + static_cast<int>(cta_rank) * (PAIR ? BLOCK_N / 2 : 0);
         if (p.wait_flags != nullptr && m_blk * BLOCK_M < p.M) wait_inbound_panel(p, m_blk);
         for (int kb = w.kb0; kb < w.kb1; ++kb, ring.advance()) {
+          if constexpr (UPD) {
+            if (kb == max(w.kb0, w.kb1 - kSgdPrefetchKBlocks))
+              prefetch_update_tile(p, m_blk * BLOCK_M, n_blk * BLOCK_N, BLOCK_N, lane);
+          }
           mbar_wait_cluster(&op.empty_bar[ring.stage], ring.phase ^ 1);
           load_k_block<BLOCK_N, A_MN, B_MN, CL>(op, ring.stage, &tmap_a, &tmap_b, kb,
                                                 m_blk * BLOCK_M, b_row0, cl_rank, p.debug == 3);
@@ -509,7 +578,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
     // before the epilogue math, fp32 gradient accumulation uses red.global.add (no
     // read-modify-write).
     const Consumer c = consumer_of(warp_idx, lane, op.base + C::kOffOut, p);
-    const bool has_aux = p.aux != nullptr;
+    const bool has_aux = !UPD && p.aux != nullptr;
     int it = 0;
     Ring<kStages> ring;
     // both MN- and K-major A tiles keep rows 64..127 one 8 KB block after rows 0..63
@@ -616,21 +685,26 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
             }
           }
         }
-        frag_add_bias(f, sb, ct, c.fc);
-        if (p.act == ACT_GELU) {
-          if (p.out2 != nullptr && p.debug != 2)
-            frag_store_bf16(f, c.stage, lane, reinterpret_cast<__nv_bfloat16*>(p.out2), p.ldo2,
-                            warp_row0, p.M, col0, p.N);
+        if constexpr (!UPD) {
+          frag_add_bias(f, sb, ct, c.fc);
+          if (p.act == ACT_GELU) {
+            if (p.out2 != nullptr && p.debug != 2)
+              frag_store_bf16(f, c.stage, lane, reinterpret_cast<__nv_bfloat16*>(p.out2), p.ldo2,
+                              warp_row0, p.M, col0, p.N);
 #pragma unroll
-          for (int i = 0; i < 32; ++i) f[i] = gelu_fast(f[i]);
-        } else if (p.act == ACT_TANH) {
+            for (int i = 0; i < 32; ++i) f[i] = gelu_fast(f[i]);
+          } else if (p.act == ACT_TANH) {
 #pragma unroll
-          for (int i = 0; i < 32; ++i) f[i] = tanh_fast(f[i]);
+            for (int i = 0; i < 32; ++i) f[i] = tanh_fast(f[i]);
+          }
+          if (c.dr.on) frag_dropout(f, c.dr.seed, c.dr.thr16, c.dr.scale, row_a, col0, p.N, lane);
+          if (has_aux) frag_apply_aux(f, ax, c.stage, lane, p.act == ACT_DGELU_MUL_AUX, p.add_aux);
         }
-        if (c.dr.on) frag_dropout(f, c.dr.seed, c.dr.thr16, c.dr.scale, row_a, col0, p.N, lane);
-        if (has_aux) frag_apply_aux(f, ax, c.stage, lane, p.act == ACT_DGELU_MUL_AUX, p.add_aux);
         if (p.debug != 2) {
-          if constexpr (OUT_F32) {
+          if constexpr (UPD) {
+            frag_sgd_update(f, p, row_a, col0, c.fc);
+            frag_store_bf16(f, c.stage, lane, p.sgd_shadow, p.ldo, warp_row0, p.M, col0, p.N);
+          } else if constexpr (OUT_F32) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               const long long row = row_a + 8 * h;
@@ -671,6 +745,22 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
     cluster_sync_all();  // no CTA may leave while a peer still multicasts into / signals it
   else
     __syncthreads();
+}
+
+template <int BLOCK_N, bool A_MN, bool B_MN, bool OUT_F32, int CL, bool SK>
+__global__ void __launch_bounds__(kNumThreads, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                  const __grid_constant__ CUtensorMap tmap_b, const GemmDev p) {
+  gemm_body<BLOCK_N, A_MN, B_MN, OUT_F32, CL, SK, false>(&tmap_a, &tmap_b, p);
+}
+
+// dW (+)= dY^T X with both operands MN-major over the tokens, and the SGD update of W in the
+// epilogue instead of the store of dW (GemmArgs::sgd_master)
+template <int BLOCK_N>
+__global__ void __launch_bounds__(kNumThreads, 1)
+gemm_wgrad_sgd_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                      const __grid_constant__ CUtensorMap tmap_b, const GemmDev p) {
+  gemm_body<BLOCK_N, true, true, true, 1, false, true>(&tmap_a, &tmap_b, p);
 }
 
 
@@ -1175,7 +1265,7 @@ GemmCommon common_of(const GemmArgs& a) {
   return c;
 }
 
-template <int BLOCK_N, bool A_MN, bool B_MN, bool OUT_F32, int CL>
+template <int BLOCK_N, bool A_MN, bool B_MN, bool OUT_F32, int CL, bool UPD = false>
 int launch_inst(const GemmArgs& a, GemmDev d, cudaStream_t stream) {
   constexpr bool PAIR = CL >= 2;
   constexpr bool MC = CL == 4;
@@ -1203,8 +1293,9 @@ int launch_inst(const GemmArgs& a, GemmDev d, cudaStream_t stream) {
   int units = max_units;
   if (a.max_ctas > 0 && units > a.max_ctas / CL) units = a.max_ctas / CL;
   if (units < 1) units = 1;
-  // stream-K instantiations exist for independent CTAs only (pairs / clusters did not profit)
-  if constexpr (CL == 1) {
+  // stream-K instantiations exist for independent CTAs only (pairs / clusters did not profit), and
+  // none with the SGD epilogue
+  if constexpr (CL == 1 && !UPD) {
     const int nk = (a.K + BLOCK_K - 1) / BLOCK_K;
     bool sk = a.stream_k < 0 ? want_stream_k(tiles, nk, units) : (a.stream_k != 0);
     // every CTA must own at least 4 k-blocks, the CTA tiles must fit the counter array, a bias
@@ -1226,6 +1317,8 @@ int launch_inst(const GemmArgs& a, GemmDev d, cudaStream_t stream) {
   if (a.max_ctas > 0 && grid > a.max_ctas / CL) grid = a.max_ctas / CL;
   if (grid < 1) grid = 1;
   grid *= CL;
+  if constexpr (UPD)
+    return launch<gemm_wgrad_sgd_kernel<BLOCK_N>>(grid, 1, C::kSmemBytes, stream, tma, tmb, d);
   if constexpr (CL == 1) {
     if (d.stream_k)
       return launch<gemm_wgmma_kernel<BLOCK_N, A_MN, B_MN, OUT_F32, 1, true>>(
@@ -1248,6 +1341,29 @@ int dispatch_major(const GemmArgs& a, const GemmDev& dev, cudaStream_t stream) {
                      : launch_inst<BLOCK_N, true, true, false, PAIR>(a, dev, stream);
   return a.out_f32 ? launch_inst<BLOCK_N, true, false, true, PAIR>(a, dev, stream)
                    : launch_inst<BLOCK_N, true, false, false, PAIR>(a, dev, stream);
+}
+
+bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15u) == 0; }
+
+// the weight gradient with the SGD update in its epilogue (GemmArgs::sgd_master)
+int launch_wgrad_sgd(const GemmArgs& a, GemmDev d, cudaStream_t stream) {
+  // an opt-in stream-K or cluster schedule would apply the update once per partial / CTA
+  if (!a.out_f32 || !a.a_mn || !a.b_mn || a.stream_k > 0 || a.pair > 0 || a.bias != nullptr ||
+      a.aux != nullptr || a.out2 != nullptr || a.act != ACT_NONE || a.dropout_p > 0.f ||
+      a.signal_flags != nullptr || a.wait_flags != nullptr)
+    return 980;
+  if (a.sgd_shadow == nullptr || a.out == nullptr || !aligned16(a.out) ||
+      !aligned16(a.sgd_master) || !aligned16(a.sgd_shadow) || (a.ldo % 8) != 0)
+    return 981;
+  d.sgd_p = a.sgd_master;
+  d.sgd_shadow = reinterpret_cast<__nv_bfloat16*>(a.sgd_shadow);
+  d.sgd_lr = a.sgd_lr;
+  d.sgd_weight_decay = a.sgd_weight_decay;
+  d.sgd_grad_scale = a.sgd_grad_scale;
+  const int bn = a.block_n ? a.block_n : gemm_pick_block_n(a.M, a.N);
+  if (bn == 256) return launch_inst<256, true, true, true, 1, true>(a, d, stream);
+  if (bn == 128) return launch_inst<128, true, true, true, 1, true>(a, d, stream);
+  return 905;
 }
 }  // namespace
 
@@ -1385,6 +1501,7 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   d.add_aux = a.add_aux ? 1 : 0;
   d.accumulate = a.accumulate ? 1 : 0;
   d.debug = a.debug;
+  if (a.sgd_master != nullptr) return launch_wgrad_sgd(a, d, stream);
   const int bn = a.block_n ? a.block_n : gemm_pick_block_n(a.M, a.N);
   const bool auto_quad = a.pair < 0 && a.block_n == 0 && pick_quad();
   const bool pair = a.pair < 0 ? (auto_quad || pick_pair(a.M)) : (a.pair != 0);

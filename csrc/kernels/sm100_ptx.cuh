@@ -457,8 +457,28 @@ __device__ __forceinline__ float tanh_fast(float x) {
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+// `bytes` (a multiple of 16) from a 16-byte aligned global address into L2, asynchronously
+__device__ __forceinline__ void prefetch_l2_bulk(const void* ptr, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(ptr), "r"(bytes) : "memory");
+}
 __device__ __forceinline__ void red_add_v2_f32(float* addr, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
+}
+
+// The SGD update of one element, shared by sgd_multi_kernel and the weight-gradient GEMM that
+// applies the update in its epilogue: d = g * grad_scale (* clip) + weight_decay * p, then
+// p - lr * d.  The roundings are spelled out (one multiply per scale, two FMAs) so that both
+// kernels compute the same bits whatever the compiler would contract around the call.
+// kScalars: the gradient is also multiplied by the clip coefficient (device OptimScalars).
+template <bool kScalars>
+__device__ __forceinline__ float sgd_direction(float g, float p, float grad_scale, float clip,
+                                               float weight_decay) {
+  float s = __fmul_rn(g, grad_scale);
+  if constexpr (kScalars) s = __fmul_rn(s, clip);
+  return __fmaf_rn(weight_decay, p, s);
+}
+__device__ __forceinline__ float sgd_apply(float p, float d, float lr) {
+  return __fmaf_rn(-lr, d, p);
 }
 
 // Counter-based RNG for dropout: splitmix64 of (seed, element-group index) -> 4 x 16-bit lanes.

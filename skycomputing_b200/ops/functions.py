@@ -59,6 +59,12 @@ class ParamBank:
         self.wgrad_target = False
         self.overwrite_first = False
         self.fresh = False
+        # encoder weight banks (SpanParams) may have the plain SGD update applied by the epilogue
+        # of their wgrad GEMM instead of by the optimizer (`update_in_wgrad_ok`); `wgrad_sgd` =
+        # (lr, weight_decay, grad_scale) while an engine arms the backward that produces the
+        # step's last gradient of the bank (EngineBase._arm_wgrad_sgd)
+        self.update_in_wgrad_ok = False
+        self.wgrad_sgd: Optional[tuple] = None
 
     def _materialise(self) -> None:
         p0 = self.params[0]
@@ -171,6 +177,9 @@ class SpanParams:
 
     def _bank(self, params, need_shadow: bool = True) -> ParamBank:
         b = ParamBank(params, need_shadow)
+        # the weights (the banks with a shadow): BertSpanFn.backward enqueues an armed wgrad
+        # behind the dgrad that reads the shadow it rewrites
+        b.update_in_wgrad_ok = need_shadow
         self.banks.append(b)
         return b
 
@@ -306,12 +315,13 @@ class BertSpanFn(torch.autograd.Function):
                                           rng_stream=sp.rng_base + 3, **wait)
             g2 = dz2d if dz2d is not None else dz2
             _ln_pgrad(dy2, sv["z2"], sv["mean2"], sv["rstd2"], sp.g2, sp.b2n, g2, sp.b2)
-            _wgrad(g2, sv["inter"], sp.w2, None)
             if sp.has_body:
-                d_h1 = nat.gemm(g2, sp.w2.shadow(), b_mn=True, aux=sv["h1"], act=nat.ACT_DGELU_MUL_AUX)
+                d_h1 = _wgrad_dgrad(g2, sv["inter"], sp.w2, None, lambda: nat.gemm(
+                    g2, sp.w2.shadow(), b_mn=True, aux=sv["h1"], act=nat.ACT_DGELU_MUL_AUX))
             else:
                 send = _grad_send_kwargs(in_ch, mb_in, which=0)
-                d_inter = nat.gemm(g2, sp.w2.shadow(), b_mn=True, **send)
+                d_inter = _wgrad_dgrad(g2, sv["inter"], sp.w2, None,
+                                       lambda: nat.gemm(g2, sp.w2.shadow(), b_mn=True, **send))
             d_a_extra = dz2
         elif sp.has_body:
             # span ends after Body: grads = (d_inter, d_attn_out)
@@ -323,10 +333,10 @@ class BertSpanFn(torch.autograd.Function):
             if sp.has_head and len(grads) > 1 and grads[1] is not None:
                 d_a_extra = _flat2d(grads[1]).contiguous()
         if sp.has_body:
-            _wgrad(d_h1, sv["a"], sp.w1, sp.b1)
             send = _grad_send_kwargs(in_ch, mb_in, which=0) if not sp.has_head else {}
-            d_a = nat.gemm(d_h1, sp.w1.shadow(), b_mn=True, aux=d_a_extra,
-                           add_aux=d_a_extra is not None, **send)
+            d_a = _wgrad_dgrad(d_h1, sv["a"], sp.w1, sp.b1, lambda: nat.gemm(
+                d_h1, sp.w1.shadow(), b_mn=True, aux=d_a_extra, add_aux=d_a_extra is not None,
+                **send))
         elif sp.has_tail:
             d_a = d_a_extra  # tail-only span: grad of the attn_out input is dz2
         else:
@@ -347,13 +357,13 @@ class BertSpanFn(torch.autograd.Function):
                                           rng_stream=sp.rng_base + 2, **wait)
             g1 = dz1d if dz1d is not None else dz1
             _ln_pgrad(dy1, sv["z1"], sv["mean1"], sv["rstd1"], sp.g1, sp.b1n, g1, sp.bo)
-            _wgrad(g1, sv["ctxt"], sp.wo, None)
-            dctx = nat.gemm(g1, sp.wo.shadow(), b_mn=True)
+            dctx = _wgrad_dgrad(g1, sv["ctxt"], sp.wo, None,
+                                lambda: nat.gemm(g1, sp.wo.shadow(), b_mn=True))
             dqkv = nat.attention_bwd(sv["qkv"], sv["mask2"], sv["ctxt"], sv["lse"], dctx, B, S,
                                      sp.heads, dropout_p=p_attn, rng=rng, rng_stream=sp.rng_base + 1)
-            _wgrad(dqkv, sv["x"], sp.wqkv, sp.bqkv)
             send = _grad_send_kwargs(in_ch, mb_in, which=0)
-            dx = nat.gemm(dqkv, sp.wqkv.shadow(), b_mn=True, aux=dz1, add_aux=True, **send)
+            dx = _wgrad_dgrad(dqkv, sv["x"], sp.wqkv, sp.bqkv, lambda: nat.gemm(
+                dqkv, sp.wqkv.shadow(), b_mn=True, aux=dz1, add_aux=True, **send))
             g_in[0] = None if dx is None else dx.view(B, S, H)
         elif sp.has_body:
             g_in[0] = None if d_a is None else d_a.view(B, S, H)
@@ -406,11 +416,19 @@ def _run_param_grad(item) -> None:
         nat.ln_param_grad(dy, z, mean, rstd, gbank.grad(), bbank.grad(), x2,
                           None if bias_bank is None else bias_bank.grad())
     else:
-        g, act, wbank, bbank = item
+        g, act, wbank, bbank, sgd = item
         wbank.wgrad_target = True
         first = wbank.overwrite_first and wbank.fresh
         wbank.fresh = False
-        nat.gemm(g, act, a_mn=True, b_mn=True, out=wbank.grad(), accumulate=not first)
+        if sgd is None:
+            nat.gemm(g, act, a_mn=True, b_mn=True, out=wbank.grad(), accumulate=not first)
+        else:
+            # the step's last gradient of the bank: the epilogue applies the SGD update to the
+            # master and its shadow and does not store the gradient
+            lr, weight_decay, grad_scale = sgd
+            nat.gemm(g, act, a_mn=True, b_mn=True, out=wbank.grad(), accumulate=not first,
+                     sgd_master=wbank.master(), sgd_shadow=wbank.shadow(), sgd_lr=lr,
+                     sgd_weight_decay=weight_decay, sgd_grad_scale=grad_scale)
         if bbank is not None:  # else: the column sum rides in the LayerNorm parameter-gradient kernel
             nat.colsum_(g, bbank.grad())
 
@@ -440,8 +458,10 @@ def pending_wgrads() -> int:
 def _wgrad(g: torch.Tensor, act: torch.Tensor, wbank: ParamBank,
            bbank: Optional[ParamBank]) -> None:
     """dW += g^T act (both operands MN-major over the token dimension), db += colsum(g) unless
-    ``bbank`` is None (the column sum then rides in the LayerNorm parameter-gradient kernel)."""
-    item = (g, act, wbank, bbank)
+    ``bbank`` is None (the column sum then rides in the LayerNorm parameter-gradient kernel).
+    An armed bank (``wbank.wgrad_sgd``) gets its SGD update in the same GEMM; the arming is read
+    here, so that a deferred gradient applies the update it was queued with."""
+    item = (g, act, wbank, bbank, wbank.wgrad_sgd)
     if _DEFER_WGRAD[0]:
         _WGRAD_QUEUE.append(item)
         return
@@ -453,6 +473,20 @@ def _wgrad(g: torch.Tensor, act: torch.Tensor, wbank: ParamBank,
         _WGRAD_KEEP.append((g, act))
         return
     _run_param_grad(item)
+
+
+def _wgrad_dgrad(g: torch.Tensor, act: torch.Tensor, wbank: ParamBank,
+                 bbank: Optional[ParamBank], dgrad):
+    """``_wgrad(g, act, wbank, bbank)`` and ``dgrad()``, the input-gradient GEMM that reads
+    ``wbank``'s shadow; returns what ``dgrad()`` returns.  The weight gradient is enqueued first,
+    so that on the side stream it overlaps the dgrad, unless it is armed: then it rewrites the
+    shadow and must fork after the dgrad has been enqueued."""
+    if wbank.wgrad_sgd is None:
+        _wgrad(g, act, wbank, bbank)
+        return dgrad()
+    out = dgrad()
+    _wgrad(g, act, wbank, bbank)
+    return out
 
 
 def _dummy_out(like: torch.Tensor) -> torch.Tensor:

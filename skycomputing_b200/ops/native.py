@@ -164,11 +164,21 @@ def gemm(
     stream_k: int = -1,
     max_ctas: int = 0,
     debug: int = 0,
+    sgd_master: Optional[torch.Tensor] = None,
+    sgd_shadow: Optional[torch.Tensor] = None,
+    sgd_lr: float = 0.0,
+    sgd_weight_decay: float = 0.0,
+    sgd_grad_scale: float = 1.0,
 ) -> Optional[torch.Tensor]:
     """out[M,N] = epilogue(sum_k A[m,k] B[n,k]) on the wgmma kernel.
 
     ``a``: [M,K] (or [K,M] when ``a_mn``); ``b``: [N,K] (or [K,N] when ``b_mn``), both bf16 with
     unit inner stride.  ``out_ptr``/``out_ld`` redirect the store to a raw (peer) pointer.
+
+    ``sgd_master`` (fp32) / ``sgd_shadow`` (bf16), laid out like the fp32 ``out`` of a weight
+    gradient (``a_mn`` and ``b_mn``): the gradient g (``out + g`` when ``accumulate``) is not
+    stored, the epilogue applies ``sgd_multi``'s plain update to the master and refreshes the
+    shadow (see GemmArgs::sgd_master in csrc/kernels/api.h).
     """
     _check(a, torch.bfloat16, "a")
     _check(b, torch.bfloat16, "b")
@@ -200,6 +210,14 @@ def gemm(
         _check(aux, torch.bfloat16, "aux")
     if out2 is not None:
         _check(out2, torch.bfloat16, "out2")
+    if sgd_master is not None:
+        if sgd_shadow is None:
+            raise ValueError("the SGD epilogue needs sgd_shadow")
+        _check(sgd_master, torch.float32, "sgd_master")
+        _check(sgd_shadow, torch.bfloat16, "sgd_shadow")
+        for t, what in ((sgd_master, "sgd_master"), (sgd_shadow, "sgd_shadow")):
+            if t.dim() != 2 or tuple(t.shape) != (M, N) or t.stride(0) != ldo:
+                raise ValueError(f"{what} must be [{M}, {N}] with the row stride of out")
     ext().gemm(
         A=a.data_ptr(), B=b.data_ptr(), M=M, N=N, K=K, lda=a.stride(0), ldb=b.stride(0),
         a_mn=a_mn, b_mn=b_mn, out=o_ptr, ldo=ldo, out_f32=out_f32, accumulate=accumulate,
@@ -208,7 +226,9 @@ def gemm(
         dropout_p=float(dropout_p), rng_state=0 if rng is None else rng.ptr,
         rng_stream=rng_stream, signal_flags=signal_flags, wait_flags=wait_flags,
         wait_epoch=wait_epoch, wait_mult=wait_mult, error_flag=error_flag, block_n=block_n, pair=pair, stream_k=stream_k,
-        max_ctas=max_ctas, debug=debug, stream=_stream(),
+        max_ctas=max_ctas, debug=debug, sgd_master=_ptr(sgd_master), sgd_shadow=_ptr(sgd_shadow),
+        sgd_lr=float(sgd_lr), sgd_weight_decay=float(sgd_weight_decay),
+        sgd_grad_scale=float(sgd_grad_scale), stream=_stream(),
     )
     return out
 

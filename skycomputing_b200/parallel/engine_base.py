@@ -19,6 +19,12 @@ that only feeds the optimizer (weight / bias / LayerNorm-parameter gradients) of
   forked at the producing kernel;
 * ``lazy`` / ``inline``: same queue flushed on the main stream / no deferral (debugging).
 
+When the optimizer's step is plain SGD (``FusedSGD`` without momentum, schedule or clipping), the
+encoder weight banks are not updated by the optimizer's pass at the end of the step: the wgrad
+GEMM that produces a bank's last gradient of the step applies the update in its epilogue (the
+backward of the last micro-batch of each local stage is "armed", ``_arm_wgrad_sgd``), and the
+optimizer's one launch covers the remaining banks.
+
 The side stream is forked from / joined to the main stream with events, which CUDA-graph capture
 records as parallel branches.  Reference context: scaelum/runner/runner.py:137 runs one monolithic
 ``dist_autograd.backward``; nothing there distinguishes the two kinds of gradient.
@@ -73,6 +79,10 @@ class EngineBase:
         self._wgrad_forked = False
         self._wgrad_keepalive: list = []
         self._wgrad_tslot: Optional[torch.Tensor] = None
+        # plain-SGD update in the weight-gradient GEMMs (_setup_wgrad_sgd): (lr, weight_decay,
+        # grad_scale), and the banks of every local stage it applies to
+        self._wgrad_sgd: Optional[tuple] = None
+        self._wgrad_sgd_banks: List[list] = [[] for _ in self.stages]
         # inline | lazy | lazy_stream | immediate | auto (see the module docstring)
         self._wgrad_mode = os.environ.get("SKY_WGRAD", "auto")
         self._wgrad_side_stream_enabled = False
@@ -114,6 +124,9 @@ class EngineBase:
             self.fused.close()
             self.fused = None
         self._release_wgrad_switches()
+        if self._wgrad_sgd is not None:
+            self.optimizer.set_update_in_wgrad([])   # step() updates every bank again
+            self._wgrad_sgd = None
 
     # ------------------------------------------------------------------ setup
     def _setup_batch_shape(self, inputs, src: Optional[int]) -> None:
@@ -393,6 +406,43 @@ class EngineBase:
             self._wgrad_stream = torch.cuda.Stream(device=self.device)
             self._wgrad_immediate = True
             set_wgrad_stream(self._wgrad_stream)
+        self._setup_wgrad_sgd()
+
+    def _setup_wgrad_sgd(self) -> None:
+        """Let the wgrad GEMMs of the encoder weight banks apply the optimizer's update when it is
+        plain SGD (``wgrad_sgd_args``): a bank then moves 10 B per parameter in that epilogue
+        (read and write the master, write the shadow) instead of 4 B there (the gradient) and
+        14 B in the optimizer's serial pass.  Other optimizers keep their step unchanged."""
+        args_of = getattr(self.optimizer, "wgrad_sgd_args", None)
+        args = args_of() if args_of is not None else None
+        if args is None:
+            return
+        from ..models.bert_layers import native_param_banks
+
+        owned = {id(b) for b in self.optimizer.banks}
+        per_stage = [[b for b in native_param_banks(st)
+                      if getattr(b, "update_in_wgrad_ok", False) and id(b) in owned]
+                     for st in self.stages]
+        if not any(per_stage):
+            return
+        self.optimizer.set_update_in_wgrad([b for banks in per_stage for b in banks])
+        self._wgrad_sgd = args
+        self._wgrad_sgd_banks = per_stage
+
+    @contextlib.contextmanager
+    def _arm_wgrad_sgd(self, stage_index: int, j: int):
+        """Around the backward of micro-batch ``j`` on local stage ``stage_index``: the last
+        micro-batch's backward produces the step's last gradient of every bank of the stage (no
+        forward of the stage follows it in the step), so its wgrad GEMMs apply the update; the
+        earlier ones accumulate as usual."""
+        banks = self._wgrad_sgd_banks[stage_index] if j == self.m - 1 else []
+        for b in banks:
+            b.wgrad_sgd = self._wgrad_sgd
+        try:
+            yield
+        finally:
+            for b in banks:
+                b.wgrad_sgd = None
 
     def _slowdown_factor(self) -> float:
         return max(float(getattr(st, "_slowdown", 0) or 0) for st in self.stages)

@@ -137,7 +137,11 @@ class FusedOptimizer:
         self._overwrite_ok = os.environ.get("SKY_SGD_OVERWRITE", "1") != "0"
         self._zeroing_decided = False
         self._desc_dev: Optional[torch.Tensor] = None
+        self._desc_count = 0
         self._max_numel = 0
+        # ids of the banks whose update an engine applies in their weight-gradient GEMMs
+        # (set_update_in_wgrad): the descriptor table leaves them out
+        self._in_wgrad: frozenset = frozenset()
         # device-side count of steps taken: Adam's bias correction and the learning-rate schedule
         self._step = torch.zeros(1, dtype=torch.int64, device=self._device) if counter else None
         self._step_offset = 0                     # schedule steps taken by an earlier optimizer
@@ -196,10 +200,10 @@ class FusedOptimizer:
                 d = self._descriptors()
                 if self._partials is None:
                     blocks = ext.grad_sumsq_blocks(self._max_numel)
-                    self._partials = torch.zeros(blocks * len(self.banks), dtype=torch.float32,
+                    self._partials = torch.zeros(blocks * self._desc_count, dtype=torch.float32,
                                                  device=self._device)
                     self._sumsq_blocks = blocks
-                ext.grad_sumsq_multi(d.data_ptr(), len(self.banks), self._sumsq_blocks,
+                ext.grad_sumsq_multi(d.data_ptr(), self._desc_count, self._sumsq_blocks,
                                      float(grad_scale), self._partials.data_ptr(), stream)
                 partials, n_part = self._partials.data_ptr(), self._partials.numel()
             if self._rest_opt is not None:
@@ -271,20 +275,42 @@ class FusedOptimizer:
         (``overwrite_first``).  Decided once, before the first descriptor or segment table."""
         if not self._zeroing_decided:
             for b in self.banks:
-                b.overwrite_first = bool(getattr(b, "wgrad_target", False)) and self._overwrite_ok
+                target = bool(getattr(b, "wgrad_target", False)) or id(b) in self._in_wgrad
+                b.overwrite_first = target and self._overwrite_ok
             self._zeroing_decided = True
 
-    def _descriptors(self) -> torch.Tensor:
-        """The SgdTensor table of the banks on the device, built once."""
+    def wgrad_sgd_args(self) -> Optional[tuple]:
+        """(lr, weight_decay, grad_scale) of the update that weight-gradient GEMMs may apply in
+        their epilogue when the engine's step is this optimizer's plain SGD update; None (the
+        default) when step() must see every gradient first."""
+        return None
+
+    def set_update_in_wgrad(self, banks: list) -> None:
+        """The engine applies the update of ``banks`` (a subset of ``self.banks``) in the last
+        weight-gradient GEMM of every step: step() leaves them out of its descriptor table, and
+        their gradients stay un-zeroed (the next step's first wgrad overwrites them).  ``[]``
+        hands every bank back to step()."""
+        ids = frozenset(id(b) for b in banks)
+        if ids != self._in_wgrad:
+            self._in_wgrad = ids
+            self._desc_dev = None
+            self._zeroing_decided = False
+
+    def _descriptors(self) -> Optional[torch.Tensor]:
+        """The SgdTensor table on the device of the banks step() updates (all of them but those
+        updated in their weight-gradient GEMMs), built once; None when there are none."""
         if self._desc_dev is None and self.banks:
             self._decide_zeroing()
             bufs = self._state_buffers()
             mom2 = bufs.get("second_moment", [None] * len(self.banks))
-            descs = [b.sgd_descriptor(m, v) for b, m, v in zip(self.banks, bufs["momentum"], mom2)]
-            raw = self._nat.ext().pack_sgd_descriptors(descs)
-            host = torch.frombuffer(bytearray(raw), dtype=torch.uint8)
-            self._desc_dev = host.to(self.banks[0].master().device)
-            self._max_numel = max(d[4] for d in descs)
+            descs = [b.sgd_descriptor(m, v) for b, m, v in zip(self.banks, bufs["momentum"], mom2)
+                     if id(b) not in self._in_wgrad]
+            self._desc_count = len(descs)
+            if descs:
+                raw = self._nat.ext().pack_sgd_descriptors(descs)
+                host = torch.frombuffer(bytearray(raw), dtype=torch.uint8)
+                self._desc_dev = host.to(self.banks[0].master().device)
+                self._max_numel = max(d[4] for d in descs)
         return self._desc_dev
 
     def step(self, grad_scale: float = 1.0) -> None:
@@ -358,10 +384,20 @@ class FusedSGD(FusedOptimizer):
     def _state_buffers(self) -> dict:
         return dict(momentum=self._mom)
 
+    def wgrad_sgd_args(self) -> Optional[tuple]:
+        """Plain SGD (no momentum, no schedule, no clipping) needs no gradient but a bank's own:
+        the update of a bank can ride in its last weight-gradient GEMM.  grad_scale is 1: the
+        engines step with it."""
+        if self.momentum != 0.0 or self._scalars is not None or not self._overwrite_ok:
+            return None
+        return (float(self.param_groups[0]["lr"]), float(self.weight_decay), 1.0)
+
     def _update(self, stream, grad_scale, scalars):
         d = self._descriptors()
+        if d is None:
+            return   # every bank is updated in its weight-gradient GEMMs
         self._nat.ext().sgd_multi(
-            d_tensors=d.data_ptr(), n=len(self.banks), max_numel=self._max_numel,
+            d_tensors=d.data_ptr(), n=self._desc_count, max_numel=self._max_numel,
             lr=float(self.param_groups[0]["lr"]), momentum=float(self.momentum),
             weight_decay=float(self.weight_decay), grad_scale=grad_scale, zero_grad=True,
             stream=stream, scalars=scalars)
@@ -393,7 +429,7 @@ class FusedAdam(FusedOptimizer):
     def _update(self, stream, grad_scale, scalars):
         d = self._descriptors()
         self._nat.ext().adam_multi(
-            d_tensors=d.data_ptr(), n=len(self.banks), max_numel=self._max_numel,
+            d_tensors=d.data_ptr(), n=self._desc_count, max_numel=self._max_numel,
             lr=float(self.param_groups[0]["lr"]), beta1=self.betas[0], beta2=self.betas[1],
             eps=float(self.eps), weight_decay=float(self.weight_decay),
             decoupled=bool(self.decoupled), step=self._step.data_ptr(), grad_scale=grad_scale,

@@ -164,13 +164,14 @@ class PipelineEngine(EngineBase):
         self._flush_wgrads()
         self._mark(("B", j, "begin"))
         st.begin_backward()
-        if self.is_last:
-            self._backward_from_loss(outs, loss)
-        elif self.out_fused:
-            dummy = outs[0]
-            torch.autograd.backward([dummy], [torch.zeros_like(dummy)])
-        else:
-            self._backward_from_grads(outs, grads)
+        with self._arm_wgrad_sgd(0, j):
+            if self.is_last:
+                self._backward_from_loss(outs, loss)
+            elif self.out_fused:
+                dummy = outs[0]
+                torch.autograd.backward([dummy], [torch.zeros_like(dummy)])
+            else:
+                self._backward_from_grads(outs, grads)
         st.end_backward()
         self._mark(("B", j, "end"))
         if self.is_first or self.in_fused:

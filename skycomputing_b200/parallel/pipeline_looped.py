@@ -156,10 +156,11 @@ class LoopedPipelineEngine(EngineBase):
                 self._flush_wgrads()
                 self._mark(("B", slot, "begin"))
                 st.begin_backward()
-                if last_stage:
-                    self._backward_from_loss(outs, loss)
-                else:
-                    torch.autograd.backward([outs[0]], [torch.zeros_like(outs[0])])
+                with self._arm_wgrad_sgd(c, j):
+                    if last_stage:
+                        self._backward_from_loss(outs, loss)
+                    else:
+                        torch.autograd.backward([outs[0]], [torch.zeros_like(outs[0])])
                 st.end_backward()
                 self._mark(("B", slot, "end"))
         self._flush_wgrads()
@@ -205,13 +206,14 @@ class LoopedPipelineEngine(EngineBase):
                 args, outs, loss = saved.pop((c, j))
                 self._flush_wgrads()
                 st.begin_backward()
-                if last_stage:
-                    self._backward_from_loss(outs, loss)
-                else:
-                    grads, reqs = self.comm.recv(self.next_rank, f"bwd{c}",
-                                                 metas=self._grad_metas(outs))
-                    self.comm.wait(reqs)
-                    self._backward_from_grads(outs, grads)
+                with self._arm_wgrad_sgd(c, j):
+                    if last_stage:
+                        self._backward_from_loss(outs, loss)
+                    else:
+                        grads, reqs = self.comm.recv(self.next_rank, f"bwd{c}",
+                                                     metas=self._grad_metas(outs))
+                        self.comm.wait(reqs)
+                        self._backward_from_grads(outs, grads)
                 st.end_backward()
                 if not first_stage:
                     self._pending_sends += self.comm.send(self._in_grads(args), self.prev_rank,
