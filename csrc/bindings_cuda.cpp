@@ -658,6 +658,24 @@ PYBIND11_MODULE(_cuda, m) {
                                        P<uint32_t>(flags), n_flags, inc, S(s)),
           "peer_copy_signal");
   });
+  m.def("tied_grad_push", [](uintptr_t src, uintptr_t dst, long long n, uintptr_t flag,
+                             uintptr_t done, uintptr_t s) {
+    check(sky::launch_tied_grad_push(P<const float>(src), P<float>(dst), n, P<uint32_t>(flag),
+                                     P<unsigned int>(done), S(s)),
+          "tied_grad_push");
+  }, py::arg("src"), py::arg("dst"), py::arg("n"), py::arg("flag"), py::arg("done"),
+     py::arg("stream") = 0);
+  m.def("tied_grad_reduce", [](uintptr_t g, uintptr_t inbox, uintptr_t peer_g, long long n,
+                               uintptr_t wait_flag, uintptr_t epoch, uintptr_t err,
+                               uintptr_t publish_flag, uintptr_t done, uintptr_t s) {
+    check(sky::launch_tied_grad_reduce(P<float>(g), P<const float>(inbox), P<float>(peer_g), n,
+                                       P<const uint32_t>(wait_flag), P<const uint32_t>(epoch),
+                                       P<int>(err), P<uint32_t>(publish_flag),
+                                       P<unsigned int>(done), S(s)),
+          "tied_grad_reduce");
+  }, py::arg("g"), py::arg("inbox"), py::arg("peer_g"), py::arg("n"), py::arg("wait_flag"),
+     py::arg("epoch"), py::arg("error_flag"), py::arg("publish_flag"), py::arg("done"),
+     py::arg("stream") = 0);
 
   m.def("ipc_alloc", &ipc_alloc);
   m.def("ipc_open", &ipc_open);

@@ -436,5 +436,17 @@ int launch_spin_factor(const uint64_t* t_start_slot, float factor, cudaStream_t 
 // (peer pointer) and bumps `n_flags` counters with release.sys.
 int launch_peer_copy_signal(const void* src, void* dst, long long nbytes, uint32_t* flags,
                             int n_flags, uint32_t inc, cudaStream_t stream);
+// Tied word-embedding gradient exchange between the first and the last pipeline rank (parallel/
+// p2p.py: TiedGradExchange).  push (last rank): dst[0:n] = src[0:n] with 16-byte peer stores, then
+// the last block to finish adds 1 to *flag (release.sys).  reduce (first rank): waits until
+// *wait_flag >= *epoch (acquire.sys; after 4 s *error_flag = 5 and the sum is skipped), then
+// s = g + inbox once per element, stored into g and peer_g, then the last block adds 1 to
+// *publish_flag.  `done`: a zeroed device counter private to the launching rank.  Pointers 16-byte
+// aligned (931); null pointers or n <= 0: 930.
+int launch_tied_grad_push(const float* src, float* dst, long long n, uint32_t* flag,
+                          unsigned int* done, cudaStream_t stream);
+int launch_tied_grad_reduce(float* g, const float* inbox, float* peer_g, long long n,
+                            const uint32_t* wait_flag, const uint32_t* epoch, int* error_flag,
+                            uint32_t* publish_flag, unsigned int* done, cudaStream_t stream);
 
 }  // namespace sky

@@ -1553,6 +1553,77 @@ peer_copy_signal_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, 
   }
 }
 
+// ---- tied word-embedding gradient exchange (parallel/p2p.py: TiedGradExchange) ------------------
+// After a block's stores: the last block of the grid to finish publishes `flag` (release.sys), so
+// a reader that acquires the flag sees every block's stores.  `done` is reset for the next launch.
+__device__ __forceinline__ void last_block_publish(uint32_t* flag, unsigned int* done) {
+  __threadfence_system();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const unsigned int prev = atomicAdd(done, 1u);
+    if (prev == gridDim.x - 1) {
+      *done = 0;
+      __threadfence_system();
+      red_release_sys_add(flag, 1u);
+    }
+  }
+}
+// Last rank: the replica's gradient -> the first rank's inbox (16-byte peer stores), then +1 on the
+// first rank's push flag.
+__global__ void __launch_bounds__(256)
+tied_grad_push_kernel(const float* __restrict__ src, float* __restrict__ dst, long long n,
+                      uint32_t* flag, unsigned int* done) {
+  const long long n4 = n >> 2;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  const long long t0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const float4* s4 = reinterpret_cast<const float4*>(src);
+  float4* d4 = reinterpret_cast<float4*>(dst);
+  for (long long i = t0; i < n4; i += stride) d4[i] = __ldcs(s4 + i);
+  for (long long i = (n4 << 2) + t0; i < n; i += stride) dst[i] = src[i];
+  last_block_publish(flag, done);
+}
+// First rank: wait until the push flag reaches *epoch (acquire.sys, 4 s timeout -> error 5), then
+// s = g + inbox ONCE per element, stored into g and through the peer pointer into the replica's
+// gradient, then +1 on the last rank's flag.  One writer of the sum: both copies bit-identical.
+__global__ void __launch_bounds__(256)
+tied_grad_reduce_kernel(float* __restrict__ g, const float* __restrict__ inbox,
+                        float* __restrict__ peer_g, long long n, const uint32_t* wait_flag,
+                        const uint32_t* epoch, int* error_flag, uint32_t* publish_flag,
+                        unsigned int* done) {
+  __shared__ int arrived;
+  if (threadIdx.x == 0) {
+    const uint32_t target = *epoch;
+    bool ok = ld_acquire_sys(wait_flag) >= target;
+    // after a timeout elsewhere in the step the run is failing: do not wait 4 s per block
+    if (!ok && !(error_flag && *reinterpret_cast<volatile int*>(error_flag) != 0))
+      ok = wait_flag_ge(wait_flag, target, kFlagTimeoutNs);
+    if (!ok && error_flag) atomicExch(error_flag, 5);
+    arrived = ok;
+  }
+  __syncthreads();
+  if (arrived) {
+    const long long n4 = n >> 2;
+    const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+    const long long t0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    float4* g4 = reinterpret_cast<float4*>(g);
+    const float4* in4 = reinterpret_cast<const float4*>(inbox);
+    float4* p4 = reinterpret_cast<float4*>(peer_g);
+    for (long long i = t0; i < n4; i += stride) {
+      const float4 a = g4[i];
+      const float4 b = __ldcs(in4 + i);
+      const float4 s = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+      g4[i] = s;
+      p4[i] = s;
+    }
+    for (long long i = (n4 << 2) + t0; i < n; i += stride) {
+      const float s = g[i] + inbox[i];
+      g[i] = s;
+      peer_g[i] = s;
+    }
+  }
+  last_block_publish(publish_flag, done);
+}
+
 // SMs of the current device (grid caps of the grid-stride kernels are multiples of it)
 inline int num_sms() {
   static int n = 0;
@@ -2046,6 +2117,30 @@ int launch_peer_copy_signal(const void* src, void* dst, long long nbytes, uint32
   peer_copy_signal_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
       reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), n16, flags, n_flags, inc,
       d_counter);
+  SKY_LAUNCH_CHECK();
+}
+
+static int tied_grid(long long n) {
+  long long blocks = ((n >> 2) + 255) / 256;
+  if (blocks > num_sms() * 4) blocks = num_sms() * 4;
+  return blocks < 1 ? 1 : static_cast<int>(blocks);
+}
+
+int launch_tied_grad_push(const float* src, float* dst, long long n, uint32_t* flag,
+                          unsigned int* done, cudaStream_t stream) {
+  if (!src || !dst || !flag || !done || n <= 0) return 930;
+  if (!aligned16(src) || !aligned16(dst)) return 931;
+  tied_grad_push_kernel<<<tied_grid(n), 256, 0, stream>>>(src, dst, n, flag, done);
+  SKY_LAUNCH_CHECK();
+}
+int launch_tied_grad_reduce(float* g, const float* inbox, float* peer_g, long long n,
+                            const uint32_t* wait_flag, const uint32_t* epoch, int* error_flag,
+                            uint32_t* publish_flag, unsigned int* done, cudaStream_t stream) {
+  if (!g || !inbox || !peer_g || !wait_flag || !epoch || !publish_flag || !done || n <= 0)
+    return 930;
+  if (!aligned16(g) || !aligned16(inbox) || !aligned16(peer_g)) return 931;
+  tied_grad_reduce_kernel<<<tied_grid(n), 256, 0, stream>>>(g, inbox, peer_g, n, wait_flag, epoch,
+                                                             error_flag, publish_flag, done);
   SKY_LAUNCH_CHECK();
 }
 

@@ -48,6 +48,9 @@ if TASK not in ("cls", "mlm"):
 # MLM_MAX_PREDICTIONS=P (TASK=mlm): the head decodes only the labelled positions, at most P per
 # sequence (P >= round(0.15 * (SEQ_LEN - 2)): 20 at 128 tokens); unset = every position decoded
 MLM_MAX_PREDICTIONS = int(os.getenv("MLM_MAX_PREDICTIONS")) if os.getenv("MLM_MAX_PREDICTIONS") else None
+# MLM_TIE=1 (TASK=mlm): the head's decoder weight is tied to the word-embedding table, as in BERT
+# (the two live on the first and the last pipeline stage; see README "Tied decoder")
+MLM_TIE = os.getenv("MLM_TIE", "0") == "1"
 
 # OPTIM=sgd|adam|adamw|lamb and LR: the optimizer (LAMB with BERT's weight-decay exclusion of
 # biases and LayerNorm parameters, skycomputing_b200.parallel.optim); unset = SGD, lr 0.001
@@ -81,6 +84,8 @@ if TASK == "mlm":
     _TAIL = [dict(layer_type="BertTailForMaskedLM", config=_config.__dict__)]
     if MLM_MAX_PREDICTIONS is not None:
         _TAIL[0]["max_predictions"] = MLM_MAX_PREDICTIONS
+    if MLM_TIE:
+        _TAIL[0]["tie_word_embeddings"] = True
 
 model_config = [dict(layer_type="BertEmbeddings", config=_config.__dict__)] + _ENCODER + _TAIL
 

@@ -169,6 +169,11 @@ class ModuleWrapper(nn.Module):
         # no labels and gets the dense logits
         self.labels = None
         children = list(module.children())
+        from ..models.bert_layers import tie_decoder_to_embeddings
+
+        # a tied masked-language-model decoder on the stage of the word embeddings shares their
+        # table (one Parameter); without the embeddings in front it stays a replica of it
+        tie_decoder_to_embeddings(children)
         for i, layer in enumerate(children[:-1]):
             if getattr(layer, "consumes_labels", False):
                 raise ValueError("{} (layer {} of {}) consumes labels and must be the model's "

@@ -11,6 +11,9 @@ Registered names and calling conventions are those of scaelum/model/bert_layers.
     BertTailForMaskedLM(config)       (hidden, mask)            -> logits [B, S, vocab]
     BertTailForMaskedLM(config, max_predictions=P)
                                       (hidden, mask, labels)    -> (logits [B*P, vocab], slot_labels [B*P])
+    BertTailForMaskedLM(config, tie_word_embeddings=True)
+                                      as above; decoder weight = the word-embedding table
+                                      (``tie_word_embeddings``, set up by the stage / engine)
 
 Parameter names match the reference (``attention.self.query.weight`` ...), so layer-indexed
 checkpoints interchange.  Every layer has two execution paths behind the same class:
@@ -205,6 +208,9 @@ class BertEmbeddings(nn.Module):
         self.token_type_embeddings = nn.Embedding(config.type_vocab_size, config.hidden_size)
         self.LayerNorm = BertLayerNorm(config.hidden_size, eps=1e-12)
         self.dropout = nn.Dropout(config.hidden_dropout_prob)
+        # the tied BertTailForMaskedLM of the same stage that decodes with this table (not a
+        # submodule), see tie_decoder_to_embeddings
+        object.__setattr__(self, "_tied_head", None)
         self._native = None
 
     def _native_params(self):
@@ -505,7 +511,14 @@ class BertTailForMaskedLM(nn.Module):
     then a decoder to vocabulary logits.  ``(hidden [B,S,H], mask) -> logits [B,S,V]``; every
     token is decoded unless ``max_predictions`` is set (below).
 
-    The decoder weight is a parameter of its own, not tied to the word embeddings.  The native
+    By default the decoder weight is a parameter of its own.  ``tie_word_embeddings=True`` ties
+    it to the word-embedding table of the model's first layer, as BERT, HF
+    ``BertForPreTraining`` and NVIDIA's recipe do (the decoder bias stays the head's own).  The head
+    still constructs its own ``decoder.weight``, so it can be built and benchmarked alone; whoever
+    assembles the model sets up the tie: a stage that holds both layers replaces the head's
+    Parameter by the table's (``tie_decoder_to_embeddings``, one Parameter and, on the GPU, one
+    parameter bank), and a pipeline whose head sits on another rank keeps a bit-identical replica
+    there (``parallel.engine_base``: both copies step on the summed gradient).  The native
     path needs ``H % 8 == 0`` and ``V % 8 == 0`` (GEMM output widths), which is why BERT configs
     pad the vocabulary (30522 -> 30528); other shapes run the eager path.
 
@@ -524,7 +537,8 @@ class BertTailForMaskedLM(nn.Module):
 
     MAX_PREDICTIONS_LIMIT = 8192   # csrc/kernels/api.h: kMlmMaxPredictions
 
-    def __init__(self, config, max_predictions=None, ignore_index: int = -100):
+    def __init__(self, config, max_predictions=None, ignore_index: int = -100,
+                 tie_word_embeddings: bool = False):
         super().__init__()
         config = BertConfig.from_dict(config) if isinstance(config, dict) else config
         bound = min(config.max_position_embeddings, self.MAX_PREDICTIONS_LIMIT)
@@ -539,7 +553,37 @@ class BertTailForMaskedLM(nn.Module):
         self.consumes_labels = max_predictions is not None
         self.transform = BertPredictionHeadTransform(config)
         self.decoder = nn.Linear(config.hidden_size, config.vocab_size)
+        self.tie_word_embeddings = bool(tie_word_embeddings)
+        if self.tie_word_embeddings:
+            # a replica (head on another stage) takes the table's weight-decay decisions
+            self.decoder.weight.tied_name = TIED_TABLE_NAME
+        # the BertEmbeddings of the same stage whose table this head's decoder shares (not a
+        # submodule: the table stays the embeddings' parameter); None for an untied head or a replica
+        object.__setattr__(self, "_tied_embeddings", None)
         self._native = None
+
+    @property
+    def is_replica(self) -> bool:
+        """Tied, but the table lives on another stage: ``decoder.weight`` is a copy of it."""
+        return self.tie_word_embeddings and self._tied_embeddings is None
+
+    def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
+        """A head tied to the table of its own stage does not load ``decoder.weight``: the shared
+        Parameter holds the embeddings' entry of the same file (loaded first, layer 0), which wins.
+        A file whose decoder weight differs (saved from an untied model) is reported once."""
+        key = "decoder.weight"
+        if self._tied_embeddings is None or key not in state_dict:
+            return super().load_state_dict(state_dict, strict=strict, assign=assign)
+        if not torch.equal(state_dict[key].to(self.decoder.weight.device, torch.float32),
+                           self.decoder.weight.detach().float()):
+            _warn_decoder_unused()
+        rest = {k: v for k, v in state_dict.items() if k != key}
+        res = super().load_state_dict(rest, strict=False, assign=assign)
+        missing = [k for k in res.missing_keys if k != key]
+        if strict and (missing or res.unexpected_keys):
+            raise RuntimeError("Error(s) in loading state_dict for {}: missing keys {}, unexpected "
+                               "keys {}".format(type(self).__name__, missing, res.unexpected_keys))
+        return res
 
     def _native_params(self):
         from ..ops.functions import MaskedLMHeadParams
@@ -577,6 +621,72 @@ class BertTailForMaskedLM(nn.Module):
         return self.decoder(self.transform(x)), slot_labels
 
 
+TIED_TABLE_NAME = "word_embeddings.weight"
+
+
+def _warn_decoder_unused() -> None:
+    import warnings
+
+    warnings.warn("the checkpoint's decoder.weight differs from its word_embeddings.weight (saved "
+                  "from an untied model): the tied decoder uses the word-embedding entry, the "
+                  "decoder entry is not used")
+
+
+def check_tied_layers(first, head) -> None:
+    """ValueError unless ``head`` (a tied BertTailForMaskedLM, or its layer config dict) can share
+    the table of ``first``, the model's first layer (module or config dict)."""
+    def shape(layer, kind):
+        if isinstance(layer, dict):
+            if layer.get("layer_type") != kind:
+                return None
+            c = layer.get("config")
+            c = BertConfig.from_dict(c) if isinstance(c, dict) else c
+            return (int(c.vocab_size), int(c.hidden_size))
+        if kind == "BertEmbeddings":
+            return tuple(layer.word_embeddings.weight.shape) if isinstance(layer, BertEmbeddings) else None
+        return (layer.decoder.out_features, layer.decoder.in_features)
+
+    table = shape(first, "BertEmbeddings")
+    if table is None:
+        got = first.get("layer_type") if isinstance(first, dict) else type(first).__name__
+        raise ValueError("tie_word_embeddings=True needs a BertEmbeddings as the model's first "
+                         "layer, got {}".format(got))
+    dec = shape(head, "BertTailForMaskedLM")
+    if dec != table:
+        raise ValueError("tie_word_embeddings=True: the decoder is [vocab, hidden] = {} but the "
+                         "word-embedding table is {}".format(list(dec), list(table)))
+
+
+def is_tied_head_cfg(layer_cfg: dict) -> bool:
+    return (layer_cfg.get("layer_type") == "BertTailForMaskedLM"
+            and bool(layer_cfg.get("tie_word_embeddings", False)))
+
+
+def tie_decoder_to_embeddings(layers) -> bool:
+    """Same-stage tie: when ``layers`` (one stage, in order) start with a BertEmbeddings and hold a
+    ``tie_word_embeddings`` head, the head's ``decoder.weight`` becomes the table's Parameter (the
+    same object; the decoder bias stays the head's).  A tied head without the embeddings in front
+    is left alone: it is a replica of a table on another stage.  Returns True when it tied."""
+    layers = list(layers)
+    heads = [l for l in layers if isinstance(l, BertTailForMaskedLM) and l.tie_word_embeddings]
+    if not heads or not isinstance(layers[0], BertEmbeddings):
+        return False
+    emb = layers[0]
+    for head in heads:
+        check_tied_layers(emb, head)
+        if head._tied_embeddings is emb:
+            continue
+        table = emb.word_embeddings.weight
+        table.tied_name = TIED_TABLE_NAME
+        head.decoder.weight = table
+        object.__setattr__(head, "_tied_embeddings", emb)
+        object.__setattr__(head, "_native", None)
+        object.__setattr__(emb, "_tied_head", head)
+        if emb._native is not None:
+            emb._native.tie_word_bank()
+    return True
+
+
 def native_param_banks(module: nn.Module):
     """All ParamBanks of `module`'s native layers (created eagerly; used by the fused optimizer).
 
@@ -612,4 +722,5 @@ def native_param_banks(module: nn.Module):
             banks.extend(_lone_span(m, body=m).params.banks)
         elif isinstance(m, BertLayer_Tail):
             banks.extend(_lone_span(m, tail=m).params.banks)
-    return banks
+    # a tied decoder's bank IS the embeddings' table bank: listed once, where the embeddings are
+    return list({id(b): b for b in banks}.values())

@@ -65,6 +65,11 @@ class ParamBank:
         # step's last gradient of the bank (EngineBase._arm_wgrad_sgd)
         self.update_in_wgrad_ok = False
         self.wgrad_sgd: Optional[tuple] = None
+        # the word-embedding table shared with a masked-language-model decoder on the same stage:
+        # it has two gradient writers (embed_bwd's atomics, the decoder wgrad's red.add, possibly
+        # on the side stream or deferred), so it is never `overwrite_first` and never updated
+        # inside a wgrad GEMM
+        self.tied = False
 
     def _materialise(self) -> None:
         p0 = self.params[0]
@@ -602,6 +607,8 @@ class EmbeddingsFn(torch.autograd.Function):
 class EmbeddingParams:
     def __init__(self, mod):
         self.word = ParamBank([mod.word_embeddings.weight], False)
+        if getattr(mod, "_tied_head", None) is not None:
+            self.tie_word_bank()
         self.pos = ParamBank([mod.position_embeddings.weight], False)
         self.type = ParamBank([mod.token_type_embeddings.weight], False)
         self.gamma = ParamBank([mod.LayerNorm.weight], False)
@@ -611,6 +618,13 @@ class EmbeddingParams:
         self.p_drop = float(mod.dropout.p)
         self.rng: Optional[nat.RngState] = None
         self.rng_base = 0
+
+    def tie_word_bank(self) -> None:
+        """The table is also the decoder weight of a tied head on this stage: the decoder GEMMs
+        read a bf16 shadow, which the fused optimizers keep fresh; the embedding kernels keep
+        reading the fp32 master."""
+        self.word.need_shadow = True
+        self.word.tied = True
 
     def all_params(self):
         return [p for b in self.banks for p in b.params]
@@ -758,7 +772,17 @@ class MaskedLMHeadParams:
         self.b_t = ParamBank([tr.dense_act.bias], False)
         self.gamma = ParamBank([tr.LayerNorm.weight], False)
         self.beta = ParamBank([tr.LayerNorm.bias], False)
-        self.w_dec = ParamBank([mod.decoder.weight])
+        emb = getattr(mod, "_tied_embeddings", None)
+        if emb is not None:
+            # one Parameter, one bank: a second bank around the table would re-materialise it
+            self.w_dec = emb._native_params().word
+            emb._native_params().tie_word_bank()
+        else:
+            # untied, or the replica of a table on another stage.  A replica is not `tied`: its
+            # gradient has one writer on this rank (the decoder wgrads, stream-ordered like any
+            # weight bank's), and the exchange of the summed gradient stores over it before the
+            # optimizer, so overwrite-first zeroing stays valid for it
+            self.w_dec = ParamBank([mod.decoder.weight])
         self.b_dec = ParamBank([mod.decoder.bias], False)
         self.banks = [self.w_t, self.b_t, self.gamma, self.beta, self.w_dec, self.b_dec]
         self.eps = float(tr.LayerNorm.eps)

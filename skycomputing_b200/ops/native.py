@@ -43,7 +43,7 @@ _KERNELS_PER_CALL = {
     "grad_sumsq_multi": 1, "optim_finalize": 1,
     "cast_f32_to_bf16": 1, "cast_bf16_to_f32": 1, "advance_counter": 1, "advance_epoch": 1,
     "signal_flags": 1, "wait_flags": 1, "spin_ns": 1, "record_time": 1, "spin_factor": 1,
-    "peer_copy_signal": 1,
+    "peer_copy_signal": 1, "tied_grad_push": 1, "tied_grad_reduce": 1,
 }
 _launches = [0]
 _counting_proxy = None

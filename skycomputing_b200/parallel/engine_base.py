@@ -96,6 +96,13 @@ class EngineBase:
         self._trace_tags: list = []
         self._trace_capacity = 0
         self._norm_exchange = None
+        # a word-embedding table tied to the decoder of a head on another rank (_setup_tie): the
+        # local copy (table on the first rank, replica on the last), the two-rank group, and the
+        # peer-memory exchange when the boundaries are fused
+        self._tied_param: Optional[torch.nn.Parameter] = None
+        self._tied_group = None
+        self._tied_src = 0
+        self._tied_exchange = None
 
     # the captured training step (None until it is captured), the native kernel launches of one
     # replay, and its static input / label buffers
@@ -120,6 +127,7 @@ class EngineBase:
             torch.cuda.synchronize(self.device)  # nothing of ours may still touch a peer region
         self._eval = None   # the evaluation graph is rebuilt by the next engine
         self._close_grad_norm()
+        self._close_tie()
         if self.fused is not None:
             self.fused.close()
             self.fused = None
@@ -268,6 +276,7 @@ class EngineBase:
         if pending and self._sends_before_optimizer():
             self.comm.wait(pending)
             pending.clear()
+        self._exchange_tied_grads()
         self.optimizer.step()
         self._mark(("OPT", 0, "end"))
         if pending:
@@ -373,14 +382,112 @@ class EngineBase:
 
     def _sends_before_optimizer(self) -> bool:
         """The optimizer's reduction of the norm must not overtake outstanding p2p sends (an NCCL
-        all_reduce behind them would dead-lock): engines with such sends wait for them first."""
-        return bool(getattr(self.optimizer, "needs_global_norm", False))
+        all_reduce behind them would dead-lock): engines with such sends wait for them first.
+        The same holds for the all_reduce of a tied table's gradient."""
+        return bool(getattr(self.optimizer, "needs_global_norm", False)) or \
+            (self._tied_group is not None and self._tied_exchange is None)
 
     def _close_grad_norm(self) -> None:
         if self._norm_exchange is not None:
             self._norm_exchange.close()
             self._norm_exchange = None
             self.optimizer.set_norm_reduction()
+
+    # ------------------------------------------------------------------ tied word embeddings
+    def _local_tied_params(self) -> tuple:
+        """(word table of this rank's first layer or None, replica head or None)."""
+        from ..models.bert_layers import BertEmbeddings, BertTailForMaskedLM
+
+        table = head = None
+        for st in self.stages:
+            layers = list(st.layers.children())
+            if layers and isinstance(layers[0], BertEmbeddings):
+                table = layers[0].word_embeddings.weight
+            for l in layers:
+                if isinstance(l, BertTailForMaskedLM) and l.is_replica:
+                    head = l
+        return table, head
+
+    def _setup_tie(self, first_rank: int, last_rank: int) -> None:
+        """A masked-language-model decoder tied to the word embeddings of another rank: its weight
+        is a replica of the first rank's table.  Here, in setup: the two-rank group {first, last}
+        (``new_group``: every rank calls it), the replica set equal to the table bit for bit, and
+        the per-step gradient sum (``_exchange_tied_grads``): a peer-memory exchange when the
+        boundaries are fused, one all_reduce over the group otherwise.  The replica's bank is left
+        out of this rank's share of the global gradient norm.  Collective."""
+        table, head = self._local_tied_params()
+        flags: list = [None] * dist.get_world_size(self.group)
+        dist.all_gather_object(flags, head is not None, group=self.group)
+        if not any(flags):
+            return
+
+        def glob(r):
+            return r if self.group is None else dist.get_global_rank(self.group, r)
+
+        self._tied_src = glob(first_rank)
+        self._tied_group = dist.new_group(sorted({glob(first_rank), glob(last_rank)}))
+        if self.is_first:
+            self._tied_param = table
+        elif self.is_last:
+            self._tied_param = head.decoder.weight
+        self.sync_tied_weights()
+        if self.is_last and hasattr(self.optimizer, "set_norm_exclude"):
+            self.optimizer.set_norm_exclude([self._tied_param])
+        if self.fused is not None and self._native_active():
+            from .p2p import TiedGradExchange
+
+            bank = None
+            if self.is_first:
+                bank = self.stages[0].layers[0]._native_params().word
+            elif self.is_last:
+                bank = head._native_params().w_dec
+            self._tied_exchange = TiedGradExchange(
+                bank, self.is_first, last_rank if self.is_first else first_rank, self.device,
+                self.fused.epoch_ptr, self.fused.error_ptr, group=self.group)
+            if bank is not None and hasattr(self.optimizer, "rebind_banks"):
+                self.optimizer.rebind_banks()
+
+    def sync_tied_weights(self) -> bool:
+        """Set the replica of a tied table equal to the table, bit for bit (in setup and after
+        every weight load).  Collective over the first and the last rank; returns True on the
+        replica's rank when the replica changed."""
+        if self._tied_param is None:
+            return False
+        p = self._tied_param
+        buf = p.detach().clone()
+        dist.broadcast(buf, src=self._tied_src, group=self._tied_group)
+        if self.is_first:
+            return False
+        changed = not torch.equal(buf, p.detach())
+        with torch.no_grad():
+            p.copy_(buf)   # bumps the version: the bf16 shadow is refreshed before its next read
+        return changed
+
+    def _exchange_tied_grads(self) -> None:
+        """Before the optimizer step (and so before its gradient norm): both copies of a tied
+        table get ``g_embeddings + g_decoder``."""
+        if self._tied_param is None:
+            return
+        ex = self._tied_exchange
+        if ex is not None:
+            if self.is_first:
+                ex.reduce()
+            else:
+                ex.push()
+                ex.wait()
+            return
+        p = self._tied_param
+        if p.grad is None:
+            p.grad = torch.zeros_like(p)
+        dist.all_reduce(p.grad, group=self._tied_group)   # two addends: identical on both ranks
+
+    def _close_tie(self) -> None:
+        if self._tied_exchange is not None:
+            self._tied_exchange.close()
+            self._tied_exchange = None
+            if hasattr(self.optimizer, "rebind_banks"):
+                self.optimizer.rebind_banks()
+        self._tied_param = None
 
     # ------------------------------------------------------------------ backend
     def _native_active(self) -> bool:
@@ -420,8 +527,10 @@ class EngineBase:
         from ..models.bert_layers import native_param_banks
 
         owned = {id(b) for b in self.optimizer.banks}
+        # a tied table has several gradient writers: it is never updated inside a wgrad GEMM
         per_stage = [[b for b in native_param_banks(st)
-                      if getattr(b, "update_in_wgrad_ok", False) and id(b) in owned]
+                      if getattr(b, "update_in_wgrad_ok", False) and id(b) in owned
+                      and not getattr(b, "tied", False)]
                      for st in self.stages]
         if not any(per_stage):
             return

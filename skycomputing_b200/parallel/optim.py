@@ -155,6 +155,12 @@ class FusedOptimizer:
         self._norm_allreduce = False
         self._norm_group = None
         self._norm_exchange = None
+        # banks / torch-path parameters left out of this rank's share of the squared norm: a tied
+        # table's replica, whose (identical) gradient the table's rank counts
+        self._norm_skip: frozenset = frozenset()
+        self._norm_desc: Optional[torch.Tensor] = None
+        self._norm_desc_count = 0
+        self._norm_max_numel = 0
         self._stepped = False
 
     @property
@@ -190,25 +196,61 @@ class FusedOptimizer:
         self._norm_allreduce = bool(allreduce) and exchange is None
         self._norm_group = group
 
+    def set_norm_exclude(self, params) -> None:
+        """Leave ``params`` (and the banks that hold them) out of this rank's share of the global
+        gradient norm: the replica of a tied table, counted on the table's rank."""
+        ids = frozenset(id(p) for p in params)
+        self._norm_skip = ids | frozenset(id(b) for b in self.banks
+                                          if any(id(p) in ids for p in b.params))
+        self._norm_desc = None
+        self._partials = None
+
+    def rebind_banks(self) -> None:
+        """A bank's buffers moved (a tied replica's gradient now lives in exchange memory):
+        rebuild the descriptor / segment tables on the next step.  Not inside a captured step."""
+        self._desc_dev = None
+        self._norm_desc = None
+        self._partials = None
+        if getattr(self, "_lamb", None) is not None:
+            self._lamb = None
+
+    def _norm_table(self):
+        """(descriptor table, count, max numel) of the banks whose gradients make up this rank's
+        share of the squared norm: the update table, or a table without the excluded banks."""
+        d = self._descriptors()
+        if not self._norm_skip:
+            return d, self._desc_count, self._max_numel
+        if self._norm_desc is None:
+            self._decide_zeroing()
+            descs = [b.sgd_descriptor() for b in self.banks
+                     if id(b) not in self._in_wgrad and id(b) not in self._norm_skip]
+            self._norm_desc_count = len(descs)
+            self._norm_max_numel = max((x[4] for x in descs), default=0)
+            if descs:
+                raw = self._nat.ext().pack_sgd_descriptors(descs)
+                host = torch.frombuffer(bytearray(raw), dtype=torch.uint8)
+                self._norm_desc = host.to(self._device)
+        return self._norm_desc, self._norm_desc_count, self._norm_max_numel
+
     def _compute_scalars(self, grad_scale: float, stream: int) -> None:
         """grad_sumsq_multi + optim_finalize: writes lr / clip_coef / grad_norm for this step,
         reading k from the step counter before step() advances it."""
         ext = self._nat.ext()
         partials, n_part, extra = 0, 0, 0
         if self._max_norm is not None:
-            if self.banks:
-                d = self._descriptors()
+            d, count, max_numel = self._norm_table() if self.banks else (None, 0, 0)
+            if count:
                 if self._partials is None:
-                    blocks = ext.grad_sumsq_blocks(self._max_numel)
-                    self._partials = torch.zeros(blocks * self._desc_count, dtype=torch.float32,
+                    blocks = ext.grad_sumsq_blocks(max_numel)
+                    self._partials = torch.zeros(blocks * count, dtype=torch.float32,
                                                  device=self._device)
                     self._sumsq_blocks = blocks
-                ext.grad_sumsq_multi(d.data_ptr(), self._desc_count, self._sumsq_blocks,
+                ext.grad_sumsq_multi(d.data_ptr(), count, self._sumsq_blocks,
                                      float(grad_scale), self._partials.data_ptr(), stream)
                 partials, n_part = self._partials.data_ptr(), self._partials.numel()
             if self._rest_opt is not None:
                 # torch fallback layers (eager anyway: such an optimizer is not graph-safe)
-                grads = self._rest_grads()
+                grads = self._rest_grads(counted_only=True)
                 self._rest_sumsq = (torch.stack([g.float().pow(2).sum() for g in grads]).sum()
                                     if grads else torch.zeros((), device=self._device)).reshape(1)
                 extra = self._rest_sumsq.data_ptr()
@@ -236,9 +278,9 @@ class FusedOptimizer:
         else:
             ext.optim_finalize(partials, n_part, extra, **common)
 
-    def _rest_grads(self) -> list:
+    def _rest_grads(self, counted_only: bool = False) -> list:
         return [p.grad for g in self._rest_opt.param_groups for p in g["params"]
-                if p.grad is not None]
+                if p.grad is not None and not (counted_only and id(p) in self._norm_skip)]
 
     def _rest_step(self) -> None:
         if self._scalars is not None:
@@ -276,7 +318,8 @@ class FusedOptimizer:
         if not self._zeroing_decided:
             for b in self.banks:
                 target = bool(getattr(b, "wgrad_target", False)) or id(b) in self._in_wgrad
-                b.overwrite_first = target and self._overwrite_ok
+                # a tied table has several gradient writers: always accumulate into zeros
+                b.overwrite_first = target and self._overwrite_ok and not getattr(b, "tied", False)
             self._zeroing_decided = True
 
     def wgrad_sgd_args(self) -> Optional[tuple]:
@@ -469,8 +512,11 @@ def check_lamb_cfg(cfg: dict) -> dict:
                 exclude_from_weight_decay=tuple(excl))
 
 
-def lamb_weight_decay(name: str, weight_decay: float, exclude) -> float:
-    """λ of the parameter called ``name``: 0 when the name contains one of ``exclude``."""
+def lamb_weight_decay(name: str, weight_decay: float, exclude, param=None) -> float:
+    """λ of the parameter called ``name``: 0 when the name contains one of ``exclude``.  A word
+    table tied to a decoder (``param.tied_name``) decides under that name, so that the table and
+    its replica on another rank cannot be treated differently."""
+    name = getattr(param, "tied_name", None) or name
     return 0.0 if any(s in name for s in exclude) else weight_decay
 
 
@@ -482,7 +528,7 @@ def lamb_param_groups(module: nn.Module, weight_decay: float, exclude, params=No
     for name, p in module.named_parameters():
         if not p.requires_grad or (keep is not None and id(p) not in keep):
             continue
-        wd = lamb_weight_decay(name, weight_decay, exclude)
+        wd = lamb_weight_decay(name, weight_decay, exclude, p)
         g = groups.setdefault(wd, dict(params=[], names=[], weight_decay=wd))
         g["params"].append(p)
         g["names"].append(name)
@@ -643,7 +689,7 @@ def lamb_segments(banks: list, names: dict, weight_decay: float, exclude) -> lis
         for p in b.params:
             off = (p.data_ptr() - flat.data_ptr()) // flat.element_size()
             name = names.get(id(p), f"<bank {i}>.{len(out)}")
-            wd = lamb_weight_decay(name, weight_decay, exclude)
+            wd = lamb_weight_decay(name, weight_decay, exclude, p)
             if p.numel() == 0:
                 continue
             out.append(dict(name=name, bank=i, offset=int(off), numel=p.numel(), weight_decay=wd,
@@ -669,6 +715,7 @@ class TorchOptimizerAdapter:
         self._norm_group = None
         self._last_lr: Optional[float] = None
         self._last_norm: Optional[torch.Tensor] = None
+        self._norm_skip: frozenset = frozenset()
 
     def configure(self, lr_schedule: Optional[dict] = None, max_norm: Optional[float] = None) -> None:
         """Learning-rate schedule (a LambdaLR stepped after every step()) and / or global-norm
@@ -685,13 +732,18 @@ class TorchOptimizerAdapter:
         self._norm_allreduce = bool(allreduce) or exchange is not None
         self._norm_group = group
 
+    def set_norm_exclude(self, params) -> None:
+        """See FusedOptimizer.set_norm_exclude: still clipped, not counted in the norm."""
+        self._norm_skip = frozenset(id(p) for p in params)
+
     def _clip(self) -> None:
         """torch.nn.utils.clip_grad_norm_ over every stage: local sum of squares, all_reduce of
         that one element, then the same coefficient on every rank."""
         params = [p for g in self.optimizer.param_groups for p in g["params"]]
         grads = [p.grad for p in params if p.grad is not None]
-        if grads:
-            sumsq = torch.stack([torch.linalg.vector_norm(g.detach(), 2.0) for g in grads]
+        counted = [p.grad for p in params if p.grad is not None and id(p) not in self._norm_skip]
+        if counted:
+            sumsq = torch.stack([torch.linalg.vector_norm(g.detach(), 2.0) for g in counted]
                                 ).float().pow(2).sum()
         else:
             sumsq = torch.zeros((), dtype=torch.float32, device=params[0].device)

@@ -365,3 +365,94 @@ class GradNormExchange:
         self._opened = []
         ext.dev_free(self.ptr)
         self.ptr = 0
+
+
+class TiedGradExchange:
+    """One summed gradient per step for a word-embedding table tied to a masked-language-model
+    decoder on another rank: the first rank holds the table, the last rank a replica.  Both must
+    step on ``g = g_embeddings + g_decoder``; then any optimizer keeps the copies bit-identical.
+    Runs inside the captured step (``tied_grad_push`` / ``tied_grad_reduce`` kernels, csrc/kernels/
+    elementwise_sm100.cu).
+
+    Each of the two ranks owns one region in its own HBM, mapped by the other: 256 bytes of words
+    (``[0]`` the inbound flag, ``[1]`` the done counter of the kernel this rank launches), then one
+    fp32 buffer of the table's size: on the first rank the INBOX, on the last rank the replica's
+    gradient itself (the bank's gradient is rebound to it, so the sum can be stored into it).
+
+    Per step: the last rank pushes its gradient into the inbox and bumps the first rank's flag; the
+    first rank, after its own backward, waits for that flag (>= epoch), computes the sum once,
+    stores it into its own gradient and into the replica's, and bumps the last rank's flag, which
+    the last rank waits for before its optimizer.  A timeout sets error 5 in the boundary manager's
+    error word.  The single inbox is safe to reuse: step k+1's push follows the last rank's wait
+    for step k's sum, which the first rank released only after it had read the inbox.  Collective:
+    every rank of ``group`` constructs it (``bank`` None on the others)."""
+
+    HEADER = 256
+
+    def __init__(self, bank, is_first: bool, peer_rank: Optional[int], device: torch.device,
+                 epoch_ptr: int, error_ptr: int, group=None):
+        ext = nat.ext()
+        self.bank, self.is_first, self.device = bank, is_first, device
+        self.epoch_ptr, self.error_ptr = epoch_ptr, error_ptr
+        self.ptr = self.peer_base = 0
+        self.buffer: Optional[torch.Tensor] = None
+        mine = {"rank": dist.get_rank(group), "gpu": None, "handle": None}
+        if bank is not None:
+            bank.ensure()
+            self.numel = bank.flat.numel()
+            nbytes = self.HEADER + ((self.numel * 4 + 255) // 256) * 256
+            self.ptr, handle = ext.ipc_alloc(nbytes)
+            tensor_from_ptr(self.ptr, (self.HEADER // 4,), torch.int32, device).zero_()
+            self.buffer = tensor_from_ptr(self.ptr + self.HEADER, tuple(bank.flat.shape),
+                                          torch.float32, device)
+            self.buffer.zero_()
+            if not is_first:
+                self.buffer.copy_(bank.flat_grad)
+                bank.flat_grad = self.buffer
+                bank._bind_grads()
+            mine.update(gpu=FusedBoundaryManager._gpu_uuid(device), handle=handle)
+        gathered: List[dict] = [None] * dist.get_world_size(group)  # type: ignore[list-item]
+        dist.all_gather_object(gathered, mine, group=group)
+        if bank is not None:
+            peer = {g["rank"]: g for g in gathered}[peer_rank]
+            ext.enable_peer_access(FusedBoundaryManager._local_device_of(peer["gpu"], peer_rank))
+            self.peer_base = ext.ipc_open(peer["handle"])
+        torch.cuda.synchronize(device)
+        dist.barrier(group=group)   # both regions are zeroed and mapped before either is written
+
+    def push(self) -> None:
+        """Last rank, once its weight gradients have joined."""
+        nat.ext().tied_grad_push(src=self.bank.grad().data_ptr(), dst=self.peer_base + self.HEADER,
+                                 n=self.numel, flag=self.peer_base, done=self.ptr + 4,
+                                 stream=torch.cuda.current_stream().cuda_stream)
+
+    def wait(self) -> None:
+        """Last rank, before its optimizer: the summed gradient has arrived."""
+        nat.ext().wait_flags(self.ptr, 1, self.epoch_ptr, 1, self.error_ptr,
+                             torch.cuda.current_stream().cuda_stream)
+
+    def reduce(self) -> None:
+        """First rank, after its last backward (embedding backward included) has joined."""
+        nat.ext().tied_grad_reduce(g=self.bank.grad().data_ptr(), inbox=self.ptr + self.HEADER,
+                                   peer_g=self.peer_base + self.HEADER, n=self.numel,
+                                   wait_flag=self.ptr, epoch=self.epoch_ptr,
+                                   error_flag=self.error_ptr, publish_flag=self.peer_base,
+                                   done=self.ptr + 4,
+                                   stream=torch.cuda.current_stream().cuda_stream)
+
+    def close(self) -> None:
+        """Hands the replica its own gradient memory again (not zeroed), then unmaps and frees."""
+        if not self.ptr:
+            return
+        ext = nat.ext()
+        torch.cuda.synchronize(self.device)
+        if not self.is_first and self.bank.flat_grad is self.buffer:
+            self.bank.flat_grad = self.buffer.clone()
+            self.bank._bind_grads()
+        try:
+            ext.ipc_close(self.peer_base)
+        except Exception:
+            pass
+        self.buffer = None
+        ext.dev_free(self.ptr)
+        self.ptr = self.peer_base = 0

@@ -112,6 +112,7 @@ class PipelineEngine(EngineBase):
 
                 self.comm = TorchDistComm(self.device, group=self.group)
             self._setup_grad_norm(self.s, self.P, self.stage_to_rank, [f[4] for f in flags])
+            self._setup_tie(self.stage_to_rank[0], self.stage_to_rank[-1])
         self._setup_graphable(self._native_active() and (self.is_first or self.in_fused) and
                               (self.is_last or self.out_fused))
         self._configure_wgrad(multi)

@@ -114,6 +114,7 @@ class LoopedPipelineEngine(EngineBase):
             self._comm = TorchDistComm(self.device, group=self.group, directional=True)
         # one optimizer over all local chunks (optim_module): one share of the norm per position
         self._setup_grad_norm(self.pos, self.P, self.ring, [f[2] for f in flags])
+        self._setup_tie(self.ring[0], self.ring[self.P - 1])
         self._setup_done = True
 
     def _step_body(self, inputs, labels) -> None:
@@ -224,6 +225,7 @@ class LoopedPipelineEngine(EngineBase):
         if self._sends_before_optimizer():
             self.comm.wait(self._pending_sends)
             self._pending_sends = []
+        self._exchange_tied_grads()
         self.optimizer.step()
         self.comm.wait(self._pending_sends)
         self._pending_sends = []

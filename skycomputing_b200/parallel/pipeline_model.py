@@ -113,6 +113,7 @@ class RpcModel(nn.Module):
         k // D of worker k % D, so a rank owns v LocalModules."""
         model = nn.ModuleList()
         pool = list(self.worker_manager.worker_pool)
+        self.tied_word_embeddings = self._check_tie(pool)
         D = len(pool)
         single = D == 1
         v = max((len(w.chunks) for w in pool if getattr(w, "chunks", None)), default=1)
@@ -148,7 +149,29 @@ class RpcModel(nn.Module):
                                       sequential_wrapper_cfg=cfg, device_rank=dev,
                                       layer_range=layer_range)
             model.append(module)
+        if self.tied_word_embeddings:
+            from ..models.bert_layers import TIED_TABLE_NAME, BertEmbeddings
+
+            # the table's weight-decay decisions are taken under the same name on every rank that
+            # holds a copy of it (here, before any optimizer is built, even when the head is remote)
+            if model[0].is_local and isinstance(model[0].module.layers[0], BertEmbeddings):
+                model[0].module.layers[0].word_embeddings.weight.tied_name = TIED_TABLE_NAME
         return model
+
+    @staticmethod
+    def _check_tie(pool) -> bool:
+        """Is the decoder of a masked-language-model head tied to the word embeddings?  Validated
+        here, where the whole model's layer list is known: ValueError when the model's first layer
+        is not a BertEmbeddings or the vocabulary / hidden sizes differ."""
+        from ..models.bert_layers import check_tied_layers, is_tied_head_cfg
+
+        heads = [c for w in pool for c in (w.model_config or []) if is_tied_head_cfg(c)]
+        if not heads:
+            return False
+        first_cfg = pool[0].model_config[0] if pool and pool[0].model_config else {}
+        for h in heads:
+            check_tied_layers(first_cfg, h)
+        return True
 
     # ---- topology -------------------------------------------------------------------------
     @property

@@ -53,6 +53,7 @@ class CheckpointHook(Hook):
         for key, val in sd.items():
             idx, name = key.split(".", 1)
             per_layer.setdefault(int(idx), OrderedDict())[name] = val
+        self._tie_rule(runner, per_layer, self._load_checkpoint_from)
         for module in runner.model.model:
             if not module.is_local:
                 continue
@@ -63,6 +64,9 @@ class CheckpointHook(Hook):
             # layers without parameters / buffers (ReLU, Flatten, Dropout-only ...) have no keys in
             # the file: they load an empty state dict, as in the reference's ParameterServer path
             module.load_weights([per_layer.get(i, OrderedDict()) for i in range(b, e)])
+        engine = getattr(runner, "engine", None)
+        if engine is not None and hasattr(engine, "sync_tied_weights"):
+            engine.sync_tied_weights()   # an engine that is already set up: replica := table
         if runner.is_rank0:
             runner.parameter_server.load_weights_from_file(self._load_checkpoint_from)
         extra = self._extra_path(self._load_checkpoint_from, runner.rank)
@@ -82,6 +86,37 @@ class CheckpointHook(Hook):
                     runner._log(msg)
             runner.iter = st.get("iter", runner.iter)
             runner.epoch = st.get("epoch", runner.epoch)
+
+    @staticmethod
+    def _tie_rule(runner, per_layer: dict, path: str) -> None:
+        """A decoder tied to the word embeddings takes the file's ``word_embeddings.weight`` entry
+        (layer 0), whichever stage it is on: its own ``decoder.weight`` entry is replaced by it.
+        The file keeps both entries, so tied and untied checkpoints interchange; a file saved from
+        an untied model (the entries differ) is reported once."""
+        from ...models.bert_layers import BertTailForMaskedLM
+
+        table = per_layer.get(0, {}).get("word_embeddings.weight")
+        if table is None:
+            return
+        for module in runner.model.model:
+            if not module.is_local:
+                continue
+            b = module.layer_range[0] if module.layer_range is not None else 0
+            for off, layer in enumerate(module.module.layers.children()):
+                if not (isinstance(layer, BertTailForMaskedLM) and layer.tie_word_embeddings):
+                    continue
+                sd = per_layer.get(b + off)
+                if sd is None or "decoder.weight" not in sd:
+                    continue
+                if not torch.equal(sd["decoder.weight"].float(), table.float()):
+                    msg = ("CheckpointHook: {} was saved from an untied model: the tied decoder "
+                           "uses its word_embeddings.weight, its decoder.weight is not used"
+                           .format(path))
+                    import warnings
+
+                    warnings.warn(msg)
+                    runner._log(msg)
+                sd["decoder.weight"] = table
 
     # ------------------------------------------------------------------ save
     @staticmethod

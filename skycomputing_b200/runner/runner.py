@@ -467,6 +467,11 @@ class Runner:
         if fused is None or self._iter % every != 0:
             return
         code = fused.error_code()
+        if code == 5:
+            raise RuntimeError(
+                f"rank {self.rank}: the tied word-embedding gradient of the last stage did not "
+                f"arrive within 4 s (error flag 5) at iteration {self._iter}: the last stage "
+                "stopped producing - check its log")
         if code:
             raise RuntimeError(
                 f"rank {self.rank}: fused stage-boundary wait timed out (error flag {code}) at "

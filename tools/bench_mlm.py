@@ -20,10 +20,18 @@ warm-up) is reported, and the mlm_gather / mlm_scatter kernels are timed against
 floors at the benchmark's geometry with the dataset's 15 % labelling (graph replays: the
 wrappers' host time exceeds these kernels' device time).
 Kernel times are CUDA-event means over 50 launches after 5 warm-up launches.
+
+    python tools/bench_mlm.py --tie [--steps 20] [--rounds 5] [--max-predictions P]
+
+compares the decoder tied to the word embeddings (``tie_word_embeddings=True``) with the untied
+head instead, at the same geometry: SGD (momentum 0.9) and LAMB, dense and sparse head (P = 20
+unless given), each pair in alternating windows.  Per arm: ms/step (median), peak memory from its
+construction through its warm-up, parameter count and native kernel launches per step.
 """
 from __future__ import annotations
 
 import argparse
+import gc
 import json
 import os
 import statistics
@@ -49,7 +57,8 @@ def card() -> dict:
     return dict(name=name, power_limit=power, max_sm_clock=clock)
 
 
-def build_runner(layers: int, mlm: bool, max_predictions=None):
+def build_runner(layers: int, mlm: bool, max_predictions=None, tie: bool = False,
+                 optim: str = "SGD"):
     cfg = sky.BertConfig.bert_large()
     if mlm:
         cfg.vocab_size = V
@@ -59,6 +68,8 @@ def build_runner(layers: int, mlm: bool, max_predictions=None):
     head = dict(layer_type="BertTailForMaskedLM", config=cfg.__dict__)
     if max_predictions is not None:
         head["max_predictions"] = max_predictions
+    if tie:
+        head["tie_word_embeddings"] = True
     tail = ([head] if mlm else
             [dict(layer_type="BertPooler", config=cfg.__dict__),
              dict(layer_type="BertTailForClassification", hidden_dropout_prob=0.1,
@@ -72,7 +83,9 @@ def build_runner(layers: int, mlm: bool, max_predictions=None):
     wm = sky.Allocator(mc, wm, granularity="block").allocate("even")
     torch.manual_seed(0)
     model = sky.RpcModel(wm, this_rank=0)
-    opt = sky.build_optimizer(model.optim_module, dict(optim_type="SGD", lr=1e-4, momentum=0.9))
+    optim_cfg = (dict(optim_type="SGD", lr=1e-4, momentum=0.9) if optim == "SGD" else
+                 dict(optim_type=optim, lr=1e-4))
+    opt = sky.build_optimizer(model.optim_module, optim_cfg)
     runner = sky.Runner(model=model, parameter_server=None, worker_manager=wm, optimizer=opt,
                         max_epochs=1, max_iters=1, device=torch.device("cuda", 0),
                         loss_cfg=dict(type="MaskedLMLoss" if mlm else "CrossEntropyLoss"),
@@ -161,6 +174,52 @@ def slot_kernels(P: int) -> dict:
     return out
 
 
+def tie_compare(args) -> dict:
+    """Tied against untied decoder: SGD / LAMB x dense / sparse head, alternating windows."""
+    P = args.max_predictions or 20
+    nat.enable_launch_counter()
+    out = {}
+    for optim in ("SGD", "LAMB"):
+        for head in ("dense", "sparse"):
+            arms, peak, params, launches = {}, {}, {}, {}
+            for arm in ("untied", "tied"):
+                torch.cuda.synchronize()
+                base = torch.cuda.memory_allocated()
+                torch.cuda.reset_peak_memory_stats()
+                arms[arm] = build_runner(args.layers, True, P if head == "sparse" else None,
+                                         tie=arm == "tied", optim=optim)
+                runner, inputs, labels = arms[arm]
+                for _ in range(args.warmup):
+                    runner.engine.train_step(inputs, labels)
+                torch.cuda.synchronize()
+                assert runner.engine._graph is not None, arm
+                peak[arm] = (torch.cuda.max_memory_allocated() - base) / 2 ** 20
+                params[arm] = sum(p.numel() for p in runner.model.local_stage.parameters())
+                launches[arm] = runner.engine.launches_per_step
+            times = {arm: [] for arm in arms}
+            for _ in range(args.rounds):
+                for arm, (runner, inputs, labels) in arms.items():
+                    times[arm].append(step_window(runner, inputs, labels, args.steps))
+            for runner, _, _ in arms.values():
+                runner.engine.close()
+            # nothing of this pair may stay alive into the next pair's memory baseline
+            del arms, runner, inputs, labels
+            gc.collect()
+            torch.cuda.empty_cache()
+            key = "{}_{}".format(optim.lower(), head)
+            out[key] = {arm: dict(median_ms=statistics.median(times[arm]), windows_ms=times[arm],
+                                  peak_mib=peak[arm], params=params[arm],
+                                  launches_per_step=launches[arm]) for arm in times}
+            u, t = out[key]["untied"], out[key]["tied"]
+            print("{} {}{}: untied {:.3f} ms, tied {:.3f} ms ({:+.3f} ms); peak MiB {:.0f} -> {:.0f}; "
+                  "params {:.2f} M -> {:.2f} M; launches/step {} -> {}".format(
+                      optim, head, " (P = {})".format(P) if head == "sparse" else "",
+                      u["median_ms"], t["median_ms"], t["median_ms"] - u["median_ms"],
+                      u["peak_mib"], t["peak_mib"], u["params"] / 1e6, t["params"] / 1e6,
+                      u["launches_per_step"], t["launches_per_step"]), flush=True)
+    return out
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
@@ -169,6 +228,7 @@ def main() -> None:
     ap.add_argument("--layers", type=int, default=24)
     ap.add_argument("--max-predictions", type=int, default=None)
     ap.add_argument("--out", type=str, default=None)
+    ap.add_argument("--tie", action="store_true")
     args = ap.parse_args()
     if not (torch.cuda.is_available() and nat.available()):
         raise SystemExit("bench_mlm needs a GPU and the native extension")
@@ -177,6 +237,14 @@ def main() -> None:
     res = dict(card=card())
     print("card: {name}, power limit {power_limit}, max SM clock {max_sm_clock}".format(**res["card"]),
           flush=True)
+    if args.tie:
+        res["tie"] = tie_compare(args)
+        line = json.dumps(res)
+        print(line)
+        if args.out:
+            with open(args.out, "w") as f:
+                f.write(line + "\n")
+        return
 
     # --- whole steps, alternating windows ---
     P = args.max_predictions

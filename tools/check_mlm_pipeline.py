@@ -10,6 +10,15 @@ pipelines cut at different places can be compared (dropout off => the same math 
     --max-predictions P
                    the sparse head: only the labelled positions (at most P per sequence) are
                    decoded; the labels reach the head on the last stage
+    --virtual-stages v
+                   a looped pipeline (v chunks per rank on a ring; fused ring by default,
+                   torch.distributed p2p with --boundary nccl): the head sits in the last chunk of
+                   the last rank
+    --max-grad-norm x
+                   global-norm gradient clipping (the norm is printed per step: ``grad_norms``)
+    --tie          the decoder weight is tied to the word embeddings: on 2+ GPUs the last stage
+                   holds a replica of the first stage's table; the checksum of both copies is
+                   printed for every step (``tied_checksums``: [first rank's, last rank's])
 """
 import argparse
 import json
@@ -34,6 +43,10 @@ def main():
     ap.add_argument("--steps", type=int, default=6)
     ap.add_argument("--batch", type=int, default=16)
     ap.add_argument("--max-predictions", type=int, default=None)
+    ap.add_argument("--tie", action="store_true")
+    ap.add_argument("--optim", default="SGD")
+    ap.add_argument("--virtual-stages", type=int, default=1)
+    ap.add_argument("--max-grad-norm", type=float, default=None)
     a = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -52,6 +65,8 @@ def main():
     head = dict(layer_type="BertTailForMaskedLM", config=cfg.__dict__)
     if a.max_predictions is not None:
         head["max_predictions"] = a.max_predictions
+    if a.tie:
+        head["tie_word_embeddings"] = True
     model_config = [dict(layer_type="BertEmbeddings", config=cfg.__dict__)] + enc + [head]
     workers = [dict(name=f"gpu-{i}", server_config={}, device=i,
                     extra_config=dict(module_to_cuda=True, cuda_device=local, slowdown=0,
@@ -59,7 +74,10 @@ def main():
                for i in range(world)]
     wm = sky.WorkerManager(first_rank=0)
     wm.load_worker_pool_from_config(workers)
-    if a.cut == "blocks" or world == 1:
+    if a.virtual_stages > 1 and world > 1:
+        wm = sky.Allocator(model_config, wm, granularity="block").allocate(
+            "even", virtual_stages=a.virtual_stages)
+    elif a.cut == "blocks" or world == 1:
         wm = sky.Allocator(model_config, wm, granularity="block").allocate("even")
     else:
         # every layer but the head on the first world - 1 stages, the head alone on the last
@@ -76,13 +94,20 @@ def main():
         b0 = mod.layer_range[0]
         for off, layer in enumerate(mod.module.layers.children()):
             g = torch.Generator(device="cpu").manual_seed(1000 + b0 + off)
+            # a tied decoder is the table (one GPU) or its replica, synchronised by the engine
+            skip = {id(layer.decoder.weight)} if getattr(layer, "tie_word_embeddings", False) else set()
             with torch.no_grad():
                 for p in layer.parameters():
+                    if id(p) in skip:
+                        continue
                     p.copy_((torch.randn(p.shape, generator=g) * 0.02).to(p.device))
                 for n_, p in layer.named_parameters():
                     if n_.endswith("LayerNorm.weight"):
                         p.fill_(1.0)
-    opt = sky.build_optimizer(model.optim_module, dict(optim_type="SGD", lr=0.01))
+    lr = 0.01 if a.optim == "SGD" else 1e-3
+    opt = sky.build_optimizer(model.optim_module, dict(optim_type=a.optim, lr=lr),
+                              grad_clip=(dict(max_norm=a.max_grad_norm)
+                                         if a.max_grad_norm is not None else None))
     runner = sky.Runner(model=model, parameter_server=None, worker_manager=wm, optimizer=opt,
                         max_epochs=1, max_iters=10 ** 9, loss_cfg=dict(type="MaskedLMLoss"),
                         timer_cfg=dict(root="/tmp/sky_check_mlm"), logging_cfg=None,
@@ -91,20 +116,34 @@ def main():
     model.train(True)
     ds = sky.SynthMLMDataset(num_samples=a.batch * 2, max_seq_length=128, vocab_size=30528, seed=3)
     batches = list(torch.utils.data.DataLoader(ds, batch_size=a.batch))
-    losses = []
+    losses, checksums, norms = [], [], []
+    eng = runner.engine
     for step in range(a.steps):
         data, labels = batches[step % 2]
         out = runner.train_iteration(data, labels)
         if out is not None:
             losses.append(out)
+        if a.max_grad_norm is not None:
+            norms.append(opt.scalars()["grad_norm"])
+        if a.tie:
+            # the bits of this rank's copy of the table (table on the first rank, replica on the
+            # last): equal checksums on both ranks every step
+            table, head_mod = eng._local_tied_params()
+            copy = head_mod.decoder.weight if (head_mod is not None and not eng.is_first) else table
+            checksums.append(None if copy is None else
+                             int(copy.detach().view(torch.int32).to(torch.int64).sum()))
     torch.cuda.synchronize()
-    eng = runner.engine
+    looped = getattr(model, "virtual_stages", 1) > 1
     info = dict(cut=a.cut, world=world, fused=(eng.in_fused or eng.out_fused),
                 layers=[len(w.model_config) for w in wm.worker_pool],
-                last_stage_first_layer=model_config[
+                last_stage_first_layer=None if looped else model_config[
                     max(w.layer_range for w in wm.worker_pool)[0]]["layer_type"],
+                engine=type(eng).__name__, grad_norms=norms,
                 graph=eng._graph is not None, losses=losses,
-                err=eng.fused.error_code() if eng.fused is not None else 0)
+                err=eng.fused.error_code() if eng.fused is not None else 0,
+                first=eng.is_first, checksums=checksums,
+                tied_exchange=("peer" if eng._tied_exchange is not None else
+                               "all_reduce" if eng._tied_group is not None else None))
     gathered = [None] * world
     dist.all_gather_object(gathered, info)
     if rank == 0:
@@ -112,6 +151,10 @@ def main():
         last["fused_any"] = any(g["fused"] for g in gathered)
         last["graph_all"] = all(g["graph"] for g in gathered)
         last["err_any"] = max(g["err"] for g in gathered)
+        if a.tie:
+            first = [g for g in gathered if g["first"]][0]
+            last["tied_checksums"] = [first["checksums"], last["checksums"]]
+            last["tied_exchange"] = first["tied_exchange"]
         print("CHECK " + json.dumps(last), flush=True)
     eng.close()
     dist.destroy_process_group()

@@ -10,6 +10,8 @@
 #                  wait_flags, flag-gated GEMM) on one GPU
 #         mlm      the sparse masked-language-model slot kernels (mlm_gather / mlm_scatter) over
 #                  the shape grid, and one graph replayed with different label counts
+#         tied     the tied word-embedding gradient exchange (tied_grad_push / tied_grad_reduce)
+#                  in loopback on one GPU, and the tied masked-language-model head
 #         all      everything above (default)
 # Runs on ONE GPU; reports land in bench_out/sanitizer_<tool>_<suite>.log.  The sanitizer slows
 # kernels 10-100x: the 4 s flag-wait timeouts are only meaningful under memcheck / synccheck.
@@ -36,6 +38,9 @@ case "$SUITE" in attn|all)
 esac
 case "$SUITE" in mlm|all)
   run mlm tests/test_mlm_sparse_gpu.py -k "gather_and_scatter or different_label_counts" ;;
+esac
+case "$SUITE" in tied|all)
+  run tied tests/test_mlm_tied_gpu.py -k "loopback or reject_bad_arguments or matches_eager" ;;
 esac
 case "$SUITE" in layers|all)
   run layers tests/test_layers_gpu.py tests/test_kernels_gpu.py -k "embeddings_pooler_classifier or handshake or signals_panels" ;;
