@@ -304,10 +304,22 @@ void mlm_gather(uintptr_t hidden, uintptr_t labels, int B, int seq, int H, int m
         "mlm_gather");
 }
 void mlm_scatter(uintptr_t dx_c, uintptr_t slot_of_row, long long rows, int H, uintptr_t dhidden,
-                 uintptr_t stream) {
+                 uintptr_t stream, uintptr_t dcls, int seq) {
   check(sky::launch_mlm_scatter(P<const void>(dx_c), P<const int>(slot_of_row), rows, H,
-                                P<void>(dhidden), S(stream)),
+                                P<void>(dhidden), S(stream), P<const void>(dcls), seq),
         "mlm_scatter");
+}
+void cls_grad_add(uintptr_t dhidden, uintptr_t dcls, int B, int seq, int H, uintptr_t stream) {
+  check(sky::launch_cls_grad_add(P<void>(dhidden), P<const void>(dcls), B, seq, H, S(stream)),
+        "cls_grad_add");
+}
+void masked_softmax_ce(uintptr_t logits, int ldl, uintptr_t labels, int M, int C,
+                       long long ignore_index, uintptr_t dlogits, float grad_scale, uintptr_t loss,
+                       uintptr_t loss_acc, uintptr_t stream) {
+  check(sky::launch_masked_softmax_ce(P<const float>(logits), ldl, P<const int64_t>(labels), M, C,
+                                      ignore_index, P<float>(dlogits), grad_scale, P<float>(loss),
+                                      P<float>(loss_acc), S(stream)),
+        "masked_softmax_ce");
 }
 
 // descriptors: list of (p, g, mom, p_bf16, numel) -> packed host bytes to upload once
@@ -594,7 +606,14 @@ PYBIND11_MODULE(_cuda, m) {
         py::arg("S"), py::arg("H"), py::arg("P"), py::arg("ignore_index"), py::arg("V"),
         py::arg("slot_of_row"), py::arg("slot_labels"), py::arg("x_c"), py::arg("stream") = 0);
   m.def("mlm_scatter", &mlm_scatter, py::arg("dx_c"), py::arg("slot_of_row"), py::arg("rows"),
-        py::arg("H"), py::arg("dhidden"), py::arg("stream") = 0);
+        py::arg("H"), py::arg("dhidden"), py::arg("stream") = 0, py::arg("dcls") = 0,
+        py::arg("S") = 1);
+  m.def("cls_grad_add", &cls_grad_add, py::arg("dhidden"), py::arg("dcls"), py::arg("B"),
+        py::arg("S"), py::arg("H"), py::arg("stream") = 0);
+  m.def("masked_softmax_ce", &masked_softmax_ce, py::arg("logits"), py::arg("ldl"),
+        py::arg("labels"), py::arg("M"), py::arg("C"), py::arg("ignore_index"), py::arg("dlogits"),
+        py::arg("grad_scale") = 1.f, py::arg("loss") = 0, py::arg("loss_acc") = 0,
+        py::arg("stream") = 0);
   m.def("mlm_max_predictions", []() { return sky::kMlmMaxPredictions; });
   m.def("pack_sgd_descriptors", &pack_sgd_descriptors);
   m.def("sgd_multi", &sgd_multi, py::arg("d_tensors"), py::arg("n"), py::arg("max_numel"),

@@ -305,8 +305,26 @@ constexpr int kMlmMaxPredictions = 8192;  // slot map of one sequence in shared 
 int launch_mlm_gather(const void* hidden, const int64_t* labels, int B, int S, int H, int P,
                       long long ignore_index, int V, int* slot_of_row, int64_t* slot_labels,
                       void* x_c, cudaStream_t stream);
+// With dcls ([rows / S, H] bf16, 16-byte aligned; S divides rows) row b*S, the [CLS] position of
+// sequence b, gets dcls[b] added (each lane rounded once from fp32; dcls[b] exactly when the row
+// is not decoded): the pooler branch's input gradient joins the head's in the same pass.
 int launch_mlm_scatter(const void* dx_c, const int* slot_of_row, long long rows, int H,
-                       void* dhidden, cudaStream_t stream);
+                       void* dhidden, cudaStream_t stream, const void* dcls = nullptr, int S = 1);
+// cls_grad_add (one launch): dhidden[b*S] += dcls[b] in place (bf16 [B*S, H] and [B, H], lanes
+// rounded once from fp32), the dense head's [CLS]-row join.  Errors: 982 bad shape (B, S >= 1, H a
+// positive multiple of 8), 983 null pointer, 984 a buffer is not 16-byte aligned.
+int launch_cls_grad_add(void* dhidden, const void* dcls, int B, int S, int H, cudaStream_t stream);
+
+// Cross entropy over fp32 logits [M, C] (row stride ldl) with ignore_index, the next-sentence-
+// prediction loss.  n_valid = rows whose label is in [0, C).  dlogits [M, C] (contiguous) =
+// (softmax - onehot) * grad_scale / n_valid on those rows and an exact 0 on every other row.
+// loss[0] = mean over the n_valid rows (0 when n_valid == 0), NaN when any label is neither
+// ignore_index nor in [0, C) (such a label is never used as an index); loss_acc[0] += loss *
+// grad_scale.  loss / loss_acc may be null.  One CTA, fixed-order fp64 reduction, no host sync,
+// graph-capturable.  Errors: 985 bad shape (M < 0, C < 1, ldl < C), 986 null pointer.
+int launch_masked_softmax_ce(const float* logits, int ldl, const int64_t* labels, int M, int C,
+                             long long ignore_index, float* dlogits, float grad_scale,
+                             float* loss, float* loss_acc, cudaStream_t stream);
 
 // ---------------------------------------------------------------------------------------------
 // Optimizer / parameter maintenance

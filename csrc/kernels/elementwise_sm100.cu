@@ -1051,16 +1051,120 @@ mlm_gather_kernel(const uint4* __restrict__ hidden, const int64_t* __restrict__ 
   }
 }
 
+// 8 bf16 lanes of a + b, each sum rounded once from fp32
+__device__ __forceinline__ uint4 bf16x8_add(uint4 a, uint4 b) {
+  const __nv_bfloat162* pa = reinterpret_cast<const __nv_bfloat162*>(&a);
+  const __nv_bfloat162* pb = reinterpret_cast<const __nv_bfloat162*>(&b);
+  uint4 out;
+  __nv_bfloat162* po = reinterpret_cast<__nv_bfloat162*>(&out);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 fa = __bfloat1622float2(pa[j]), fb = __bfloat1622float2(pb[j]);
+    po[j] = __floats2bfloat162_rn(fa.x + fb.x, fa.y + fb.y);
+  }
+  return out;
+}
+
+// kCls: row b*S (a sequence's [CLS] position) also gets dcls[b], the pooler's input gradient, so
+// that the input gradient of a head with a pooler branch is written once
+template <bool kCls>
 __global__ void __launch_bounds__(kMlmThreads)
 mlm_scatter_kernel(const uint4* __restrict__ dx_c, const int* __restrict__ slot_of_row,
-                   long long rows, int H8, uint4* __restrict__ dhidden) {
+                   long long rows, int H8, uint4* __restrict__ dhidden,
+                   const uint4* __restrict__ dcls, int S) {
   const long long total = rows * H8;
   const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const long long r = i / H8;
     const int s = slot_of_row[r];
-    dhidden[i] = s >= 0 ? dx_c[static_cast<long long>(s) * H8 + (i - r * H8)] : zero;
+    uint4 v = s >= 0 ? dx_c[static_cast<long long>(s) * H8 + (i - r * H8)] : zero;
+    if (kCls && r % S == 0) {
+      const uint4 c = dcls[(r / S) * H8 + (i - r * H8)];
+      v = s >= 0 ? bf16x8_add(v, c) : c;
+    }
+    dhidden[i] = v;
+  }
+}
+
+// dhidden[b*S] += dcls[b] in place: the dense head's [CLS]-row join
+__global__ void __launch_bounds__(kMlmThreads)
+cls_grad_add_kernel(uint4* __restrict__ dhidden, const uint4* __restrict__ dcls, int B, int S,
+                    int H8) {
+  const long long total = static_cast<long long>(B) * H8;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long b = i / H8;
+    uint4* p = dhidden + b * S * H8 + (i - b * H8);
+    *p = bf16x8_add(*p, dcls[i]);
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// Cross entropy over a few classes with ignore_index (the next-sentence-prediction loss).  One
+// CTA: pass 1 counts the labelled rows (label != ignore_index) and the invalid ones (outside
+// [0, C)), pass 2 writes every gradient row and the row losses, which are summed in a fixed fp64
+// tree.  An invalid label is never dereferenced: its row gradient is 0 and the loss NaN.  No
+// float atomics, no host sync: graph replays are bit-identical.
+// ------------------------------------------------------------------------------------------
+constexpr int kMaskedCeThreads = 256;
+
+__global__ void __launch_bounds__(kMaskedCeThreads)
+masked_softmax_ce_kernel(const float* __restrict__ logits, int ldl,
+                         const int64_t* __restrict__ labels, int M, int C, long long ignore_index,
+                         float* __restrict__ dlogits, float grad_scale, float* __restrict__ loss,
+                         float* __restrict__ loss_acc) {
+  __shared__ double red[kMaskedCeThreads];
+  __shared__ int cnt[kMaskedCeThreads], bad[kMaskedCeThreads];
+  const int tid = threadIdx.x;
+  int n = 0, nbad = 0;
+  for (int m = tid; m < M; m += kMaskedCeThreads) {
+    const long long lab = labels[m];
+    if (lab != ignore_index) {
+      if (lab < 0 || lab >= C) ++nbad;
+      else ++n;
+    }
+  }
+  cnt[tid] = n;
+  bad[tid] = nbad;
+  __syncthreads();
+  for (int s = kMaskedCeThreads / 2; s > 0; s >>= 1) {
+    if (tid < s) {
+      cnt[tid] += cnt[tid + s];
+      bad[tid] += bad[tid + s];
+    }
+    __syncthreads();
+  }
+  const int n_valid = cnt[0];
+  const float gscale = n_valid > 0 ? grad_scale / static_cast<float>(n_valid) : 0.f;
+  double local = 0.0;
+  for (int m = tid; m < M; m += kMaskedCeThreads) {
+    const float* l = logits + static_cast<long long>(m) * ldl;
+    float* d = dlogits + static_cast<long long>(m) * C;
+    const long long lab = labels[m];
+    if (lab == ignore_index || lab < 0 || lab >= C) {
+      for (int c = 0; c < C; ++c) d[c] = 0.f;
+      continue;
+    }
+    float mx = -INFINITY;
+    for (int c = 0; c < C; ++c) mx = fmaxf(mx, l[c]);
+    float se = 0.f;
+    for (int c = 0; c < C; ++c) se += expf(l[c] - mx);
+    const float lse = mx + logf(se);
+    local += static_cast<double>(lse - l[lab]);
+    for (int c = 0; c < C; ++c) d[c] = (expf(l[c] - lse) - (c == lab ? 1.f : 0.f)) * gscale;
+  }
+  red[tid] = local;
+  __syncthreads();
+  for (int s = kMaskedCeThreads / 2; s > 0; s >>= 1) {
+    if (tid < s) red[tid] += red[tid + s];
+    __syncthreads();
+  }
+  if (tid == 0) {
+    float mean = n_valid > 0 ? static_cast<float>(red[0] / n_valid) : 0.f;
+    if (bad[0] > 0) mean = __int_as_float(0x7fc00000);  // NaN: an invalid label is never silent
+    if (loss != nullptr) loss[0] = mean;
+    if (loss_acc != nullptr) loss_acc[0] += mean * grad_scale;
   }
 }
 
@@ -1900,15 +2004,47 @@ int launch_mlm_gather(const void* hidden, const int64_t* labels, int B, int S, i
 }
 
 int launch_mlm_scatter(const void* dx_c, const int* slot_of_row, long long rows, int H,
-                       void* dhidden, cudaStream_t stream) {
+                       void* dhidden, cudaStream_t stream, const void* dcls, int S) {
   if (rows < 1 || H < 8 || H % 8 != 0) return 960;
   if (!dx_c || !slot_of_row || !dhidden) return 961;
   if (!aligned16(dx_c) || !aligned16(dhidden)) return 962;
+  if (dcls != nullptr && (S < 1 || rows % S != 0)) return 960;
+  if (dcls != nullptr && !aligned16(dcls)) return 962;
   const long long vec = rows * (H / 8);
   long long blocks = (vec + kMlmThreads - 1) / kMlmThreads;
   if (blocks > num_sms() * 8LL) blocks = num_sms() * 8LL;
-  mlm_scatter_kernel<<<static_cast<unsigned>(blocks), kMlmThreads, 0, stream>>>(
-      static_cast<const uint4*>(dx_c), slot_of_row, rows, H / 8, static_cast<uint4*>(dhidden));
+  if (dcls == nullptr) {
+    mlm_scatter_kernel<false><<<static_cast<unsigned>(blocks), kMlmThreads, 0, stream>>>(
+        static_cast<const uint4*>(dx_c), slot_of_row, rows, H / 8, static_cast<uint4*>(dhidden),
+        nullptr, 1);
+  } else {
+    mlm_scatter_kernel<true><<<static_cast<unsigned>(blocks), kMlmThreads, 0, stream>>>(
+        static_cast<const uint4*>(dx_c), slot_of_row, rows, H / 8, static_cast<uint4*>(dhidden),
+        static_cast<const uint4*>(dcls), S);
+  }
+  SKY_LAUNCH_CHECK();
+}
+
+int launch_cls_grad_add(void* dhidden, const void* dcls, int B, int S, int H,
+                        cudaStream_t stream) {
+  if (B < 1 || S < 1 || H < 8 || H % 8 != 0) return 982;
+  if (!dhidden || !dcls) return 983;
+  if (!aligned16(dhidden) || !aligned16(dcls)) return 984;
+  const long long vec = static_cast<long long>(B) * (H / 8);
+  long long blocks = (vec + kMlmThreads - 1) / kMlmThreads;
+  if (blocks > num_sms() * 8LL) blocks = num_sms() * 8LL;
+  cls_grad_add_kernel<<<static_cast<unsigned>(blocks), kMlmThreads, 0, stream>>>(
+      static_cast<uint4*>(dhidden), static_cast<const uint4*>(dcls), B, S, H / 8);
+  SKY_LAUNCH_CHECK();
+}
+
+int launch_masked_softmax_ce(const float* logits, int ldl, const int64_t* labels, int M, int C,
+                             long long ignore_index, float* dlogits, float grad_scale,
+                             float* loss, float* loss_acc, cudaStream_t stream) {
+  if (M < 0 || C < 1 || ldl < C) return 985;
+  if (M > 0 && (!logits || !labels || !dlogits)) return 986;
+  masked_softmax_ce_kernel<<<1, kMaskedCeThreads, 0, stream>>>(
+      logits, ldl, labels, M, C, ignore_index, dlogits, grad_scale, loss, loss_acc);
   SKY_LAUNCH_CHECK();
 }
 

@@ -41,14 +41,22 @@ EVAL_SAMPLES = int(os.getenv("EVAL_SAMPLES", "256"))
 TINY = os.getenv("TINY", "0") == "1"                          # shrink the geometry for CPU smoke runs
 # TASK=mlm: masked-language-model pretraining (RoBERTa style, no next-sentence head) on the
 # learnable SynthMLMDataset with a BertTailForMaskedLM head and MaskedLMLoss; the vocabulary is
-# padded to a multiple of 8 (30522 -> 30528) for the head's GEMMs.  Default: classification
+# padded to a multiple of 8 (30522 -> 30528) for the head's GEMMs.  TASK=pretrain: BERT's masked-LM
+# + next-sentence pretraining on SynthPretrainingDataset with a BertTailForPreTraining head and
+# PreTrainingLoss (same vocabulary padding).  Default: classification
 TASK = os.getenv("TASK", "cls")
-if TASK not in ("cls", "mlm"):
-    raise ValueError("TASK must be 'cls' or 'mlm', got {!r}".format(TASK))
-# MLM_MAX_PREDICTIONS=P (TASK=mlm): the head decodes only the labelled positions, at most P per
+if TASK not in ("cls", "mlm", "pretrain"):
+    raise ValueError("TASK must be 'cls', 'mlm' or 'pretrain', got {!r}".format(TASK))
+# SAVE_PATH=dir: save a checkpoint into dir after every epoch; INIT_FROM=path: initialise the
+# weights from a checkpoint of a pretraining run (TASK=mlm or pretrain), e.g. to fine-tune
+# TASK=cls from it: the encoder (and the pooler of a pretraining head) load, the rest keeps its
+# initialisation (the vocabulary is padded as the pretraining run padded it)
+SAVE_PATH = os.getenv("SAVE_PATH")
+INIT_FROM = os.getenv("INIT_FROM")
+# MLM_MAX_PREDICTIONS=P (TASK=mlm or pretrain): the head decodes only the labelled positions, at most P per
 # sequence (P >= round(0.15 * (SEQ_LEN - 2)): 20 at 128 tokens); unset = every position decoded
 MLM_MAX_PREDICTIONS = int(os.getenv("MLM_MAX_PREDICTIONS")) if os.getenv("MLM_MAX_PREDICTIONS") else None
-# MLM_TIE=1 (TASK=mlm): the head's decoder weight is tied to the word-embedding table, as in BERT
+# MLM_TIE=1 (TASK=mlm or pretrain): the head's decoder weight is tied to the word-embedding table, as in BERT
 # (the two live on the first and the last pipeline stage; see README "Tied decoder")
 MLM_TIE = os.getenv("MLM_TIE", "0") == "1"
 
@@ -65,7 +73,9 @@ if TINY:
     _config = BertConfig(1000, hidden_size=64, num_hidden_layers=LAYER_NUM, num_attention_heads=4,
                          intermediate_size=128, max_position_embeddings=128)
 _SEQ = int(os.getenv("SEQ_LEN", "128" if not TINY else "16"))
-if TASK == "mlm":
+if TASK in ("mlm", "pretrain") or INIT_FROM:
+    # the masked-LM heads' GEMMs need a multiple of 8; a model initialised from such a run has
+    # to match its padded word-embedding table
     _config.vocab_size = (_config.vocab_size + 7) // 8 * 8
 
 _ENCODER = [
@@ -80,8 +90,9 @@ _TAIL = [
          hidden_dropout_prob=_config.hidden_dropout_prob,
          hidden_size=_config.hidden_size, num_classes=3),
 ]
-if TASK == "mlm":
-    _TAIL = [dict(layer_type="BertTailForMaskedLM", config=_config.__dict__)]
+if TASK in ("mlm", "pretrain"):
+    _TAIL = [dict(layer_type="BertTailForMaskedLM" if TASK == "mlm" else "BertTailForPreTraining",
+                  config=_config.__dict__)]
     if MLM_MAX_PREDICTIONS is not None:
         _TAIL[0]["max_predictions"] = MLM_MAX_PREDICTIONS
     if MLM_TIE:
@@ -119,12 +130,13 @@ data_config = dict(
                      max_seq_length=_SEQ, vocab_size=_config.vocab_size, num_classes=3, seed=0),
     dataloader_cfg=dict(batch_size=BATCH_SIZE, shuffle=True, num_workers=0, drop_last=True),
 )
-if TASK == "mlm":
-    data_config["dataset_cfg"] = dict(type="SynthMLMDataset", num_samples=BATCH_SIZE * (MAX_ITERS + 2),
+if TASK in ("mlm", "pretrain"):
+    _DATA = "SynthMLMDataset" if TASK == "mlm" else "SynthPretrainingDataset"
+    data_config["dataset_cfg"] = dict(type=_DATA, num_samples=BATCH_SIZE * (MAX_ITERS + 2),
                                       max_seq_length=_SEQ, vocab_size=_config.vocab_size, seed=0)
     if EVAL_EVERY is not None:  # the held-out split: another seed of the same task
         data_config["eval_datasets"] = dict(
-            dev=dict(type="SynthMLMDataset", num_samples=EVAL_SAMPLES, max_seq_length=_SEQ,
+            dev=dict(type=_DATA, num_samples=EVAL_SAMPLES, max_seq_length=_SEQ,
                      vocab_size=_config.vocab_size, seed=1))
 elif EVAL_EVERY is not None:
     # a learnable task (label = first token after [CLS] mod 3) for training and the held-out split,
@@ -168,13 +180,16 @@ train_config = dict(
     lr_schedule_cfg=(dict(type=LR_SCHEDULE, warmup_steps=WARMUP_STEPS, total_steps=TOTAL_STEPS)
                      if LR_SCHEDULE else None),
     grad_clip_cfg=dict(max_norm=MAX_GRAD_NORM) if MAX_GRAD_NORM is not None else None,
-    loss_cfg=dict(type="MaskedLMLoss" if TASK == "mlm" else "CrossEntropyLoss"),
+    loss_cfg=dict(type=dict(mlm="MaskedLMLoss", pretrain="PreTrainingLoss").get(TASK, "CrossEntropyLoss")),
     runner_cfg=dict(max_epochs=1, max_iters=MAX_ITERS, micro_batches=MICRO_BATCHES),
     hook_config=[dict(type="StopHook", root=_LOG_ROOT), dict(type="DistributedTimerHelperHook")]
     # REALLOCATE_EVERY=N: re-benchmark the devices and re-run the allocator every N iterations,
     # migrating layers when the predicted bottleneck improves (needs ALLOCATE_TYPE dynamic|optimal)
     + ([dict(type="ReallocateHook", interval=int(os.getenv("REALLOCATE_EVERY")))]
-       if os.getenv("REALLOCATE_EVERY") else []),
+       if os.getenv("REALLOCATE_EVERY") else [])
+    + ([dict(type="CheckpointHook", save_path=SAVE_PATH, save_interval=1)] if SAVE_PATH else [])
+    + ([dict(type="CheckpointHook", load_checkpoint_from=INIT_FROM, from_pretraining=True)]
+       if INIT_FROM else []),
     timer_config=dict(root=_LOG_ROOT),
 )
 if EVAL_EVERY is not None:

@@ -1,7 +1,8 @@
-from .bert_dataset import GlueDataset, MaskedLMDataset
+from .bert_dataset import GlueDataset, MaskedLMDataset, PreTrainingDataset
 from .data_generator import BaseGenerator, DataloaderGenerator, RandomTensorGenerator
 from .dataset import (CIFAR10Dataset, RandomImageDataset, RandomMlpDataset, SynthMLMDataset,
-                      SynthMNLIDataset)
+                      SynthMNLIDataset, SynthPretrainingDataset)
 
 __all__ = ["GlueDataset", "BaseGenerator", "DataloaderGenerator", "RandomTensorGenerator",
-           "CIFAR10Dataset", "RandomImageDataset", "RandomMlpDataset", "SynthMNLIDataset", "SynthMLMDataset", "MaskedLMDataset"]
+           "CIFAR10Dataset", "RandomImageDataset", "RandomMlpDataset", "SynthMNLIDataset", "SynthMLMDataset", "MaskedLMDataset",
+           "SynthPretrainingDataset", "PreTrainingDataset"]

@@ -1,4 +1,4 @@
-"""GlueDataset and MaskedLMDataset.
+"""GlueDataset, MaskedLMDataset and PreTrainingDataset.
 
 GlueDataset: tokenises a local GLUE split (``train.tsv`` by default) and caches the features.
 
@@ -18,7 +18,7 @@ import torch
 from torch.utils.data import Dataset, TensorDataset
 
 from ..registry import DATASET
-from .dataset import _item_generator, bert_mask
+from .dataset import _item_generator, bert_mask, pretraining_item
 from .glue import PROCESSORS, BertTokenizer, convert_examples_to_features
 
 
@@ -122,3 +122,86 @@ class MaskedLMDataset(Dataset):
         if self.reference_order:
             return (ids, mask, self.segment_ids[idx]), labels
         return (ids, self.segment_ids[idx], mask), labels
+
+
+@DATASET.register_module
+class PreTrainingDataset(Dataset):
+    """Masked-LM + next-sentence data from a local text file in the input format of BERT's
+    ``create_pretraining_data``: one sentence per line, a blank line between documents.  The
+    text is tokenised with ``BertTokenizer`` (``vocab_file`` must hold [CLS], [SEP], [MASK] and
+    [PAD]).  Item i starts segment A at the i-th sentence of the corpus and takes a random run of
+    sentences of its document; B is, chosen 50/50, the sentences that follow A (next-sentence
+    label 0; an A that would start at its document's last sentence starts one sentence earlier)
+    or a run from a random other document (label 1; always for a one-sentence document).  The
+    pair is truncated to S - 3 tokens, longer side first, and masked as ``MaskedLMDataset`` does
+    (never [CLS], [SEP] or padding).  Item i depends only on ``(seed, i)``.  Items are
+    ``((input_ids, token_type_ids, attention_mask), labels [S + 1])``
+    (``ops.functions.split_pretraining_labels``).  A file with fewer than two documents raises
+    ``ValueError``: the random B needs another document."""
+
+    def __init__(self, text_file, vocab_file, max_seq_length, mask_prob: float = 0.15,
+                 seed: int = 0, do_lower_case: bool = True):
+        if max_seq_length < 5:
+            raise ValueError("max_seq_length must be at least 5 ([CLS] A [SEP] B [SEP])")
+        tok = BertTokenizer(vocab_file, do_lower_case=do_lower_case, max_len=1 << 30)
+        for name in ("[CLS]", "[SEP]", "[MASK]", "[PAD]"):
+            if name not in tok.vocab:
+                raise ValueError("{} has no {} token".format(vocab_file, name))
+        self.cls_id, self.sep_id = tok.vocab["[CLS]"], tok.vocab["[SEP]"]
+        self.mask_id, self.pad_id = tok.vocab["[MASK]"], tok.vocab["[PAD]"]
+        self.vocab_size = len(tok.vocab)
+        self.S, self.mask_prob, self.seed = max_seq_length, mask_prob, seed
+        docs, cur = [], []
+        with open(text_file, encoding="utf-8") as f:
+            for line in f:
+                if not line.strip():
+                    if cur:
+                        docs.append(cur)
+                    cur = []
+                    continue
+                ids = tok.convert_tokens_to_ids(tok.tokenize(line))
+                if ids:
+                    cur.append(ids)
+        if cur:
+            docs.append(cur)
+        if len(docs) < 2:
+            raise ValueError("{} holds {} document(s); next-sentence pairs need at least two "
+                             "(documents are separated by blank lines)".format(text_file, len(docs)))
+        self.docs = docs
+        self.index = [(d, k) for d, doc in enumerate(docs) for k in range(len(doc))]
+
+    def __len__(self):
+        return len(self.index)
+
+    def __getitem__(self, idx):
+        g = _item_generator(self.seed, idx)
+        target = self.S - 3
+        d, k = self.index[idx]
+        doc = self.docs[d]
+        is_random = float(torch.rand(1, generator=g)) < 0.5 or len(doc) < 2
+        if not is_random:
+            # B follows A: A starts early enough to leave at least one sentence after it
+            k = min(k, len(doc) - 2)
+            n_a = int(torch.randint(1, len(doc) - k, (1,), generator=g))
+        else:
+            n_a = int(torch.randint(1, len(doc) - k + 1, (1,), generator=g))
+        a = [t for s in doc[k:k + n_a] for t in s]
+        if not is_random:
+            rest = doc[k + n_a:]
+        else:
+            other = int(torch.randint(0, len(self.docs) - 1, (1,), generator=g))
+            other += other >= d
+            odoc = self.docs[other]
+            rest = odoc[int(torch.randint(0, len(odoc), (1,), generator=g)):]
+        b = []
+        for s in rest:
+            if len(a) + len(b) >= target:
+                break
+            b.extend(s)
+        while len(a) + len(b) > target:
+            (a if len(a) > len(b) else b).pop()
+        if not b:   # A alone filled the budget: keep one B token
+            a.pop()
+            b = rest[0][:1]
+        return pretraining_item(a, b, int(is_random), self.S, self.cls_id, self.sep_id,
+                                self.pad_id, self.mask_id, 0, self.vocab_size, self.mask_prob, g)

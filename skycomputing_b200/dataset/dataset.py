@@ -141,6 +141,77 @@ class SynthMLMDataset(Dataset):
         return (ids, self.segment_ids[idx], self.input_mask[idx]), labels
 
 
+def pretraining_item(a, b, is_random: int, S: int, cls_id: int, sep_id: int, pad_id: int,
+                     mask_id: int, random_low: int, vocab_size: int, mask_prob: float,
+                     g: torch.Generator):
+    """One masked-LM + next-sentence item from the token lists ``a`` and ``b`` (their total
+    already at most S - 3): ``[CLS] a [SEP] b [SEP]`` padded to S, token types 0 up to the first
+    [SEP] and 1 after it, ``bert_mask`` over the body tokens only.  Returns ``((input_ids,
+    token_type_ids, attention_mask), labels [S + 1])``, the next-sentence label ``is_random`` in
+    the last column (``ops.functions.split_pretraining_labels``)."""
+    row = [cls_id] + list(a) + [sep_id] + list(b) + [sep_id]
+    n = len(row)
+    ids = torch.full((S,), pad_id, dtype=torch.long)
+    ids[:n] = torch.tensor(row, dtype=torch.long)
+    types = torch.zeros(S, dtype=torch.long)
+    types[len(a) + 2:n] = 1
+    mask = torch.zeros(S, dtype=torch.long)
+    mask[:n] = 1
+    maskable = mask.bool()
+    maskable[0] = maskable[len(a) + 1] = maskable[n - 1] = False
+    ids, labels = bert_mask(ids, maskable, mask_id, random_low, vocab_size, mask_prob, g)
+    return (ids, types, mask), torch.cat([labels, torch.tensor([int(is_random)])])
+
+
+@DATASET.register_module
+class SynthPretrainingDataset(Dataset):
+    """Synthetic masked-LM + next-sentence data that a model can learn.  An item is ``[CLS] A
+    [SEP] B [SEP]`` (S tokens, no padding): A is an arithmetic progression as in
+    ``SynthMLMDataset`` of random length; for next-sentence label 0 B continues A's progression,
+    for label 1 B is the same progression shifted by a random non-zero offset, so it never
+    continues A.  The labels are exactly balanced (an odd ``num_samples`` leaves one more 0) and
+    drawn with everything else from ``seed``; the masking (``bert_mask``, never a special token)
+    depends only on ``(seed, index)``.  Items are ``((input_ids, token_type_ids,
+    attention_mask), labels [S + 1])``, the layout of ``ops.functions.split_pretraining_labels``.
+    Token ids are ``SynthMLMDataset``'s."""
+
+    def __init__(self, num_samples: int = 1024, max_seq_length: int = 128,
+                 vocab_size: int = 30528, mask_prob: float = 0.15, seed: int = 0,
+                 max_step: int = 4):
+        if max_seq_length < 5:
+            raise ValueError("max_seq_length must be at least 5 ([CLS] A [SEP] B [SEP])")
+        big = vocab_size > 2000
+        self.cls_id, self.sep_id, self.mask_id = (101, 102, 103) if big else (1, 2, 3)
+        self.first = 1000 if big else 4
+        if vocab_size <= self.first + 1:
+            raise ValueError("vocab_size {} leaves too few body tokens".format(vocab_size))
+        self.vocab_size, self.mask_prob, self.seed = vocab_size, mask_prob, seed
+        self.S = max_seq_length
+        g = torch.Generator().manual_seed(seed)
+        span = vocab_size - self.first
+        self.span = span
+        self.start = torch.randint(0, span, (num_samples,), generator=g)
+        self.step = torch.randint(1, max_step + 1, (num_samples,), generator=g)
+        self.len_a = torch.randint(1, max_seq_length - 3, (num_samples,), generator=g)
+        self.offset = torch.randint(1, span, (num_samples,), generator=g)
+        self.nsp = (torch.randperm(num_samples, generator=g) >= (num_samples + 1) // 2).long()
+
+    def __len__(self):
+        return self.start.numel()
+
+    def __getitem__(self, idx):
+        S, la = self.S, int(self.len_a[idx])
+        pos = torch.arange(S - 3)
+        seq = self.first + (self.start[idx] + pos * self.step[idx]) % self.span
+        a = seq[:la]
+        b = seq[la:]
+        if int(self.nsp[idx]):
+            b = self.first + (b - self.first + self.offset[idx]) % self.span
+        return pretraining_item(a.tolist(), b.tolist(), int(self.nsp[idx]), S, self.cls_id,
+                                self.sep_id, 0, self.mask_id, self.first, self.vocab_size,
+                                self.mask_prob, _item_generator(self.seed, idx))
+
+
 @DATASET.register_module
 class RandomMlpDataset(Dataset):
     def __init__(self, num=1000, dim=1024):

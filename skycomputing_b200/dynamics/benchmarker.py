@@ -24,6 +24,8 @@ from typing import Dict, List, Optional
 import torch
 
 from ..builder import build_layer, build_module_from_cfg
+from ..models.bert_layers import MASKED_LM_HEADS
+from ..ops.functions import join_pretraining_labels
 from ..stimulator import Stimulator
 from ..utils import generate_worker_name
 from .estimator import Estimator
@@ -153,6 +155,8 @@ class ModelBenchmarker(BaseBenchmarker):
         B, S = hidden.shape[:2]
         labels = torch.full((B, S), int(layer_cfg.get("ignore_index", -100)), dtype=torch.int64)
         labels[:, :layer_cfg["max_predictions"]] = 0
+        if layer_cfg.get("layer_type") == "BertTailForPreTraining":
+            labels = join_pretraining_labels(labels, torch.zeros(B, dtype=torch.int64))
         return labels
 
     def benchmark(self):
@@ -164,7 +168,7 @@ class ModelBenchmarker(BaseBenchmarker):
         cache: Dict[tuple, tuple] = {}
         for layer_cfg in self._model_config:
             if layer_cfg.get("max_predictions") is not None and \
-                    layer_cfg.get("layer_type") == "BertTailForMaskedLM":
+                    layer_cfg.get("layer_type") in MASKED_LM_HEADS:
                 # a sparse head decodes the labelled positions: bind labels with P of them per
                 # sequence, so that the measured cost is that of a full slot map
                 data = list(data) + [self._head_labels(data[0], layer_cfg)]

@@ -90,8 +90,17 @@ class Estimator:
             mem = (2 * outs + param_scale * params + B * H) * 4 / mb
             return 2.0 * B * H * C, mem, [((B, C), f32)]
         if c is None or lt not in ("BertEmbeddings", "BertLayer_Head", "BertLayer_Body",
-                                   "BertLayer_Tail", "BertPooler", "BertTailForMaskedLM"):
+                                   "BertLayer_Tail", "BertPooler", "BertTailForMaskedLM",
+                                   "BertTailForPreTraining"):
             return None
+        if lt == "BertTailForPreTraining":
+            # the masked-LM head, plus the pooler on the [CLS] rows and the 2-way classifier
+            flops, mem, outs = Estimator.analytic_layer_cost(dict(layer_cfg, layer_type="BertTailForMaskedLM"),
+                                                data, param_scale)
+            B, H = data[0].shape[0], c["hidden_size"]
+            params = H * H + H + 2 * H + 2
+            mem += (2 * 2 * B * (H + 2) + param_scale * params) * 4 / mb
+            return flops + 2.0 * B * H * (H + 2), mem, outs + [((B, 2), f32)]
         H, I, A = c["hidden_size"], c["intermediate_size"], c["num_attention_heads"]
         if lt == "BertTailForMaskedLM":
             B, S, _ = data[0].shape

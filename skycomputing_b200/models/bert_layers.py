@@ -621,7 +621,78 @@ class BertTailForMaskedLM(nn.Module):
         return self.decoder(self.transform(x)), slot_labels
 
 
+@LAYER.register_module
+class BertTailForPreTraining(BertTailForMaskedLM):
+    """Masked-LM and next-sentence-prediction heads (HF ``BertPreTrainingHeads`` plus the pooler
+    it reads): the ``BertTailForMaskedLM`` head, a ``pooler`` (dense + tanh on the [CLS] row) and
+    ``seq_relationship`` (``Linear(H, 2)``, no dropout).  ``(hidden, mask) -> (mlm_logits
+    [B, S, V], nsp_logits [B, 2])``.
+
+    Labels are one int64 tensor ``[B, S + 1]`` (``ops.functions.split_pretraining_labels``).
+    With ``max_predictions=P`` the head takes them and returns ``(mlm_logits [B*P, V],
+    slot_labels [B*P], nsp_logits)``; without labels it returns the dense outputs.  Decoder tie,
+    sparse decoding, argument checks and the last-layer rule are the masked-LM head's.  The
+    native path also needs the batch to be a multiple of 8 (the pooler's weight-gradient GEMM
+    runs over it); other shapes run the eager path."""
+
+    # the outputs the loss differentiates: masked-LM logits first, next-sentence logits last
+    logit_outputs = (0, -1)
+
+    def __init__(self, config, max_predictions=None, ignore_index: int = -100,
+                 tie_word_embeddings: bool = False):
+        super().__init__(config, max_predictions, ignore_index, tie_word_embeddings)
+        config = BertConfig.from_dict(config) if isinstance(config, dict) else config
+        self.pooler = BertPooler(config.__dict__)
+        self.seq_relationship = nn.Linear(config.hidden_size, 2)
+
+    def _native_params(self):
+        from ..ops.functions import PreTrainingHeadParams
+
+        if self._native is None:
+            object.__setattr__(self, "_native", PreTrainingHeadParams(self))
+        return self._native
+
+    def _supports(self, hidden: torch.Tensor) -> bool:
+        return super()._supports(hidden) and hidden.shape[0] % 8 == 0
+
+    def forward(self, hidden_states, attention_mask=None, labels=None):
+        from ..ops.functions import split_pretraining_labels
+
+        if labels is not None and not self.consumes_labels:
+            raise ValueError("labels reach a BertTailForPreTraining without max_predictions")
+        if labels is not None:
+            labels = labels.to(torch.int64).reshape(hidden_states.shape[0], -1)
+        if _native_enabled(hidden_states) and self._supports(hidden_states):
+            from ..ops.functions import PreTrainingHeadFn
+
+            hp = self._native_params()
+            x = hidden_states.to(torch.bfloat16)
+            if not self.training and not torch.is_grad_enabled():
+                return PreTrainingHeadFn.infer(hp, x, labels)
+            return PreTrainingHeadFn.apply(hp, x, labels, *hp.all_params())
+        if hidden_states.is_cuda and _BACKEND != "torch" and super()._supports(hidden_states):
+            _warn_eager_batch(hidden_states.shape[0])
+        nsp = self.seq_relationship(self.pooler.dense_act(hidden_states[:, 0].float()))
+        mlm = super().forward(hidden_states, attention_mask,
+                              None if labels is None else split_pretraining_labels(labels)[0])
+        return (*mlm, nsp) if isinstance(mlm, tuple) else (mlm, nsp)
+
+
 TIED_TABLE_NAME = "word_embeddings.weight"
+_WARNED_EAGER_BATCH = [False]
+
+
+def _warn_eager_batch(batch: int) -> None:
+    """Once per process: a pretraining head on the GPU whose batch is not a multiple of 8 runs
+    the eager fp32 path (the whole vocabulary-wide decoder in fp32)."""
+    if _WARNED_EAGER_BATCH[0]:
+        return
+    _WARNED_EAGER_BATCH[0] = True
+    import warnings
+
+    warnings.warn("BertTailForPreTraining: a batch of {} sequences is not a multiple of 8, so the "
+                  "head runs its eager fp32 path, which is much slower than the native one; use "
+                  "micro-batches of a multiple of 8 sequences".format(batch))
 
 
 def _warn_decoder_unused() -> None:
@@ -651,15 +722,19 @@ def check_tied_layers(first, head) -> None:
         got = first.get("layer_type") if isinstance(first, dict) else type(first).__name__
         raise ValueError("tie_word_embeddings=True needs a BertEmbeddings as the model's first "
                          "layer, got {}".format(got))
-    dec = shape(head, "BertTailForMaskedLM")
+    dec = shape(head, head.get("layer_type") if isinstance(head, dict) else "BertTailForMaskedLM")
     if dec != table:
         raise ValueError("tie_word_embeddings=True: the decoder is [vocab, hidden] = {} but the "
                          "word-embedding table is {}".format(list(dec), list(table)))
 
 
 def is_tied_head_cfg(layer_cfg: dict) -> bool:
-    return (layer_cfg.get("layer_type") == "BertTailForMaskedLM"
+    return (layer_cfg.get("layer_type") in MASKED_LM_HEADS
             and bool(layer_cfg.get("tie_word_embeddings", False)))
+
+
+# registered names of the heads with a masked-LM decoder (BertTailForMaskedLM and its subclass)
+MASKED_LM_HEADS = ("BertTailForMaskedLM", "BertTailForPreTraining")
 
 
 def tie_decoder_to_embeddings(layers) -> bool:

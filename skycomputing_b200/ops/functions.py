@@ -762,6 +762,23 @@ def mlm_slots_ref(labels: torch.Tensor, P: int, ignore_index: int = -100, V: int
     return row_of_slot, slot_of_row, slot_labels
 
 
+def split_pretraining_labels(labels: torch.Tensor):
+    """The labels of a masked-LM + next-sentence item are ONE int64 tensor ``[..., S + 1]``:
+    columns 0..S-1 are the token labels (``ignore_index`` where a position is not predicted),
+    column S is the next-sentence label (0: B follows A, 1: B is random).  Returns ``(mlm [...,
+    S], nsp [...])`` as views.  One tensor keeps the engine's chunking, label buffers and label
+    routing unchanged; this function and ``join_pretraining_labels`` are the only places that
+    know the layout."""
+    return labels[..., :-1], labels[..., -1]
+
+
+def join_pretraining_labels(mlm: torch.Tensor, nsp: torch.Tensor) -> torch.Tensor:
+    """Inverse of ``split_pretraining_labels``: ``mlm`` [B, S'] (or flat B*S') and ``nsp`` [B]
+    -> [B, S' + 1] int64."""
+    nsp = nsp.reshape(-1, 1).to(torch.int64)
+    return torch.cat([mlm.reshape(nsp.shape[0], -1).to(torch.int64), nsp], dim=1)
+
+
 class MaskedLMHeadParams:
     """Parameter banks of ``BertTailForMaskedLM``: transform dense (+ GELU), LayerNorm, decoder;
     and the head's slot contract (``max_predictions``, ``ignore_index``)."""
@@ -841,9 +858,18 @@ class MaskedLMHeadFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dlogits, *_dslot_labels):
-        hp = ctx.hp
-        x, h1, t, mean, rstd, y = ctx.saved
-        B, S, H = ctx.shape3
+        dx = MaskedLMHeadFn._backward(ctx.hp, ctx.saved, ctx.shape3, ctx.slot_of_row, dlogits)
+        ctx.saved = ctx.slot_of_row = None
+        return (None, dx, None, *([None] * ctx.n_params))
+
+    @staticmethod
+    def _backward(hp, saved, shape3, slot_of_row, dlogits, dcls=None) -> torch.Tensor:
+        """The head's chain backward to the [B, S, H] input gradient.  ``dcls`` [B, H] (the
+        pooler branch of the pretraining head) is added into the [CLS] rows as the gradient is
+        written: in ``mlm_scatter`` for the sparse head, in place after the dgrad GEMM for the
+        dense one."""
+        x, h1, t, mean, rstd, y = saved
+        B, S, H = shape3
         g = _flat2d(dlogits)
         if g.dtype != torch.bfloat16:
             g = g.to(torch.bfloat16)
@@ -857,10 +883,93 @@ class MaskedLMHeadFn(torch.autograd.Function):
                             torch.cuda.current_stream().cuda_stream)
         _wgrad(dh1, x, hp.w_t, hp.b_t)
         dx = nat.gemm(dh1, hp.w_t.shadow(), b_mn=True)
-        if ctx.slot_of_row is not None:
-            dx = nat.mlm_scatter(dx, ctx.slot_of_row)
-        ctx.saved = ctx.slot_of_row = None
-        return (None, dx.view(B, S, H), None, *([None] * ctx.n_params))
+        if slot_of_row is not None:
+            return nat.mlm_scatter(dx, slot_of_row, dcls).view(B, S, H)
+        dx = dx.view(B, S, H)
+        if dcls is not None:
+            nat.cls_grad_add_(dx, dcls)
+        return dx
+
+
+class PreTrainingHeadParams(MaskedLMHeadParams):
+    """Banks of ``BertTailForPreTraining``: the masked-LM head's, then the pooler's (the banks of
+    its ``BertPooler`` submodule, shared, so every bank exists once) and the next-sentence
+    classifier's."""
+
+    def __init__(self, mod):
+        super().__init__(mod)
+        self.pool = mod.pooler._native_params()
+        self.nsp = SmallLinearParams(mod.seq_relationship.weight, mod.seq_relationship.bias,
+                                     act_tanh=False, first_token=False)
+        self.banks = self.banks + self.pool.banks + self.nsp.banks
+
+
+class PreTrainingHeadFn(torch.autograd.Function):
+    """BertTailForPreTraining as ONE autograd node: the masked-LM chain of ``MaskedLMHeadFn`` and
+    the next-sentence branch (the pooler's wgmma GEMM with the tanh epilogue on the strided
+    [CLS]-row view, then ``small_linear`` to 2 logits).  Outputs ``(mlm_logits, nsp_logits
+    [B, 2])``, or ``(mlm_logits [B*P, V], slot_labels, nsp_logits)`` with labels [B, S + 1].
+    Backward writes the input gradient once: the pooler's [B, H] input gradient joins the MLM
+    gradient in the [CLS] rows (``MaskedLMHeadFn._backward``)."""
+
+    @staticmethod
+    def _run(hp: PreTrainingHeadParams, hidden: torch.Tensor, keep: bool, labels=None):
+        mlm_labels = None if labels is None else split_pretraining_labels(labels)[0].contiguous()
+        logits, saved, slots = MaskedLMHeadFn._run(hp, hidden, keep, mlm_labels)
+        B, S, H = hidden.shape
+        x0 = hidden.contiguous().view(B, S * H)[:, :H]
+        pooled = nat.gemm(x0, hp.pool.w.shadow(), bias=hp.pool.b.master(), act=nat.ACT_TANH,
+                          out_dtype=torch.float32)
+        w, b = hp.nsp.w.master(), hp.nsp.b.master()
+        nsp = torch.empty((B, w.shape[0]), dtype=torch.float32, device=hidden.device)
+        nat.ext().small_linear_fwd(x=pooled.data_ptr(), x_bf16=False, ldx=H, w=w.data_ptr(),
+                                   b=b.data_ptr(), y=nsp.data_ptr(), M=B, N=w.shape[0], K=H,
+                                   act_tanh=0, dropout_p=0.0, rng_state=0, rng_stream=0,
+                                   stream=torch.cuda.current_stream().cuda_stream)
+        return logits, saved, slots, (x0, pooled, nsp)
+
+    @staticmethod
+    def infer(hp: PreTrainingHeadParams, hidden: torch.Tensor, labels=None):
+        logits, _, slots, (_, _, nsp) = PreTrainingHeadFn._run(hp, hidden, False, labels)
+        return (logits, nsp) if slots is None else (logits, slots[1], nsp)
+
+    @staticmethod
+    def forward(ctx, hp, hidden, labels, *params):
+        logits, saved, slots, nsp_saved = PreTrainingHeadFn._run(hp, hidden, True, labels)
+        ctx.hp, ctx.saved, ctx.nsp_saved = hp, saved, nsp_saved
+        ctx.shape3 = tuple(hidden.shape)
+        ctx.slot_of_row = None if slots is None else slots[0]
+        ctx.n_params = len(params)
+        nsp = nsp_saved[2]
+        if slots is None:
+            return logits, nsp
+        ctx.mark_non_differentiable(slots[1])
+        return logits, slots[1], nsp
+
+    @staticmethod
+    def backward(ctx, dlogits, *rest):
+        hp = ctx.hp
+        dnsp = rest[-1]
+        x0, pooled, nsp = ctx.nsp_saved
+        B, S, H = ctx.shape3
+        # next-sentence classifier, then the pooler (bias + tanh derivative as in PoolerFn)
+        w = hp.nsp.w.master()
+        dpooled = torch.empty_like(pooled)
+        nat.ext().small_linear_bwd(x=pooled.data_ptr(), x_bf16=False, ldx=H, w=w.data_ptr(),
+                                   y=nsp.data_ptr(), dy=dnsp.contiguous().float().data_ptr(),
+                                   dx=dpooled.data_ptr(), dx_bf16=False, lddx=H,
+                                   dw=hp.nsp.w.grad().data_ptr(), db=hp.nsp.b.grad().data_ptr(),
+                                   M=B, N=w.shape[0], K=H, act_tanh=0, dropout_p=0.0,
+                                   rng_state=0, rng_stream=0,
+                                   stream=torch.cuda.current_stream().cuda_stream)
+        g = dpooled * (1.0 - pooled * pooled)
+        hp.pool.b.grad().add_(g.sum(0))
+        gb = g.to(torch.bfloat16)
+        nat.gemm(gb, x0, a_mn=True, b_mn=True, out=hp.pool.w.grad(), accumulate=True)
+        dcls = nat.gemm(gb, hp.pool.w.shadow(), b_mn=True)
+        dx = MaskedLMHeadFn._backward(hp, ctx.saved, ctx.shape3, ctx.slot_of_row, dlogits, dcls)
+        ctx.saved = ctx.nsp_saved = ctx.slot_of_row = None
+        return (None, dx, None, *([None] * ctx.n_params))
 
 
 class SoftmaxCrossEntropyFn(torch.autograd.Function):

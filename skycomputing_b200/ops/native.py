@@ -494,18 +494,67 @@ def mlm_gather(hidden: torch.Tensor, labels: torch.Tensor, P: int, V: int,
     return x_c, slot_of_row, slot_labels
 
 
-def mlm_scatter(dx_c: torch.Tensor, slot_of_row: torch.Tensor) -> torch.Tensor:
+def mlm_scatter(dx_c: torch.Tensor, slot_of_row: torch.Tensor,
+                dcls: Optional[torch.Tensor] = None) -> torch.Tensor:
     """The input gradient of a sparse head: ``dhidden[r] = dx_c[slot_of_row[r]]`` for a decoded
-    row, zeros otherwise; ``dhidden`` [len(slot_of_row), H] bf16, every row written once."""
+    row, zeros otherwise; ``dhidden`` [len(slot_of_row), H] bf16, every row written once.  With
+    ``dcls`` [B, H] bf16 (a pooler branch's input gradient) the [CLS] row b*S of each sequence
+    also gets ``dcls[b]`` added, S = len(slot_of_row) / B."""
     _check(dx_c, torch.bfloat16, "dx_c")
     if slot_of_row.dtype != torch.int32 or not slot_of_row.is_cuda:
         raise ValueError("slot_of_row must be a CUDA int32 tensor")
     dx_c = dx_c.contiguous()
     H = dx_c.shape[-1]
+    S = 1
+    if dcls is not None:
+        _check(dcls, torch.bfloat16, "dcls")
+        if dcls.dim() != 2 or dcls.shape[1] != H or slot_of_row.numel() % dcls.shape[0]:
+            raise ValueError("dcls must be [B, H] with B dividing the number of rows")
+        dcls = dcls.contiguous()
+        S = slot_of_row.numel() // dcls.shape[0]
     dhidden = torch.empty((slot_of_row.numel(), H), dtype=torch.bfloat16, device=dx_c.device)
     ext().mlm_scatter(dx_c=dx_c.data_ptr(), slot_of_row=slot_of_row.data_ptr(),
-                      rows=slot_of_row.numel(), H=H, dhidden=dhidden.data_ptr(), stream=_stream())
+                      rows=slot_of_row.numel(), H=H, dhidden=dhidden.data_ptr(), stream=_stream(),
+                      dcls=_ptr(dcls), S=S)
     return dhidden
+
+
+def cls_grad_add_(dhidden: torch.Tensor, dcls: torch.Tensor) -> torch.Tensor:
+    """``dhidden[b, 0] += dcls[b]`` in place (bf16 [B, S, H] and [B, H]): the [CLS]-row join of a
+    dense head with a pooler branch.  One launch."""
+    _check(dhidden, torch.bfloat16, "dhidden")
+    _check(dcls, torch.bfloat16, "dcls")
+    B, S, H = dhidden.shape
+    if not dhidden.is_contiguous() or tuple(dcls.shape) != (B, H):
+        raise ValueError("dhidden must be a contiguous [B, S, H] tensor and dcls [B, H]")
+    dcls = dcls.contiguous()
+    ext().cls_grad_add(dhidden=dhidden.data_ptr(), dcls=dcls.data_ptr(), B=B, S=S, H=H,
+                       stream=_stream())
+    return dhidden
+
+
+def masked_softmax_ce(logits: torch.Tensor, labels: torch.Tensor, grad_scale: float = 1.0,
+                      loss_acc: Optional[torch.Tensor] = None, ignore_index: int = -100):
+    """Cross entropy over fp32 logits ``[M, C]`` with ``ignore_index`` (the next-sentence loss).
+    Returns ``(loss [1], dlogits [M, C])``: the mean over the labelled rows and d(loss *
+    grad_scale)/dlogits, exact 0 on every other row; 0 and an all-zero gradient without a
+    labelled row; a NaN loss and a zero gradient row for a label outside [0, C) that is not
+    ``ignore_index``.  ``loss_acc[0] += loss * grad_scale`` when given.  One launch, no host
+    synchronisation, deterministic."""
+    _check(logits, torch.float32, "logits")
+    if logits.dim() != 2 or logits.stride(1) != 1:
+        raise ValueError("logits must be a 2-D [M, C] tensor with unit column stride")
+    M, C = logits.shape
+    if not labels.is_cuda or labels.dtype != torch.int64 or labels.numel() != M:
+        raise ValueError("labels must be a CUDA int64 tensor with one entry per logits row")
+    labels = labels.reshape(-1).contiguous()
+    loss = torch.empty(1, dtype=torch.float32, device=logits.device)
+    dlogits = torch.empty((M, C), dtype=torch.float32, device=logits.device)
+    ext().masked_softmax_ce(logits=logits.data_ptr(), ldl=max(logits.stride(0), C),
+                            labels=labels.data_ptr(), M=M, C=C, ignore_index=int(ignore_index),
+                            dlogits=dlogits.data_ptr(), grad_scale=float(grad_scale),
+                            loss=loss.data_ptr(), loss_acc=_ptr(loss_acc), stream=_stream())
+    return loss, dlogits
 
 
 class TokenEvalAccumulator:

@@ -233,29 +233,50 @@ class EngineBase:
         st.labels = label_chunks[j] if (label_chunks is not None and consumes) else None
 
     @staticmethod
+    def _logit_outputs(st, outs) -> list:
+        """The logits among the last stage's outputs, where the loss's gradients go: ``outs[0]``,
+        or the outputs a last layer lists in ``logit_outputs`` (the pretraining head: masked-LM
+        and next-sentence logits)."""
+        layers = getattr(st, "layers", None)
+        last = layers[-1] if layers is not None and len(layers) else None
+        return [outs[i] for i in getattr(last, "logit_outputs", (0,))]
+
+    @staticmethod
     def _head_outputs(st, outs, labels):
         """(logits, labels) that the loss / the evaluation accumulator read from the last stage's
-        outputs: a label-consuming last layer returns its own labels, one per decoded row, as
-        ``outs[1]`` (viewed as [sequences, rows per sequence]); backward still starts at
-        ``outs[0]``."""
+        outputs.  ``logits`` is the one logits tensor, or the tuple of them for a head with
+        several (the pretraining head).  A label-consuming last layer returns its own labels, one
+        per decoded row, as ``outs[1]`` (viewed as [sequences, rows per sequence]); a pretraining
+        head's next-sentence labels stay in the last column (``split_pretraining_labels``)."""
+        logits = EngineBase._logit_outputs(st, outs)
         if getattr(st, "consumes_labels", False):
-            return outs[0], outs[1].view(labels.shape[0], -1)
-        return outs[0], labels
+            slot = outs[1].view(labels.shape[0], -1)
+            if len(logits) > 1:
+                from ..ops.functions import join_pretraining_labels, split_pretraining_labels
+
+                slot = join_pretraining_labels(slot, split_pretraining_labels(labels)[1])
+            labels = slot
+        return (logits[0] if len(logits) == 1 else tuple(logits)), labels
 
     def _last_stage_loss(self, st, outs, labels):
         """The loss of one micro-batch on the last stage, added into ``_loss_acc``."""
         logits, labels = self._head_outputs(st, outs, labels)
-        if hasattr(self.loss_fn, "fused") and logits.is_cuda and self._loss_acc.dtype == torch.float32:
-            # (dlogits,) instead of a scalar loss: see _NativeCrossEntropy.fused
-            return (self.loss_fn.fused(logits, labels, 1.0 / self.m, self._loss_acc.view(1)),)
+        first = logits[0] if isinstance(logits, tuple) else logits
+        if hasattr(self.loss_fn, "fused") and first.is_cuda and self._loss_acc.dtype == torch.float32:
+            # gradients of the logits instead of a scalar loss: see _NativeCrossEntropy.fused
+            grads = self.loss_fn.fused(logits, labels, 1.0 / self.m, self._loss_acc.view(1))
+            return grads if isinstance(grads, tuple) else (grads,)
         loss = self.loss_fn(logits, labels) / self.m
         self._loss_acc += loss.detach().float()
         return loss
 
     @staticmethod
-    def _backward_from_loss(outs, loss) -> None:
+    def _backward_from_loss(st, outs, loss) -> None:
+        """``loss`` is a scalar, or the tuple of gradients of the head's logit outputs (the fused
+        loss): backward then starts at each of them."""
         if isinstance(loss, tuple):
-            torch.autograd.backward([outs[0]], [loss[0].to(outs[0].dtype)])
+            ts = EngineBase._logit_outputs(st, outs)[:len(loss)]
+            torch.autograd.backward(ts, [g.to(t.dtype) for t, g in zip(ts, loss)])
         else:
             loss.backward()
 

@@ -167,7 +167,7 @@ class PipelineEngine(EngineBase):
         st.begin_backward()
         with self._arm_wgrad_sgd(0, j):
             if self.is_last:
-                self._backward_from_loss(outs, loss)
+                self._backward_from_loss(st, outs, loss)
             elif self.out_fused:
                 dummy = outs[0]
                 torch.autograd.backward([dummy], [torch.zeros_like(dummy)])

@@ -159,7 +159,7 @@ class LoopedPipelineEngine(EngineBase):
                 st.begin_backward()
                 with self._arm_wgrad_sgd(c, j):
                     if last_stage:
-                        self._backward_from_loss(outs, loss)
+                        self._backward_from_loss(st, outs, loss)
                     else:
                         torch.autograd.backward([outs[0]], [torch.zeros_like(outs[0])])
                 st.end_backward()
@@ -209,7 +209,7 @@ class LoopedPipelineEngine(EngineBase):
                 st.begin_backward()
                 with self._arm_wgrad_sgd(c, j):
                     if last_stage:
-                        self._backward_from_loss(outs, loss)
+                        self._backward_from_loss(st, outs, loss)
                     else:
                         grads, reqs = self.comm.recv(self.next_rank, f"bwd{c}",
                                                      metas=self._grad_metas(outs))

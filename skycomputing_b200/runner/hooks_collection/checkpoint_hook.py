@@ -33,7 +33,10 @@ def _dist():
 class CheckpointHook(Hook):
     def __init__(self, load_checkpoint_from: str = None, save_path: str = None,
                  save_interval: int = None, save_optimizer: bool = True,
-                 resume_training_state: bool = False, strict_optimizer: bool = False):
+                 resume_training_state: bool = False, strict_optimizer: bool = False,
+                 from_pretraining: bool = False):
+        # from_pretraining=True initialises a model (a classification config, typically) from a
+        # file saved by a pretraining run: weights only, see _from_pretraining_entry
         # resume_training_state=True also restores optimizer state and the epoch / iteration
         # counters from the per-rank ``.extra`` shards (same world size required); the default
         # restores weights only, like the reference.
@@ -43,6 +46,10 @@ class CheckpointHook(Hook):
         self._save_interval = save_interval
         self._save_path = save_path
         self._save_optimizer = save_optimizer
+        self._from_pretraining = from_pretraining
+        if from_pretraining and resume_training_state:
+            raise ValueError("from_pretraining loads weights only: it cannot resume the training "
+                             "state of another run")
 
     # ------------------------------------------------------------------ load
     def before_run(self, runner):
@@ -54,6 +61,7 @@ class CheckpointHook(Hook):
             idx, name = key.split(".", 1)
             per_layer.setdefault(int(idx), OrderedDict())[name] = val
         self._tie_rule(runner, per_layer, self._load_checkpoint_from)
+        dropped, kept_init = [], []
         for module in runner.model.model:
             if not module.is_local:
                 continue
@@ -61,13 +69,33 @@ class CheckpointHook(Hook):
             if runner.parameter_server is not None:
                 n_layers = max(n_layers, len(runner.parameter_server))
             b, e = module.layer_range if module.layer_range is not None else (0, n_layers)
-            # layers without parameters / buffers (ReLU, Flatten, Dropout-only ...) have no keys in
-            # the file: they load an empty state dict, as in the reference's ParameterServer path
-            module.load_weights([per_layer.get(i, OrderedDict()) for i in range(b, e)])
+            layers = list(module.module.layers.children())
+            sds = []
+            for i in range(b, e):
+                # layers without parameters / buffers (ReLU, Flatten, Dropout-only ...) have no keys
+                # in the file: they load an empty state dict, as in the reference's ParameterServer
+                sd = per_layer.get(i, OrderedDict())
+                if self._from_pretraining:
+                    sd = self._from_pretraining_entry(layers[i - b], i, sd, dropped, kept_init)
+                else:
+                    self._check_not_pretraining(layers[i - b], i, sd)
+                sds.append(sd)
+            module.load_weights(sds)
+        if self._from_pretraining:
+            msg = ("CheckpointHook: initialised from the pretraining checkpoint {}; dropped "
+                   "entries: {}; left at initialisation: {}".format(
+                       self._load_checkpoint_from, "; ".join(dropped) or "none",
+                       "; ".join(kept_init) or "none"))
+            runner._log(msg)
+            print(msg, flush=True)
         engine = getattr(runner, "engine", None)
         if engine is not None and hasattr(engine, "sync_tied_weights"):
             engine.sync_tied_weights()   # an engine that is already set up: replica := table
-        if runner.is_rank0:
+        if self._from_pretraining:
+            # rank 0's copy takes what the workers hold now: the loaded entries and, for the
+            # layers left at initialisation, the workers' own initial weights
+            self._gather_to_parameter_server(runner)
+        elif runner.is_rank0:
             runner.parameter_server.load_weights_from_file(self._load_checkpoint_from)
         extra = self._extra_path(self._load_checkpoint_from, runner.rank)
         if self._resume_training_state and osp.exists(extra):
@@ -86,6 +114,52 @@ class CheckpointHook(Hook):
                     runner._log(msg)
             runner.iter = st.get("iter", runner.iter)
             runner.epoch = st.get("epoch", runner.epoch)
+
+    @staticmethod
+    def _from_pretraining_entry(layer, idx: int, sd, dropped: list, kept_init: list):
+        """What layer ``idx`` of the model loads from a pretraining file's entry ``sd``: the entry
+        when its names are the layer's; for a ``BertPooler``, the ``pooler.*`` entries of a
+        pretraining head saved at the same index; otherwise the layer's own current state (it
+        keeps its initialisation).  Entries not taken are reported in ``dropped`` (as
+        ``layer idx: prefix.*``), layers left at initialisation in ``kept_init``."""
+        from ...models.bert_layers import BertPooler
+
+        own = layer.state_dict()
+        take, used = None, ()
+        if set(sd) == set(own):
+            take, used = sd, tuple(sd)
+        elif isinstance(layer, BertPooler) and all("pooler." + k in sd for k in own):
+            used = tuple("pooler." + k for k in own)
+            take = OrderedDict((k, sd["pooler." + k]) for k in own)
+        if take is not None:
+            for k, v in take.items():
+                if tuple(v.shape) != tuple(own[k].shape):
+                    raise ValueError(
+                        "layer {} ({}): the checkpoint's {} is {} but the model's is {}; build the "
+                        "model with the pretraining run's geometry (a masked-LM run pads the "
+                        "vocabulary to a multiple of 8)".format(idx, type(layer).__name__, k,
+                                                               list(v.shape), list(own[k].shape)))
+        rest = sorted({k.split(".", 1)[0] for k in sd if k not in used})
+        if rest:
+            dropped.append("layer {}: {}".format(idx, ", ".join(r + ".*" for r in rest)))
+        if take is None:
+            if own:
+                kept_init.append("layer {} ({})".format(idx, type(layer).__name__))
+            return own
+        return take
+
+    @staticmethod
+    def _check_not_pretraining(layer, idx: int, sd) -> None:
+        """A classification layer fed a pretraining head's entry: a clear error instead of a
+        ``load_state_dict`` traceback."""
+        own = layer.state_dict()
+        if own and set(sd) != set(own) and any(k.startswith(("transform.", "decoder.",
+                                                             "seq_relationship.")) for k in sd):
+            raise ValueError(
+                "layer {} ({}) gets the entries of a masked-LM / pretraining head ({}): the "
+                "checkpoint comes from a pretraining model; load it with CheckpointHook("
+                "load_checkpoint_from=..., from_pretraining=True)".format(
+                    idx, type(layer).__name__, ", ".join(sorted({k.split(".", 1)[0] for k in sd}))))
 
     @staticmethod
     def _tie_rule(runner, per_layer: dict, path: str) -> None:
@@ -133,9 +207,9 @@ class CheckpointHook(Hook):
         # an evaluation pass is not a training epoch: no checkpoint
         return None
 
-    def save(self, runner, file_name: str) -> None:
-        if runner.is_rank0:
-            os.makedirs(osp.dirname(osp.abspath(file_name)), exist_ok=True)
+    @staticmethod
+    def _gather_to_parameter_server(runner) -> None:
+        """Every rank's layer weights into rank 0's ParameterServer.  Collective."""
         local = {}
         for module in runner.model.model:
             if not module.is_local:
@@ -157,8 +231,15 @@ class CheckpointHook(Hook):
                     except Exception as exc:
                         raise Exception("have {} state dicts, have {} layers, error occurs at {}".format(
                             sum(len(p) for p in gathered), len(runner.parameter_server), idx)) from exc
+
+    def save(self, runner, file_name: str) -> None:
+        if runner.is_rank0:
+            os.makedirs(osp.dirname(osp.abspath(file_name)), exist_ok=True)
+        self._gather_to_parameter_server(runner)
+        if runner.is_rank0:
             runner.parameter_server.save_weights_to_file(file_name)
         if self._save_optimizer:
+            d = _dist()
             if d is not None:
                 d.barrier()
             torch.save(dict(optimizer=runner.optimizer.state_dict() if runner.optimizer else None,

@@ -137,7 +137,10 @@ class LazyEvalAccumulator:
         if self.inner is not None:
             self.inner.reset()
 
-    def add(self, logits: torch.Tensor, labels: torch.Tensor) -> None:
+    def add(self, logits, labels: torch.Tensor) -> None:
+        if self.inner is None and isinstance(logits, (tuple, list)):
+            # pretraining head: (masked-LM logits, next-sentence logits)
+            self.inner = PreTrainingAccumulator(logits[0].shape[-1], logits[0].device)
         if self.inner is None:
             # one prediction per token (MLM head: [B, S, V] logits, [B, S] labels) or per sequence
             per_token = logits.dim() == 3 or labels.dim() == 2
@@ -149,6 +152,47 @@ class LazyEvalAccumulator:
         if self.inner is None:
             return dict(loss_sum=0.0, count=0, invalid=0, confusion=torch.zeros(0, 0, dtype=torch.int64))
         return self.inner.read()
+
+
+class PreTrainingAccumulator:
+    """Both objectives of a pretraining head: the masked-LM token totals and the next-sentence
+    classification totals (two classes), each in the accumulator ``make_token_accumulator`` /
+    ``make_accumulator`` picks for the device.  ``add`` takes ``(mlm_logits, nsp_logits)`` and
+    the one-tensor labels of ``ops.functions.split_pretraining_labels``."""
+
+    def __init__(self, V: int, device):
+        self.mlm = make_token_accumulator(V, device)
+        self.nsp = make_accumulator(2, device)
+
+    def reset(self) -> None:
+        self.mlm.reset()
+        self.nsp.reset()
+
+    def add(self, logits, labels: torch.Tensor, ignore_index: int = -100) -> None:
+        from ..ops.functions import split_pretraining_labels
+
+        mlm_labels, nsp_labels = split_pretraining_labels(labels)
+        self.mlm.add(logits[0], mlm_labels, ignore_index)
+        self.nsp.add(logits[1], nsp_labels, ignore_index)
+
+    def read(self) -> dict:
+        return dict(mlm=self.mlm.read(), nsp=self.nsp.read())
+
+
+def pretraining_metrics(totals: dict) -> dict:
+    """``mlm_n``, ``mlm_loss``, ``mlm_accuracy``, ``perplexity`` (``token_metrics`` of the
+    masked-LM totals), ``nsp_n``, ``nsp_loss``, ``nsp_accuracy`` (``classification_metrics`` of the
+    next-sentence totals) and ``loss = mlm_loss + nsp_loss``, an objective without a labelled row
+    counting 0 (None when neither has one)."""
+    m, n = totals["mlm"], totals["nsp"]
+    tok = token_metrics(m["loss_sum"], m["count"], m["correct"])
+    cls = classification_metrics(n["confusion"], n["loss_sum"], n["count"])
+    out = dict(mlm_n=tok["n"], mlm_loss=tok["loss"], mlm_accuracy=tok["accuracy"],
+               perplexity=tok["perplexity"], nsp_n=cls["n"], nsp_loss=cls["loss"],
+               nsp_accuracy=cls["accuracy"])
+    out["loss"] = (None if tok["n"] == 0 and cls["n"] == 0
+                   else (tok["loss"] or 0.0) + (cls["loss"] or 0.0))
+    return out
 
 
 def classification_metrics(confusion, loss_sum: float, count: int) -> dict:
@@ -181,7 +225,8 @@ def token_metrics(loss_sum: float, count: int, correct: int) -> dict:
 
 def format_metrics(metrics: dict) -> str:
     parts = []
-    for k in ("n", "loss", "accuracy", "perplexity", "f1", "mcc"):
+    for k in ("n", "loss", "accuracy", "perplexity", "f1", "mcc", "mlm_n", "mlm_loss",
+              "mlm_accuracy", "nsp_n", "nsp_loss", "nsp_accuracy"):
         if k in metrics:
             v = metrics[k]
             parts.append("{}={}".format(k, "None" if v is None else (
@@ -191,4 +236,5 @@ def format_metrics(metrics: dict) -> str:
 
 __all__ = ["TorchEvalAccumulator", "TorchTokenAccumulator", "LazyEvalAccumulator",
            "make_accumulator", "make_token_accumulator", "classification_metrics", "token_metrics",
+           "PreTrainingAccumulator", "pretraining_metrics",
            "format_metrics"]

@@ -84,9 +84,55 @@ class _NativeMaskedLMLoss(MaskedLMLoss):
         return dlogits.view(logits.shape)
 
 
+class PreTrainingLoss(nn.Module):
+    """BERT's pretraining loss (HF ``BertForPreTraining``'s ``total_loss``): the ``MaskedLMLoss``
+    mean of the masked-LM logits plus the next-sentence cross entropy, each a mean over its
+    labelled rows (0 without one).  ``logits`` = ``(mlm_logits, nsp_logits)``, ``labels`` the
+    one-tensor layout of ``ops.functions.split_pretraining_labels``."""
+
+    def __init__(self, ignore_index: int = -100):
+        super().__init__()
+        self.ignore_index = int(ignore_index)
+        self.mlm = MaskedLMLoss(ignore_index)
+
+    def forward(self, logits, labels):
+        from ..ops.functions import split_pretraining_labels
+
+        mlm_logits, nsp_logits = logits
+        mlm_labels, nsp_labels = split_pretraining_labels(labels)
+        return self.mlm(mlm_logits, mlm_labels) + self.mlm(nsp_logits, nsp_labels)
+
+
+class _NativePreTrainingLoss(PreTrainingLoss):
+    def __init__(self, ignore_index: int = -100):
+        super().__init__(ignore_index)
+        self.mlm = _NativeMaskedLMLoss(ignore_index)
+
+    def fused(self, logits, labels, scale: float, loss_acc: torch.Tensor):
+        """Engine fast path: ``vocab_ce`` and ``masked_softmax_ce`` each add their ``loss *
+        scale`` into ``loss_acc``; returns the gradients of (mlm_logits, nsp_logits)."""
+        from ..ops import native as nat
+        from ..ops.functions import split_pretraining_labels
+
+        mlm_logits, nsp_logits = logits
+        mlm_labels, nsp_labels = split_pretraining_labels(labels)
+        dmlm = self.mlm.fused(mlm_logits, mlm_labels, scale, loss_acc)
+        _, dnsp = nat.masked_softmax_ce(nsp_logits.detach().float(), nsp_labels, grad_scale=scale,
+                                        loss_acc=loss_acc, ignore_index=self.ignore_index)
+        return dmlm, dnsp
+
+
 def build_loss(loss_cfg: dict, device: torch.device) -> nn.Module:
     cfg = dict(loss_cfg)
     name = cfg.pop("type")
+    if name == "PreTrainingLoss":
+        if device.type == "cuda":
+            from ..models.bert_layers import get_backend
+            from ..ops import native as nat
+
+            if get_backend() != "torch" and nat.available():
+                return _NativePreTrainingLoss(**cfg)
+        return PreTrainingLoss(**cfg)
     if name == "MaskedLMLoss":
         if device.type == "cuda":
             from ..models.bert_layers import get_backend
@@ -343,7 +389,10 @@ class Runner:
         """Classification metrics of the model on ``data_loader`` (collective: every rank calls
         it and every rank gets the same dict, broadcast by the last stage).  For a token-level
         head (3-D logits / 2-D labels, e.g. ``BertTailForMaskedLM``) the metrics are those of
-        ``token_metrics``: labelled tokens, loss, top-1 accuracy and perplexity.
+        ``token_metrics``: labelled tokens, loss, top-1 accuracy and perplexity.  For a
+        pretraining head (``BertTailForPreTraining``) they are those of ``pretraining_metrics``:
+        the masked-LM ones with an ``mlm_`` prefix (and ``perplexity``), the next-sentence ``nsp_n``,
+        ``nsp_loss`` and ``nsp_accuracy``, and ``loss`` = the sum of the two losses.
 
         The model runs in eval mode (the previous mode is restored) through the engine's
         forward-only pass with ``micro_batches`` chunks per batch (default: the training value;
@@ -356,7 +405,7 @@ class Runner:
         import torch.distributed as dist
 
         from .metrics import (LazyEvalAccumulator, classification_metrics, format_metrics,
-                              token_metrics)
+                              pretraining_metrics, token_metrics)
 
         eng = self.engine
         m = int(micro_batches or self.micro_batches)
@@ -395,7 +444,11 @@ class Runner:
                 self._call_hook("after_val_iter")
             totals = acc.read() if eng.is_last else None
             payload = None
-            if totals is not None and "confusion" not in totals:   # token-level (MLM head)
+            if totals is not None and "mlm" in totals:   # pretraining head: both objectives
+                m, n = totals["mlm"], totals["nsp"]
+                payload = dict(pretraining_metrics(totals), invalid=m["invalid"] + n["invalid"],
+                               classes=m["classes"], nsp_invalid=n["invalid"])
+            elif totals is not None and "confusion" not in totals:   # token-level (MLM head)
                 payload = dict(token_metrics(totals["loss_sum"], totals["count"],
                                              totals["correct"]),
                                invalid=totals["invalid"], classes=totals["classes"])
@@ -416,9 +469,13 @@ class Runner:
             torch.random.set_rng_state(cpu_rng)
         invalid, classes = payload.pop("invalid"), payload.pop("classes")
         max_predictions = payload.pop("max_predictions")
+        nsp_invalid = payload.pop("nsp_invalid", None)
         if invalid:
             msg = "evaluation {}: {} labels are outside [0, {}) and not ignore_index ({})".format(
                 name, invalid, classes, ignore_index)
+            if nsp_invalid is not None:
+                msg += " ({} of them next-sentence labels, which must be in [0, 2))".format(
+                    nsp_invalid)
             if max_predictions is not None:
                 msg += ("; the sparse masked-language-model head decodes at most max_predictions = "
                         "{} labelled positions per sequence, and a sequence with more gets the "

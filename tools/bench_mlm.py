@@ -27,6 +27,16 @@ compares the decoder tied to the word embeddings (``tie_word_embeddings=True``) 
 head instead, at the same geometry: SGD (momentum 0.9) and LAMB, dense and sparse head (P = 20
 unless given), each pair in alternating windows.  Per arm: ms/step (median), peak memory from its
 construction through its warm-up, parameter count and native kernel launches per step.
+
+    python tools/bench_mlm.py --nsp [--steps 20] [--rounds 5] [--max-predictions P]
+
+compares the masked-LM head (``BertTailForMaskedLM`` + ``MaskedLMLoss``) with the pretraining head
+(``BertTailForPreTraining`` + ``PreTrainingLoss``: the same head plus the pooler, the
+next-sentence classifier and its loss) at the same geometry, dense and sparse (P = 20 unless
+given), SGD, each pair in alternating windows.  Per arm: ms/step (median), peak memory from its
+construction through its warm-up and native kernel launches per step.  The [CLS]-row join kernels
+(``cls_grad_add``; ``mlm_scatter`` with and without the [CLS]-row gradient) are timed from graph
+replays against their byte floors.
 """
 from __future__ import annotations
 
@@ -58,14 +68,15 @@ def card() -> dict:
 
 
 def build_runner(layers: int, mlm: bool, max_predictions=None, tie: bool = False,
-                 optim: str = "SGD"):
+                 optim: str = "SGD", nsp: bool = False):
     cfg = sky.BertConfig.bert_large()
     if mlm:
         cfg.vocab_size = V
     enc = [dict(layer_type="BertLayer_Head", config=cfg.__dict__),
            dict(layer_type="BertLayer_Body", config=cfg.__dict__),
            dict(layer_type="BertLayer_Tail", config=cfg.__dict__)] * layers
-    head = dict(layer_type="BertTailForMaskedLM", config=cfg.__dict__)
+    head = dict(layer_type="BertTailForPreTraining" if nsp else "BertTailForMaskedLM",
+                config=cfg.__dict__)
     if max_predictions is not None:
         head["max_predictions"] = max_predictions
     if tie:
@@ -88,11 +99,14 @@ def build_runner(layers: int, mlm: bool, max_predictions=None, tie: bool = False
     opt = sky.build_optimizer(model.optim_module, optim_cfg)
     runner = sky.Runner(model=model, parameter_server=None, worker_manager=wm, optimizer=opt,
                         max_epochs=1, max_iters=1, device=torch.device("cuda", 0),
-                        loss_cfg=dict(type="MaskedLMLoss" if mlm else "CrossEntropyLoss"),
+                        loss_cfg=dict(type="PreTrainingLoss" if nsp else
+                                      "MaskedLMLoss" if mlm else "CrossEntropyLoss"),
                         timer_cfg=dict(root="/tmp/sky_bench_mlm"), logging_cfg=None,
                         micro_batches=1, use_cuda_graph=True)
     model.train(True)
-    if mlm:
+    if nsp:
+        ds = sky.SynthPretrainingDataset(num_samples=B, max_seq_length=S, vocab_size=V, seed=0)
+    elif mlm:
         ds = sky.SynthMLMDataset(num_samples=B, max_seq_length=S, vocab_size=V, seed=0)
     else:
         ds = sky.SynthMNLIDataset(num_samples=B, max_seq_length=S, seed=0)
@@ -220,6 +234,77 @@ def tie_compare(args) -> dict:
     return out
 
 
+def join_kernels(P: int) -> dict:
+    """The [CLS]-row join at the benchmark's geometry against the byte floors."""
+    H = 1024
+    g = torch.Generator(device="cuda").manual_seed(2)
+    ds = sky.SynthPretrainingDataset(num_samples=B, max_seq_length=S, vocab_size=V, seed=0)
+    _, labels = next(iter(torch.utils.data.DataLoader(ds, batch_size=B)))
+    labels = labels[:, :S].contiguous().cuda()
+    hidden = torch.randn(B * S, H, generator=g, device="cuda").to(torch.bfloat16)
+    _, slot_of_row, _ = nat.mlm_gather(hidden, labels, P, V)
+    dx_c = torch.randn(B * P, H, generator=g, device="cuda").to(torch.bfloat16)
+    dcls = torch.randn(B, H, generator=g, device="cuda").to(torch.bfloat16)
+    dense = torch.randn(B, S, H, generator=g, device="cuda").to(torch.bfloat16)
+    decoded = min(int((labels != -100).sum()), B * P)
+    scatter_bytes = B * S * 4 + decoded * H * 2 + B * S * H * 2
+    out = {}
+    for name, fn, nbytes in (
+            ("cls_grad_add", lambda: nat.cls_grad_add_(dense, dcls), 3 * B * H * 2),
+            ("mlm_scatter", lambda: nat.mlm_scatter(dx_c, slot_of_row), scatter_bytes),
+            ("mlm_scatter_with_cls", lambda: nat.mlm_scatter(dx_c, slot_of_row, dcls),
+             scatter_bytes + B * H * 2)):
+        t = graph_kernel_ms(fn)
+        floor_ms = nbytes / HBM_BYTES_PER_S * 1e3
+        out[name] = dict(ms=t, bytes=nbytes, byte_floor_ms=floor_ms, floor_over_time=floor_ms / t)
+        print("{} B={} S={} H={}: {:.2f} us, byte floor {:.2f} us ({:.2f} of the floor's time)"
+              .format(name, B, S, H, t * 1e3, floor_ms * 1e3, floor_ms / t), flush=True)
+    return out
+
+
+def nsp_compare(args) -> dict:
+    """Masked-LM head against the pretraining head: dense / sparse, alternating windows."""
+    P = args.max_predictions or 20
+    nat.enable_launch_counter()
+    out = {}
+    for head in ("dense", "sparse"):
+        arms, peak, launches = {}, {}, {}
+        for arm in ("mlm", "mlm_nsp"):
+            torch.cuda.synchronize()
+            base = torch.cuda.memory_allocated()
+            torch.cuda.reset_peak_memory_stats()
+            arms[arm] = build_runner(args.layers, True, P if head == "sparse" else None,
+                                     nsp=arm == "mlm_nsp")
+            runner, inputs, labels = arms[arm]
+            for _ in range(args.warmup):
+                runner.engine.train_step(inputs, labels)
+            torch.cuda.synchronize()
+            assert runner.engine._graph is not None, arm
+            peak[arm] = (torch.cuda.max_memory_allocated() - base) / 2 ** 20
+            launches[arm] = runner.engine.launches_per_step
+        times = {arm: [] for arm in arms}
+        for _ in range(args.rounds):
+            for arm, (runner, inputs, labels) in arms.items():
+                times[arm].append(step_window(runner, inputs, labels, args.steps))
+        for runner, _, _ in arms.values():
+            runner.engine.close()
+        del arms, runner, inputs, labels
+        gc.collect()
+        torch.cuda.empty_cache()
+        out[head] = {arm: dict(median_ms=statistics.median(times[arm]), windows_ms=times[arm],
+                               peak_mib=peak[arm], launches_per_step=launches[arm])
+                     for arm in times}
+        m, n = out[head]["mlm"], out[head]["mlm_nsp"]
+        print("{}{}: mlm {:.3f} ms, mlm + nsp {:.3f} ms ({:+.3f} ms, {:+.2%}); peak MiB {:.0f} -> "
+              "{:.0f}; launches/step {} -> {}".format(
+                  head, " (P = {})".format(P) if head == "sparse" else "", m["median_ms"],
+                  n["median_ms"], n["median_ms"] - m["median_ms"],
+                  n["median_ms"] / m["median_ms"] - 1, m["peak_mib"], n["peak_mib"],
+                  m["launches_per_step"], n["launches_per_step"]), flush=True)
+    out["join_kernels"] = join_kernels(P)
+    return out
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
@@ -229,6 +314,7 @@ def main() -> None:
     ap.add_argument("--max-predictions", type=int, default=None)
     ap.add_argument("--out", type=str, default=None)
     ap.add_argument("--tie", action="store_true")
+    ap.add_argument("--nsp", action="store_true")
     args = ap.parse_args()
     if not (torch.cuda.is_available() and nat.available()):
         raise SystemExit("bench_mlm needs a GPU and the native extension")
@@ -237,8 +323,8 @@ def main() -> None:
     res = dict(card=card())
     print("card: {name}, power limit {power_limit}, max SM clock {max_sm_clock}".format(**res["card"]),
           flush=True)
-    if args.tie:
-        res["tie"] = tie_compare(args)
+    if args.tie or args.nsp:
+        res["tie" if args.tie else "nsp"] = tie_compare(args) if args.tie else nsp_compare(args)
         line = json.dumps(res)
         print(line)
         if args.out:

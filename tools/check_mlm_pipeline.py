@@ -19,6 +19,8 @@ pipelines cut at different places can be compared (dropout off => the same math 
     --tie          the decoder weight is tied to the word embeddings: on 2+ GPUs the last stage
                    holds a replica of the first stage's table; the checksum of both copies is
                    printed for every step (``tied_checksums``: [first rank's, last rank's])
+    --nsp          the pretraining head (BertTailForPreTraining: masked-LM + next-sentence
+                   prediction) with PreTrainingLoss on SynthPretrainingDataset
 """
 import argparse
 import json
@@ -44,6 +46,7 @@ def main():
     ap.add_argument("--batch", type=int, default=16)
     ap.add_argument("--max-predictions", type=int, default=None)
     ap.add_argument("--tie", action="store_true")
+    ap.add_argument("--nsp", action="store_true")
     ap.add_argument("--optim", default="SGD")
     ap.add_argument("--virtual-stages", type=int, default=1)
     ap.add_argument("--max-grad-norm", type=float, default=None)
@@ -62,7 +65,8 @@ def main():
     enc = [dict(layer_type="BertLayer_Head", config=cfg.__dict__),
            dict(layer_type="BertLayer_Body", config=cfg.__dict__),
            dict(layer_type="BertLayer_Tail", config=cfg.__dict__)] * a.layers
-    head = dict(layer_type="BertTailForMaskedLM", config=cfg.__dict__)
+    head = dict(layer_type="BertTailForPreTraining" if a.nsp else "BertTailForMaskedLM",
+                config=cfg.__dict__)
     if a.max_predictions is not None:
         head["max_predictions"] = a.max_predictions
     if a.tie:
@@ -109,12 +113,13 @@ def main():
                               grad_clip=(dict(max_norm=a.max_grad_norm)
                                          if a.max_grad_norm is not None else None))
     runner = sky.Runner(model=model, parameter_server=None, worker_manager=wm, optimizer=opt,
-                        max_epochs=1, max_iters=10 ** 9, loss_cfg=dict(type="MaskedLMLoss"),
+                        max_epochs=1, max_iters=10 ** 9, loss_cfg=dict(type="PreTrainingLoss" if a.nsp else "MaskedLMLoss"),
                         timer_cfg=dict(root="/tmp/sky_check_mlm"), logging_cfg=None,
                         micro_batches=a.micro_batches, schedule="1f1b", boundary=a.boundary,
                         device=dev)
     model.train(True)
-    ds = sky.SynthMLMDataset(num_samples=a.batch * 2, max_seq_length=128, vocab_size=30528, seed=3)
+    data_cls = sky.SynthPretrainingDataset if a.nsp else sky.SynthMLMDataset
+    ds = data_cls(num_samples=a.batch * 2, max_seq_length=128, vocab_size=30528, seed=3)
     batches = list(torch.utils.data.DataLoader(ds, batch_size=a.batch))
     losses, checksums, norms = [], [], []
     eng = runner.engine

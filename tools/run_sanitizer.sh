@@ -12,6 +12,8 @@
 #                  the shape grid, and one graph replayed with different label counts
 #         tied     the tied word-embedding gradient exchange (tied_grad_push / tied_grad_reduce)
 #                  in loopback on one GPU, and the tied masked-language-model head
+#         pretrain the pretraining head's kernels: mlm_scatter with the [CLS]-row gradient,
+#                  cls_grad_add, masked_softmax_ce, and the native head forward / backward
 #         all      everything above (default)
 # Runs on ONE GPU; reports land in bench_out/sanitizer_<tool>_<suite>.log.  The sanitizer slows
 # kernels 10-100x: the 4 s flag-wait timeouts are only meaningful under memcheck / synccheck.
@@ -44,4 +46,7 @@ case "$SUITE" in tied|all)
 esac
 case "$SUITE" in layers|all)
   run layers tests/test_layers_gpu.py tests/test_kernels_gpu.py -k "embeddings_pooler_classifier or handshake or signals_panels" ;;
+esac
+case "$SUITE" in pretrain|all)
+  run pretrain tests/test_pretraining_gpu.py -k "scatter_joins or masked_softmax_ce or native_head_matches" ;;
 esac
