@@ -321,6 +321,36 @@ void masked_softmax_ce(uintptr_t logits, int ldl, uintptr_t labels, int M, int C
                                       P<float>(loss_acc), S(stream)),
         "masked_softmax_ce");
 }
+void qa_logits_fwd(uintptr_t hidden, int B, int seq, int H, uintptr_t w, uintptr_t b,
+                   uintptr_t logits, uintptr_t stream) {
+  check(sky::launch_qa_logits_fwd(P<const void>(hidden), B, seq, H, P<const float>(w),
+                                  P<const float>(b), P<float>(logits), S(stream)),
+        "qa_logits_fwd");
+}
+void qa_logits_bwd(uintptr_t hidden, uintptr_t dlogits, int B, int seq, int H, uintptr_t w,
+                   uintptr_t dhidden, uintptr_t workspace, uintptr_t dw, uintptr_t db,
+                   uintptr_t stream) {
+  check(sky::launch_qa_logits_bwd(P<const void>(hidden), P<const float>(dlogits), B, seq, H,
+                                  P<const float>(w), P<void>(dhidden), P<float>(workspace),
+                                  P<float>(dw), P<float>(db), S(stream)),
+        "qa_logits_bwd");
+}
+void qa_span_ce(uintptr_t logits, uintptr_t labels, int B, int seq, long long ignore_index,
+                uintptr_t dlogits, float grad_scale, uintptr_t loss, uintptr_t loss_acc,
+                uintptr_t stream) {
+  check(sky::launch_qa_span_ce(P<const float>(logits), P<const int64_t>(labels), B, seq,
+                               ignore_index, P<float>(dlogits), grad_scale, P<float>(loss),
+                               P<float>(loss_acc), S(stream)),
+        "qa_span_ce");
+}
+void qa_span_eval(uintptr_t logits, uintptr_t labels, int B, int seq, int max_answer_length,
+                  long long ignore_index, uintptr_t acc, uintptr_t pred_spans,
+                  uintptr_t pred_scores, long long capacity, uintptr_t stream) {
+  check(sky::launch_qa_span_eval(P<const float>(logits), P<const int64_t>(labels), B, seq,
+                                 max_answer_length, ignore_index, P<sky::SpanEvalAccum>(acc),
+                                 P<int>(pred_spans), P<float>(pred_scores), capacity, S(stream)),
+        "qa_span_eval");
+}
 
 // descriptors: list of (p, g, mom, p_bf16, numel) -> packed host bytes to upload once
 py::bytes pack_sgd_descriptors(
@@ -615,6 +645,22 @@ PYBIND11_MODULE(_cuda, m) {
         py::arg("grad_scale") = 1.f, py::arg("loss") = 0, py::arg("loss_acc") = 0,
         py::arg("stream") = 0);
   m.def("mlm_max_predictions", []() { return sky::kMlmMaxPredictions; });
+  m.def("qa_logits_fwd", &qa_logits_fwd, py::arg("hidden"), py::arg("B"), py::arg("S"),
+        py::arg("H"), py::arg("w"), py::arg("b"), py::arg("logits"), py::arg("stream") = 0);
+  m.def("qa_logits_bwd", &qa_logits_bwd, py::arg("hidden"), py::arg("dlogits"), py::arg("B"),
+        py::arg("S"), py::arg("H"), py::arg("w"), py::arg("dhidden"), py::arg("workspace"),
+        py::arg("dw"), py::arg("db"), py::arg("stream") = 0);
+  m.def("qa_logits_bwd_workspace_bytes", [](int B, int seq, int H) {
+    return sky::qa_logits_bwd_workspace_bytes(B, seq, H);
+  });
+  m.def("qa_span_ce", &qa_span_ce, py::arg("logits"), py::arg("labels"), py::arg("B"),
+        py::arg("S"), py::arg("ignore_index"), py::arg("dlogits"), py::arg("grad_scale") = 1.f,
+        py::arg("loss") = 0, py::arg("loss_acc") = 0, py::arg("stream") = 0);
+  m.def("qa_span_eval", &qa_span_eval, py::arg("logits"), py::arg("labels"), py::arg("B"),
+        py::arg("S"), py::arg("max_answer_length"), py::arg("ignore_index"), py::arg("acc"),
+        py::arg("pred_spans"), py::arg("pred_scores"), py::arg("capacity"),
+        py::arg("stream") = 0);
+  m.def("qa_span_eval_accum_bytes", []() { return sizeof(sky::SpanEvalAccum); });
   m.def("pack_sgd_descriptors", &pack_sgd_descriptors);
   m.def("sgd_multi", &sgd_multi, py::arg("d_tensors"), py::arg("n"), py::arg("max_numel"),
         py::arg("lr"), py::arg("momentum") = 0.f, py::arg("weight_decay") = 0.f,

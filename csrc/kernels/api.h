@@ -326,6 +326,61 @@ int launch_masked_softmax_ce(const float* logits, int ldl, const int64_t* labels
                              long long ignore_index, float* dlogits, float grad_scale,
                              float* loss, float* loss_acc, cudaStream_t stream);
 
+// Question-answering span head (HF BertForQuestionAnswering's qa_outputs = Linear(H, 2)).
+// logits / dlogits are fp32 [B, 2, S]: row 2b holds sequence b's start logits, row 2b + 1 its end
+// logits.  labels are int64 [B, kQaLabelCols] per sequence: start, end (the gold answer's first and
+// last token), start_lo, start_hi (where a predicted answer may start), end_hi (the last position
+// where it may end).  All four kernels use fixed reduction orders and no float atomics (two calls
+// or graph replays give identical bits) and never synchronise with the host.
+// Errors: 990 bad shape (B, S >= 1, H a positive multiple of 8, B * S within int range,
+// max_answer_length >= 1, capacity >= 0), 991 null pointer, 992 hidden / dhidden / w not 16-byte
+// aligned.
+constexpr int kQaLabelCols = 5;
+constexpr int kQaRowsPerCta = 128;  // rows of one partial dW / db in qa_logits_bwd
+// logits[b, c, s] = dot(hidden[b*S + s], w[c]) + bias[c] (hidden bf16 [B*S, H], w fp32 [2, H]).
+// One launch.
+int launch_qa_logits_fwd(const void* hidden, int B, int S, int H, const float* w, const float* b,
+                         float* logits, cudaStream_t stream);
+// dhidden[r] = g[b, 0, s] * w[0] + g[b, 1, s] * w[1] (bf16, every row written once), dw [2, H] +=
+// sum_r g_c[r] hidden[r], db [2] += sum_r g_c[r].  The first launch stores per-128-row partials in
+// `workspace` (qa_logits_bwd_workspace_bytes), the second adds them in row-block order (fp64).
+int launch_qa_logits_bwd(const void* hidden, const float* dlogits, int B, int S, int H,
+                         const float* w, void* dhidden, float* workspace, float* dw, float* db,
+                         cudaStream_t stream);
+size_t qa_logits_bwd_workspace_bytes(int B, int S, int H);
+// Span loss: (mean start CE + mean end CE) / 2, each mean over the sequences whose label is in
+// [0, S) (0 without one).  dlogits = d(loss * grad_scale)/dlogits, an exact 0 on a row whose label
+// is ignore_index or invalid; any label neither ignore_index nor in [0, S) makes the loss NaN and
+// is never used as an index.  loss[0] = the loss, loss_acc[0] += loss * grad_scale (either may be
+// null).  One CTA, one launch.
+int launch_qa_span_ce(const float* logits, const int64_t* labels, int B, int S,
+                      long long ignore_index, float* dlogits, float grad_scale, float* loss,
+                      float* loss_acc, cudaStream_t stream);
+// Evaluation accumulator of a span head.  Totals over the sequences whose gold start and end are
+// both in [0, S); `invalid` counts sequences with a gold label that is neither ignore_index nor in
+// [0, S).  Predictions go to pred_spans[cursor + b] / pred_scores[cursor + b] while that is below
+// the capacity (else `overflow` is counted); the cursor lives here, so a replayed graph appends.
+struct SpanEvalAccum {
+  double start_loss_sum;           // lse - logit[gold] of the start rows (fp32 rows, fp64 sum)
+  double end_loss_sum;
+  double f1_sum;                   // SQuAD token F1 of the best span against the gold interval
+  unsigned long long count;
+  unsigned long long start_correct;  // argmax (first maximum, NaN is the maximum) == gold start
+  unsigned long long end_correct;
+  unsigned long long exact;          // best span == gold span
+  unsigned long long invalid;
+  unsigned long long cursor;         // sequences seen since the last reset
+  unsigned long long overflow;       // of them, not stored: past the capacity
+};
+// Best span of each sequence: the maximum of start[i] + end[j] (one fp32 add; NaN counts as -inf)
+// over max(start_lo, 0) <= i <= min(start_hi, S - 1), i <= j <= min(i + L - 1, end_hi, S - 1);
+// among equal scores the smallest (i, j) wins; an empty range gives (-1, -1) and score -inf.
+// pred_spans int32 [capacity, 2], pred_scores fp32 [capacity].  One CTA, one launch.
+int launch_qa_span_eval(const float* logits, const int64_t* labels, int B, int S,
+                        int max_answer_length, long long ignore_index, SpanEvalAccum* acc,
+                        int* pred_spans, float* pred_scores, long long capacity,
+                        cudaStream_t stream);
+
 // ---------------------------------------------------------------------------------------------
 // Optimizer / parameter maintenance
 // ---------------------------------------------------------------------------------------------

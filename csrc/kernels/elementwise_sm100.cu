@@ -1169,6 +1169,421 @@ masked_softmax_ce_kernel(const float* __restrict__ logits, int ldl,
 }
 
 // ------------------------------------------------------------------------------------------
+// Question-answering span head (HF BertForQuestionAnswering: qa_outputs = Linear(H, 2)).
+//   qa_logits_fwd_kernel       one warp per row: the bf16 row (16-byte loads) dotted with w[0]
+//                              and w[1] in fp32, plus the bias, stored as logits [B, 2, S]
+//   qa_logits_bwd_kernel       CTA (x, y) owns 256 columns of rows [y * 128, (y + 1) * 128):
+//                              dhidden = g0 w0 + g1 w1 (bf16, every row written once) and that
+//                              row range's partial dW [2, H] / db [2]
+//   qa_logits_finalize_kernel  the partials summed in row-block order (fp64), added into dW / db
+//   qa_span_ce_kernel          one CTA: the span loss and its [B, 2, S] gradient
+//   qa_span_eval_kernel        one CTA: best span per row, totals, predictions at a device cursor
+// Warp reductions use one fixed xor pattern and every float sum a fixed order, no float atomics:
+// two calls or graph replays give identical bits.
+// ------------------------------------------------------------------------------------------
+constexpr int kQaFwdWarps = 8;
+constexpr int kQaColChunks = 32;  // bwd CTA: 32 x 8 threads, 32 16-byte chunks = 256 columns
+constexpr int kQaRowLanes = 8;
+constexpr int kQaRowUnroll = 4;   // rows a bwd thread loads before it computes
+constexpr int kQaWarps = 16;      // span_ce / span_eval: one CTA of 16 warps
+constexpr int kQaChunk = 256;     // rows per fixed-order fp64 reduction chunk
+
+__device__ __forceinline__ void unpack_bf16x8(const uint4& u, float* x) {
+  const float2 f0 = unpack_bf16x2(u.x), f1 = unpack_bf16x2(u.y);
+  const float2 f2 = unpack_bf16x2(u.z), f3 = unpack_bf16x2(u.w);
+  x[0] = f0.x;
+  x[1] = f0.y;
+  x[2] = f1.x;
+  x[3] = f1.y;
+  x[4] = f2.x;
+  x[5] = f2.y;
+  x[6] = f3.x;
+  x[7] = f3.y;
+}
+
+__global__ void __launch_bounds__(kQaFwdWarps * 32)
+qa_logits_fwd_kernel(const uint4* __restrict__ hidden, long long R, int S, int H8,
+                     const float* __restrict__ w, const float* __restrict__ bias,
+                     float* __restrict__ logits) {
+  const int lane = threadIdx.x & 31;
+  const long long H = static_cast<long long>(H8) * 8;
+  const float b0 = bias[0], b1 = bias[1];
+  for (long long r = static_cast<long long>(blockIdx.x) * kQaFwdWarps + (threadIdx.x >> 5); r < R;
+       r += static_cast<long long>(gridDim.x) * kQaFwdWarps) {
+    const uint4* x = hidden + r * H8;
+    float s0 = 0.f, s1 = 0.f;
+#pragma unroll 2
+    for (int v = lane; v < H8; v += 32) {
+      float xf[8];
+      unpack_bf16x8(x[v], xf);
+      const float4* w0 = reinterpret_cast<const float4*>(w + v * 8);
+      const float4* w1 = reinterpret_cast<const float4*>(w + H + v * 8);
+      const float4 a0 = w0[0], a1 = w0[1], c0 = w1[0], c1 = w1[1];
+      s0 += xf[0] * a0.x + xf[1] * a0.y + xf[2] * a0.z + xf[3] * a0.w +
+            xf[4] * a1.x + xf[5] * a1.y + xf[6] * a1.z + xf[7] * a1.w;
+      s1 += xf[0] * c0.x + xf[1] * c0.y + xf[2] * c0.z + xf[3] * c0.w +
+            xf[4] * c1.x + xf[5] * c1.y + xf[6] * c1.z + xf[7] * c1.w;
+    }
+    s0 = warp_sum(s0);
+    s1 = warp_sum(s1);
+    if (lane == 0) {
+      const long long b = r / S, s = r - b * S;
+      logits[b * 2 * S + s] = s0 + b0;
+      logits[b * 2 * S + S + s] = s1 + b1;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kQaColChunks * kQaRowLanes)
+qa_logits_bwd_kernel(const uint4* __restrict__ hidden, const float* __restrict__ g, long long R,
+                     int S, int H8, const float* __restrict__ w, uint4* __restrict__ dhidden,
+                     float* __restrict__ partial) {
+  __shared__ float red[kQaRowLanes][16][kQaColChunks];
+  __shared__ float redb[kQaRowLanes][2];
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  const int c8 = blockIdx.x * kQaColChunks + tx;
+  const bool col_ok = c8 < H8;
+  const long long H = static_cast<long long>(H8) * 8;
+  float w0[8], w1[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    w0[i] = col_ok ? w[c8 * 8 + i] : 0.f;
+    w1[i] = col_ok ? w[H + c8 * 8 + i] : 0.f;
+  }
+  float a0[8], a1[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) a0[i] = a1[i] = 0.f;
+  float gb0 = 0.f, gb1 = 0.f;
+  const long long r0 = static_cast<long long>(blockIdx.y) * kQaRowsPerCta;
+  const long long r1 = r0 + kQaRowsPerCta < R ? r0 + kQaRowsPerCta : R;
+  for (long long rb = r0 + ty; rb < r1; rb += kQaRowLanes * kQaRowUnroll) {
+    uint4 u[kQaRowUnroll];
+    float g0[kQaRowUnroll], g1[kQaRowUnroll];
+#pragma unroll
+    for (int k = 0; k < kQaRowUnroll; ++k) {
+      const long long r = rb + k * kQaRowLanes;
+      g0[k] = g1[k] = 0.f;
+      u[k] = make_uint4(0u, 0u, 0u, 0u);
+      if (r < r1) {
+        const long long b = r / S, s = r - b * S;
+        g0[k] = g[b * 2 * S + s];
+        g1[k] = g[b * 2 * S + S + s];
+        if (col_ok) u[k] = hidden[r * H8 + c8];
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < kQaRowUnroll; ++k) {
+      const long long r = rb + k * kQaRowLanes;
+      if (r >= r1) continue;
+      gb0 += g0[k];
+      gb1 += g1[k];
+      if (!col_ok) continue;
+      float x[8], d[8];
+      unpack_bf16x8(u[k], x);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        a0[i] = fmaf(g0[k], x[i], a0[i]);
+        a1[i] = fmaf(g1[k], x[i], a1[i]);
+        // g0 w0 + g1 w1 with the first product's rounding error added back, so that the one
+        // rounding to bf16 is the only one that matters even when the two terms cancel
+        const float p = __fmul_rn(g0[k], w0[i]);
+        const float e = __fmaf_rn(g0[k], w0[i], -p);
+        d[i] = __fadd_rn(__fmaf_rn(g1[k], w1[i], p), e);
+      }
+      dhidden[r * H8 + c8] = make_uint4(pack_bf16x2(d[0], d[1]), pack_bf16x2(d[2], d[3]),
+                                        pack_bf16x2(d[4], d[5]), pack_bf16x2(d[6], d[7]));
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    red[ty][i][tx] = a0[i];
+    red[ty][8 + i][tx] = a1[i];
+  }
+  if (tx == 0) {
+    redb[ty][0] = gb0;
+    redb[ty][1] = gb1;
+  }
+  __syncthreads();
+  float* out = partial + static_cast<long long>(blockIdx.y) * (2 * H + 2);
+  for (int i = ty * kQaColChunks + tx; i < 16 * kQaColChunks; i += kQaColChunks * kQaRowLanes) {
+    const int k = i / kQaColChunks, t = i - k * kQaColChunks;
+    float s = 0.f;
+#pragma unroll
+    for (int y = 0; y < kQaRowLanes; ++y) s += red[y][k][t];
+    const int cc = blockIdx.x * kQaColChunks + t;
+    if (cc < H8) out[(k / 8) * H + cc * 8 + (k % 8)] = s;
+  }
+  if (blockIdx.x == 0 && ty == 0 && tx < 2) {
+    float s = 0.f;
+#pragma unroll
+    for (int y = 0; y < kQaRowLanes; ++y) s += redb[y][tx];
+    out[2 * H + tx] = s;
+  }
+}
+
+// column i of the partials [n_blocks, n]: lane y of a 32 x 8 CTA sums blocks y, y + 8, ... in
+// order, then the 8 lane sums are added in lane order
+__global__ void __launch_bounds__(kQaColChunks * kQaRowLanes)
+qa_logits_finalize_kernel(const float* __restrict__ partial, int n_blocks, int H,
+                          float* __restrict__ dw, float* __restrict__ db) {
+  __shared__ double red[kQaRowLanes][kQaColChunks];
+  const int n = 2 * H + 2;
+  const int i = blockIdx.x * kQaColChunks + threadIdx.x;
+  double s = 0.0;
+  if (i < n) {
+#pragma unroll 4
+    for (int k = threadIdx.y; k < n_blocks; k += kQaRowLanes)
+      s += static_cast<double>(partial[static_cast<long long>(k) * n + i]);
+  }
+  red[threadIdx.y][threadIdx.x] = s;
+  __syncthreads();
+  if (threadIdx.y == 0 && i < n) {
+    double t = 0.0;
+#pragma unroll
+    for (int y = 0; y < kQaRowLanes; ++y) t += red[y][threadIdx.x];
+    if (i < 2 * H) dw[i] += static_cast<float>(t);
+    else db[i - 2 * H] += static_cast<float>(t);
+  }
+}
+
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// sums[0..n_arr) of the chunk's per-row values, a fixed tree over kQaChunk entries each
+__device__ __forceinline__ void qa_chunk_tree(double (*vals)[kQaChunk], int n_arr) {
+  for (int s = kQaChunk / 2; s > 0; s >>= 1) {
+    for (int i = threadIdx.x; i < n_arr * s; i += blockDim.x) {
+      const int a = i / s, j = i - a * s;
+      vals[a][j] += vals[a][j + s];
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(kQaWarps * 32)
+qa_span_ce_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels, int B,
+                  int S, long long ignore_index, float* __restrict__ dlogits, float grad_scale,
+                  float* __restrict__ loss, float* __restrict__ loss_acc) {
+  __shared__ double row_loss[1][kQaChunk];
+  __shared__ int cnt[3];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x < 3) cnt[threadIdx.x] = 0;
+  __syncthreads();
+  int n0 = 0, n1 = 0, nbad = 0;
+  for (int i = threadIdx.x; i < 2 * B; i += blockDim.x) {
+    const long long lab = labels[static_cast<long long>(i >> 1) * kQaLabelCols + (i & 1)];
+    if (lab == ignore_index) continue;
+    if (lab < 0 || lab >= S) ++nbad;
+    else if (i & 1) ++n1;
+    else ++n0;
+  }
+  // integer atomics: the counts do not depend on the order
+  if (n0) atomicAdd(&cnt[0], n0);
+  if (n1) atomicAdd(&cnt[1], n1);
+  if (nbad) atomicAdd(&cnt[2], nbad);
+  __syncthreads();
+  const int n_start = cnt[0], n_end = cnt[1];
+  const float scale0 = n_start > 0 ? grad_scale / (2.f * static_cast<float>(n_start)) : 0.f;
+  const float scale1 = n_end > 0 ? grad_scale / (2.f * static_cast<float>(n_end)) : 0.f;
+  double total = 0.0;
+  for (int base = 0; base < 2 * B; base += kQaChunk) {
+    for (int rr = warp; rr < kQaChunk; rr += kQaWarps) {
+      const int row = base + rr;  // row 2b: start logits of sequence b, 2b + 1: end logits
+      double contrib = 0.0;
+      if (row < 2 * B) {
+        const float* l = logits + static_cast<long long>(row) * S;
+        float* d = dlogits + static_cast<long long>(row) * S;
+        const long long lab = labels[static_cast<long long>(row >> 1) * kQaLabelCols + (row & 1)];
+        if (lab == ignore_index || lab < 0 || lab >= S) {
+          for (int s = lane; s < S; s += 32) d[s] = 0.f;
+        } else {
+          float mx = -INFINITY;
+          for (int s = lane; s < S; s += 32) mx = fmaxf(mx, l[s]);
+          mx = warp_max(mx);
+          float se = 0.f;
+          for (int s = lane; s < S; s += 32) se += expf(l[s] - mx);
+          se = warp_sum(se);
+          const float lse = mx + logf(se);
+          const float sc = (row & 1) ? scale1 : scale0;
+          for (int s = lane; s < S; s += 32)
+            d[s] = (expf(l[s] - lse) - (s == lab ? 1.f : 0.f)) * sc;
+          contrib = static_cast<double>(lse - l[lab]) / ((row & 1) ? n_end : n_start);
+        }
+      }
+      if (lane == 0) row_loss[0][rr] = contrib;
+    }
+    __syncthreads();
+    qa_chunk_tree(row_loss, 1);
+    if (threadIdx.x == 0) total += row_loss[0][0];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    float mean = static_cast<float>(total * 0.5);
+    if (cnt[2] > 0) mean = __int_as_float(0x7fc00000);  // NaN: an invalid label is never silent
+    if (loss != nullptr) loss[0] = mean;
+    if (loss_acc != nullptr) loss_acc[0] += mean * grad_scale;
+  }
+}
+
+// (v, i, j) is a better span than (w, k, l): a higher score, then the smaller (i, j); i < 0 marks
+// "no candidate"
+__device__ __forceinline__ bool qa_span_better(float v, int i, int j, float w, int k, int l) {
+  if (i < 0) return false;
+  if (k < 0) return true;
+  return v > w || (v == w && (i < k || (i == k && j < l)));
+}
+
+// argmax (eval_better: first maximum, NaN is the maximum) and lse of one row, warp-wide
+__device__ __forceinline__ void qa_row_stats(const float* __restrict__ l, int S, int lane,
+                                             int* arg_out, float* lse_out) {
+  float mx = -INFINITY;
+  int arg = S;
+  for (int c = lane; c < S; c += 32) {
+    const float v = l[c];
+    if (arg == S || eval_better(v, c, mx, arg)) {
+      mx = v;
+      arg = c;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float omx = __shfl_xor_sync(0xffffffffu, mx, o);
+    const int oarg = __shfl_xor_sync(0xffffffffu, arg, o);
+    if (oarg < S && (arg == S || eval_better(omx, oarg, mx, arg))) {
+      mx = omx;
+      arg = oarg;
+    }
+  }
+  float se = 0.f;
+  for (int c = lane; c < S; c += 32) se += expf(l[c] - mx);
+  se = warp_sum(se);
+  *arg_out = arg;
+  *lse_out = mx + logf(se);
+}
+
+__global__ void __launch_bounds__(kQaWarps * 32)
+qa_span_eval_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels, int B,
+                    int S, int L, long long ignore_index, SpanEvalAccum* __restrict__ acc,
+                    int* __restrict__ pred_spans, float* __restrict__ pred_scores,
+                    long long capacity) {
+  __shared__ double vals[3][kQaChunk];  // start CE, end CE, F1 of the chunk's rows
+  __shared__ unsigned long long cursor;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) cursor = acc->cursor;
+  __syncthreads();
+  unsigned long long counted = 0, start_ok = 0, end_ok = 0, exact = 0, invalid = 0, overflow = 0;
+  double tot[3] = {0.0, 0.0, 0.0};
+  for (int base = 0; base < B; base += kQaChunk) {
+    for (int rr = warp; rr < kQaChunk; rr += kQaWarps) {
+      const int b = base + rr;
+      double ce_s = 0.0, ce_e = 0.0, f1 = 0.0;
+      if (b < B) {
+        const float* st = logits + static_cast<long long>(b) * 2 * S;
+        const float* en = st + S;
+        const int64_t* lab = labels + static_cast<long long>(b) * kQaLabelCols;
+        const long long gs = lab[0], ge = lab[1];
+        // the search range, clipped to the row: a padded row (ignore_index) is empty
+        const long long lo = lab[2] > 0 ? lab[2] : 0;
+        const long long hi = lab[3] < S - 1 ? lab[3] : S - 1;
+        const long long ehi = lab[4] < S - 1 ? lab[4] : S - 1;
+        float best = -INFINITY;
+        int bi = -1, bj = -1;
+        for (long long i = lo + lane; i <= hi; i += 32) {
+          const float si = st[i];
+          const long long jmax = i + L - 1 < ehi ? i + L - 1 : ehi;
+          for (long long j = i; j <= jmax; ++j) {
+            float v = si + en[j];
+            if (v != v) v = -INFINITY;
+            // i and j ascend within a lane: only a strictly higher score replaces the candidate
+            if (bi < 0 || v > best) {
+              best = v;
+              bi = static_cast<int>(i);
+              bj = static_cast<int>(j);
+            }
+          }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+          const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+          const int oj = __shfl_xor_sync(0xffffffffu, bj, o);
+          if (qa_span_better(ov, oi, oj, best, bi, bj)) {
+            best = ov;
+            bi = oi;
+            bj = oj;
+          }
+        }
+        if (lane == 0) {
+          const unsigned long long slot = cursor + static_cast<unsigned long long>(b);
+          if (slot < static_cast<unsigned long long>(capacity)) {
+            pred_spans[2 * slot] = bi;
+            pred_spans[2 * slot + 1] = bj;
+            pred_scores[slot] = best;
+          } else {
+            ++overflow;
+          }
+        }
+        const bool ok_s = gs >= 0 && gs < S, ok_e = ge >= 0 && ge < S;
+        if ((gs != ignore_index && !ok_s) || (ge != ignore_index && !ok_e)) {
+          if (lane == 0) ++invalid;
+        } else if (ok_s && ok_e) {
+          int arg_s, arg_e;
+          float lse_s, lse_e;
+          qa_row_stats(st, S, lane, &arg_s, &lse_s);
+          qa_row_stats(en, S, lane, &arg_e, &lse_e);
+          ce_s = static_cast<double>(lse_s - st[gs]);
+          ce_e = static_cast<double>(lse_e - en[ge]);
+          // SQuAD's token F1 on position intervals: overlap / predicted and overlap / gold length
+          const long long ov_hi = bj < ge ? bj : ge, ov_lo = bi > gs ? bi : gs;
+          const long long overlap = ov_hi - ov_lo + 1;
+          if (bi >= 0 && overlap > 0) {
+            const double p = static_cast<double>(overlap) / static_cast<double>(bj - bi + 1);
+            const double r = static_cast<double>(overlap) / static_cast<double>(ge - gs + 1);
+            f1 = 2.0 * p * r / (p + r);
+          }
+          if (lane == 0) {
+            ++counted;
+            start_ok += arg_s == gs ? 1 : 0;
+            end_ok += arg_e == ge ? 1 : 0;
+            exact += (bi == gs && bj == ge) ? 1 : 0;
+          }
+        }
+      }
+      if (lane == 0) {
+        vals[0][rr] = ce_s;
+        vals[1][rr] = ce_e;
+        vals[2][rr] = f1;
+      }
+    }
+    __syncthreads();
+    qa_chunk_tree(vals, 3);
+    if (threadIdx.x == 0) {
+      tot[0] += vals[0][0];
+      tot[1] += vals[1][0];
+      tot[2] += vals[2][0];
+    }
+    __syncthreads();
+  }
+  if (lane == 0) {
+    if (counted) atomicAdd(&acc->count, counted);
+    if (start_ok) atomicAdd(&acc->start_correct, start_ok);
+    if (end_ok) atomicAdd(&acc->end_correct, end_ok);
+    if (exact) atomicAdd(&acc->exact, exact);
+    if (invalid) atomicAdd(&acc->invalid, invalid);
+    if (overflow) atomicAdd(&acc->overflow, overflow);
+  }
+  if (threadIdx.x == 0) {
+    acc->start_loss_sum += tot[0];
+    acc->end_loss_sum += tot[1];
+    acc->f1_sum += tot[2];
+    acc->cursor = cursor + static_cast<unsigned long long>(B);
+  }
+}
+
+// ------------------------------------------------------------------------------------------
 // Optimizer
 // ------------------------------------------------------------------------------------------
 // kScalars: lr and the clip coefficient come from the device-side OptimScalars (schedule / global
@@ -2045,6 +2460,78 @@ int launch_masked_softmax_ce(const float* logits, int ldl, const int64_t* labels
   if (M > 0 && (!logits || !labels || !dlogits)) return 986;
   masked_softmax_ce_kernel<<<1, kMaskedCeThreads, 0, stream>>>(
       logits, ldl, labels, M, C, ignore_index, dlogits, grad_scale, loss, loss_acc);
+  SKY_LAUNCH_CHECK();
+}
+
+namespace {
+bool qa_shape_ok(int B, int S, int H) {
+  return B >= 1 && S >= 1 && H >= 8 && H % 8 == 0 &&
+         static_cast<long long>(B) * S <= 0x7fffffffLL;
+}
+}  // namespace
+
+size_t qa_logits_bwd_workspace_bytes(int B, int S, int H) {
+  if (!qa_shape_ok(B, S, H)) return 0;
+  const long long R = static_cast<long long>(B) * S;
+  const long long blocks = (R + kQaRowsPerCta - 1) / kQaRowsPerCta;
+  return static_cast<size_t>(blocks * (2LL * H + 2) * sizeof(float));
+}
+
+int launch_qa_logits_fwd(const void* hidden, int B, int S, int H, const float* w,
+                         const float* b, float* logits, cudaStream_t stream) {
+  if (!qa_shape_ok(B, S, H)) return 990;
+  if (!hidden || !w || !b || !logits) return 991;
+  if (!aligned16(hidden) || !aligned16(w)) return 992;
+  const long long R = static_cast<long long>(B) * S;
+  const int grid = grid_for_rows(static_cast<int>(R), kQaFwdWarps, num_sms() * 16);
+  qa_logits_fwd_kernel<<<grid, kQaFwdWarps * 32, 0, stream>>>(
+      static_cast<const uint4*>(hidden), R, S, H / 8, w, b, logits);
+  SKY_LAUNCH_CHECK();
+}
+
+int launch_qa_logits_bwd(const void* hidden, const float* dlogits, int B, int S, int H,
+                         const float* w, void* dhidden, float* workspace, float* dw, float* db,
+                         cudaStream_t stream) {
+  if (!qa_shape_ok(B, S, H)) return 990;
+  if (!hidden || !dlogits || !w || !dhidden || !workspace || !dw || !db) return 991;
+  if (!aligned16(hidden) || !aligned16(dhidden)) return 992;
+  const long long R = static_cast<long long>(B) * S;
+  const int row_blocks = static_cast<int>((R + kQaRowsPerCta - 1) / kQaRowsPerCta);
+  const int H8 = H / 8;
+  dim3 grid((H8 + kQaColChunks - 1) / kQaColChunks, row_blocks);
+  qa_logits_bwd_kernel<<<grid, dim3(kQaColChunks, kQaRowLanes), 0, stream>>>(
+      static_cast<const uint4*>(hidden), dlogits, R, S, H8, w, static_cast<uint4*>(dhidden),
+      workspace);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return static_cast<int>(e);
+  const int n = 2 * H + 2;
+  qa_logits_finalize_kernel<<<(n + kQaColChunks - 1) / kQaColChunks,
+                              dim3(kQaColChunks, kQaRowLanes), 0, stream>>>(workspace, row_blocks,
+                                                                             H, dw, db);
+  SKY_LAUNCH_CHECK();
+}
+
+int launch_qa_span_ce(const float* logits, const int64_t* labels, int B, int S,
+                      long long ignore_index, float* dlogits, float grad_scale, float* loss,
+                      float* loss_acc, cudaStream_t stream) {
+  if (B < 1 || S < 1 || static_cast<long long>(B) * S > 0x3fffffffLL) return 990;
+  if (!logits || !labels || !dlogits) return 991;
+  qa_span_ce_kernel<<<1, kQaWarps * 32, 0, stream>>>(logits, labels, B, S, ignore_index, dlogits,
+                                                     grad_scale, loss, loss_acc);
+  SKY_LAUNCH_CHECK();
+}
+
+int launch_qa_span_eval(const float* logits, const int64_t* labels, int B, int S,
+                        int max_answer_length, long long ignore_index, SpanEvalAccum* acc,
+                        int* pred_spans, float* pred_scores, long long capacity,
+                        cudaStream_t stream) {
+  if (B < 1 || S < 1 || max_answer_length < 1 || capacity < 0 ||
+      static_cast<long long>(B) * S > 0x3fffffffLL)
+    return 990;
+  if (!logits || !labels || !acc || (capacity > 0 && (!pred_spans || !pred_scores))) return 991;
+  qa_span_eval_kernel<<<1, kQaWarps * 32, 0, stream>>>(logits, labels, B, S, max_answer_length,
+                                                       ignore_index, acc, pred_spans, pred_scores,
+                                                       capacity);
   SKY_LAUNCH_CHECK();
 }
 

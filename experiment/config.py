@@ -43,10 +43,16 @@ TINY = os.getenv("TINY", "0") == "1"                          # shrink the geome
 # learnable SynthMLMDataset with a BertTailForMaskedLM head and MaskedLMLoss; the vocabulary is
 # padded to a multiple of 8 (30522 -> 30528) for the head's GEMMs.  TASK=pretrain: BERT's masked-LM
 # + next-sentence pretraining on SynthPretrainingDataset with a BertTailForPreTraining head and
-# PreTrainingLoss (same vocabulary padding).  Default: classification
+# PreTrainingLoss (same vocabulary padding).  TASK=squad: extractive question answering with a
+# BertTailForQuestionAnswering head and QuestionAnsweringLoss on the learnable SynthQADataset, or
+# on SQuAD v1.1 with SQUAD_TRAIN=train.json, VOCAB_FILE=vocab.txt (and SQUAD_DEV=dev.json for the
+# evaluation); SEQ_LEN defaults to 384 there.  Default: classification
 TASK = os.getenv("TASK", "cls")
-if TASK not in ("cls", "mlm", "pretrain"):
-    raise ValueError("TASK must be 'cls', 'mlm' or 'pretrain', got {!r}".format(TASK))
+if TASK not in ("cls", "mlm", "pretrain", "squad"):
+    raise ValueError("TASK must be 'cls', 'mlm', 'pretrain' or 'squad', got {!r}".format(TASK))
+SQUAD_TRAIN = os.getenv("SQUAD_TRAIN")
+SQUAD_DEV = os.getenv("SQUAD_DEV")
+VOCAB_FILE = os.getenv("VOCAB_FILE")
 # SAVE_PATH=dir: save a checkpoint into dir after every epoch; INIT_FROM=path: initialise the
 # weights from a checkpoint of a pretraining run (TASK=mlm or pretrain), e.g. to fine-tune
 # TASK=cls from it: the encoder (and the pooler of a pretraining head) load, the rest keeps its
@@ -72,7 +78,7 @@ _config = BertConfig.bert_large()                              # wwm_uncased_L-2
 if TINY:
     _config = BertConfig(1000, hidden_size=64, num_hidden_layers=LAYER_NUM, num_attention_heads=4,
                          intermediate_size=128, max_position_embeddings=128)
-_SEQ = int(os.getenv("SEQ_LEN", "128" if not TINY else "16"))
+_SEQ = int(os.getenv("SEQ_LEN", ("384" if TASK == "squad" else "128") if not TINY else "16"))
 if TASK in ("mlm", "pretrain") or INIT_FROM:
     # the masked-LM heads' GEMMs need a multiple of 8; a model initialised from such a run has
     # to match its padded word-embedding table
@@ -97,6 +103,8 @@ if TASK in ("mlm", "pretrain"):
         _TAIL[0]["max_predictions"] = MLM_MAX_PREDICTIONS
     if MLM_TIE:
         _TAIL[0]["tie_word_embeddings"] = True
+if TASK == "squad":
+    _TAIL = [dict(layer_type="BertTailForQuestionAnswering", config=_config.__dict__)]
 
 model_config = [dict(layer_type="BertEmbeddings", config=_config.__dict__)] + _ENCODER + _TAIL
 
@@ -138,6 +146,25 @@ if TASK in ("mlm", "pretrain"):
         data_config["eval_datasets"] = dict(
             dev=dict(type=_DATA, num_samples=EVAL_SAMPLES, max_seq_length=_SEQ,
                      vocab_size=_config.vocab_size, seed=1))
+elif TASK == "squad":
+    if SQUAD_TRAIN:
+        if not VOCAB_FILE:
+            raise ValueError("SQUAD_TRAIN needs VOCAB_FILE (the WordPiece vocabulary)")
+        data_config["dataset_cfg"] = dict(type="SquadDataset", json_file=SQUAD_TRAIN,
+                                          vocab_file=VOCAB_FILE, max_seq_length=_SEQ, split="train")
+    else:
+        data_config["dataset_cfg"] = dict(type="SynthQADataset", num_samples=BATCH_SIZE * (MAX_ITERS + 2),
+                                          max_seq_length=_SEQ, vocab_size=_config.vocab_size, seed=0)
+    if EVAL_EVERY is not None:
+        if SQUAD_DEV:
+            if not VOCAB_FILE:
+                raise ValueError("SQUAD_DEV needs VOCAB_FILE (the WordPiece vocabulary)")
+            _dev = dict(type="SquadDataset", json_file=SQUAD_DEV, vocab_file=VOCAB_FILE,
+                        max_seq_length=_SEQ, split="dev")
+        else:
+            _dev = dict(type="SynthQADataset", num_samples=EVAL_SAMPLES, max_seq_length=_SEQ,
+                        vocab_size=_config.vocab_size, seed=1)
+        data_config["eval_datasets"] = dict(dev=_dev)
 elif EVAL_EVERY is not None:
     # a learnable task (label = first token after [CLS] mod 3) for training and the held-out split,
     # so that the dev accuracy measures something; random labels stay at chance
@@ -180,7 +207,8 @@ train_config = dict(
     lr_schedule_cfg=(dict(type=LR_SCHEDULE, warmup_steps=WARMUP_STEPS, total_steps=TOTAL_STEPS)
                      if LR_SCHEDULE else None),
     grad_clip_cfg=dict(max_norm=MAX_GRAD_NORM) if MAX_GRAD_NORM is not None else None,
-    loss_cfg=dict(type=dict(mlm="MaskedLMLoss", pretrain="PreTrainingLoss").get(TASK, "CrossEntropyLoss")),
+    loss_cfg=dict(type=dict(mlm="MaskedLMLoss", pretrain="PreTrainingLoss",
+                            squad="QuestionAnsweringLoss").get(TASK, "CrossEntropyLoss")),
     runner_cfg=dict(max_epochs=1, max_iters=MAX_ITERS, micro_batches=MICRO_BATCHES),
     hook_config=[dict(type="StopHook", root=_LOG_ROOT), dict(type="DistributedTimerHelperHook")]
     # REALLOCATE_EVERY=N: re-benchmark the devices and re-run the allocator every N iterations,

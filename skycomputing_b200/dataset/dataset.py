@@ -3,6 +3,7 @@
 * ``SynthMNLIDataset`` - synthetic MNLI-shaped data (three int64 ``[S]`` tensors + a label in
   ``num_classes``): the workload of every benchmark here (there is no network for GLUE).
 * ``SynthMLMDataset`` - a learnable synthetic masked-language-model task (labels ``[S]``).
+* ``SynthQADataset`` - a learnable synthetic extractive question-answering task (labels ``[5]``).
 * ``RandomMlpDataset`` / ``CIFAR10Dataset`` - parity with scaelum/dataset/dataset.py:14-48.
 """
 from __future__ import annotations
@@ -210,6 +211,65 @@ class SynthPretrainingDataset(Dataset):
         return pretraining_item(a.tolist(), b.tolist(), int(self.nsp[idx]), S, self.cls_id,
                                 self.sep_id, 0, self.mask_id, self.first, self.vocab_size,
                                 self.mask_prob, _item_generator(self.seed, idx))
+
+
+@DATASET.register_module
+class SynthQADataset(Dataset):
+    """Synthetic extractive question answering that a model can learn.  An item is ``[CLS] q1 q2
+    [SEP] context [SEP] pad...``: the context holds the token q1 and, later, the token q2 exactly
+    once each, and the answer is the 1..``max_answer_tokens`` tokens between them.  The context
+    length varies, so padding and the attention mask are exercised.  Token types are 0 for the
+    question part and 1 for the context and its final [SEP].
+
+    Labels are ``[start, end, start_lo, start_hi, end_hi]`` (``ops.functions.split_span_labels``):
+    the answer's first and last position, and the context's first and last position as the
+    search range.  Item i depends only on ``(seed, i)``; another seed draws a held-out split of
+    the same task.  Token ids are ``SynthMLMDataset``'s."""
+
+    def __init__(self, num_samples: int = 1024, max_seq_length: int = 384,
+                 vocab_size: int = 30528, seed: int = 0, max_answer_tokens: int = 8):
+        if max_answer_tokens < 1 or max_seq_length < max_answer_tokens + 7:
+            raise ValueError("max_seq_length must be at least max_answer_tokens + 7 ([CLS] q1 q2 "
+                             "[SEP] q1 answer q2 [SEP])")
+        big = vocab_size > 2000
+        self.cls_id, self.sep_id = (101, 102) if big else (1, 2)
+        self.first = 1000 if big else 4
+        if vocab_size < self.first + 3:
+            raise ValueError("vocab_size {} leaves too few body tokens".format(vocab_size))
+        self.num_samples, self.S, self.seed = num_samples, max_seq_length, seed
+        self.vocab_size, self.max_answer_tokens = vocab_size, max_answer_tokens
+
+    def __len__(self):
+        return self.num_samples
+
+    def __getitem__(self, idx):
+        if not 0 <= idx < self.num_samples:
+            raise IndexError(idx)
+        g = _item_generator(self.seed, idx)
+        S, A = self.S, self.max_answer_tokens
+        span = self.vocab_size - self.first
+        q = torch.randperm(span, generator=g)[:2] + self.first            # q1, q2: distinct
+        n_ans = int(torch.randint(1, A + 1, (1,), generator=g))
+        n_ctx = int(torch.randint(n_ans + 2, S - 5 + 1, (1,), generator=g))
+        # filler and answer tokens: body tokens other than q1 and q2
+        ctx = torch.randint(0, span - 2, (n_ctx,), generator=g) + self.first
+        for t in sorted(q.tolist()):
+            ctx = ctx + (ctx >= t).long()
+        p1 = int(torch.randint(0, n_ctx - n_ans - 1, (1,), generator=g))   # q1's context index
+        ctx[p1], ctx[p1 + n_ans + 1] = q[0], q[1]
+        row = torch.cat([torch.tensor([self.cls_id]), q, torch.tensor([self.sep_id]), ctx,
+                         torch.tensor([self.sep_id])])
+        n = row.numel()
+        ids = torch.zeros(S, dtype=torch.long)
+        ids[:n] = row
+        types = torch.zeros(S, dtype=torch.long)
+        types[4:n] = 1
+        mask = torch.zeros(S, dtype=torch.long)
+        mask[:n] = 1
+        start = 4 + p1 + 1
+        last = 4 + n_ctx - 1
+        labels = torch.tensor([start, start + n_ans - 1, 4, last, last])
+        return (ids, types, mask), labels
 
 
 @DATASET.register_module

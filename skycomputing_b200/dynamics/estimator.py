@@ -91,8 +91,16 @@ class Estimator:
             return 2.0 * B * H * C, mem, [((B, C), f32)]
         if c is None or lt not in ("BertEmbeddings", "BertLayer_Head", "BertLayer_Body",
                                    "BertLayer_Tail", "BertPooler", "BertTailForMaskedLM",
-                                   "BertTailForPreTraining"):
+                                   "BertTailForPreTraining", "BertTailForQuestionAnswering"):
             return None
+        if lt == "BertTailForQuestionAnswering":
+            # qa_outputs = Linear(H, 2) on every token: fp32 logits [B, 2, S]
+            B, S, _ = data[0].shape
+            H = c["hidden_size"]
+            params = 2 * H + 2
+            outs = 2 * B * S * 2          # the linear, the layer module itself
+            mem = (2 * outs + param_scale * params + B * S * H + B * S) * 4 / mb
+            return 2.0 * B * S * H * 2, mem, [((B, 2, S), f32)]
         if lt == "BertTailForPreTraining":
             # the masked-LM head, plus the pooler on the [CLS] rows and the 2-way classifier
             flops, mem, outs = Estimator.analytic_layer_cost(dict(layer_cfg, layer_type="BertTailForMaskedLM"),

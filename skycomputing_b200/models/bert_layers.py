@@ -14,6 +14,8 @@ Registered names and calling conventions are those of scaelum/model/bert_layers.
     BertTailForMaskedLM(config, tie_word_embeddings=True)
                                       as above; decoder weight = the word-embedding table
                                       (``tie_word_embeddings``, set up by the stage / engine)
+    BertTailForQuestionAnswering(config)
+                                      (hidden, mask)            -> logits [B, 2, S] (start, end)
 
 Parameter names match the reference (``attention.self.query.weight`` ...), so layer-indexed
 checkpoints interchange.  Every layer has two execution paths behind the same class:
@@ -678,6 +680,51 @@ class BertTailForPreTraining(BertTailForMaskedLM):
         return (*mlm, nsp) if isinstance(mlm, tuple) else (mlm, nsp)
 
 
+@LAYER.register_module
+class BertTailForQuestionAnswering(nn.Module):
+    """Extractive question-answering head (HF ``BertForQuestionAnswering``): ``qa_outputs =
+    Linear(H, 2)`` on every token, after the last encoder block (no pooler).  ``(hidden [B,S,H],
+    mask) -> logits [B, 2, S]`` in fp32, row 0 the start and row 1 the end logits (each softmax
+    row contiguous); as in HF the logits are not masked.
+
+    The native path (``QuestionAnsweringFn``) runs on a bf16 3-D input with ``H % 8 == 0``, any B
+    and S; other inputs, the CPU and ``backend="torch"`` run the eager fp32 path.  Labels are the
+    ``[B, 5]`` layout of ``ops.functions.split_span_labels``; the head is evaluated by span
+    (``evaluated_by``), and ``max_answer_length`` bounds the predicted answer in tokens."""
+
+    # the accumulator Runner.evaluate builds for this head: logit shapes alone are ambiguous
+    evaluated_by = "span"
+
+    def __init__(self, config, max_answer_length: int = 30):
+        super().__init__()
+        config = BertConfig.from_dict(config) if isinstance(config, dict) else config
+        if isinstance(max_answer_length, bool) or not isinstance(max_answer_length, int) \
+                or max_answer_length < 1:
+            raise ValueError("max_answer_length must be a positive int, got {!r}".format(
+                max_answer_length))
+        self.max_answer_length = max_answer_length
+        self.qa_outputs = nn.Linear(config.hidden_size, 2)
+        self._native = None
+
+    def _native_params(self):
+        from ..ops.functions import QuestionAnsweringParams
+
+        if self._native is None:
+            object.__setattr__(self, "_native", QuestionAnsweringParams(self))
+        return self._native
+
+    def forward(self, hidden_states, attention_mask=None):
+        if (_native_enabled(hidden_states) and hidden_states.dim() == 3
+                and hidden_states.dtype == torch.bfloat16 and hidden_states.shape[-1] % 8 == 0):
+            from ..ops.functions import QuestionAnsweringFn
+
+            hp = self._native_params()
+            if not self.training and not torch.is_grad_enabled():
+                return QuestionAnsweringFn.infer(hp, hidden_states)
+            return QuestionAnsweringFn.apply(hp, hidden_states, *hp.all_params())
+        return self.qa_outputs(hidden_states.float()).transpose(1, 2).contiguous()
+
+
 TIED_TABLE_NAME = "word_embeddings.weight"
 _WARNED_EAGER_BATCH = [False]
 
@@ -790,6 +837,8 @@ def native_param_banks(module: nn.Module):
         elif isinstance(m, BertTailForClassification):
             banks.extend(m._native_params().banks)
         elif isinstance(m, BertTailForMaskedLM):
+            banks.extend(m._native_params().banks)
+        elif isinstance(m, BertTailForQuestionAnswering):
             banks.extend(m._native_params().banks)
         elif isinstance(m, BertLayer_Head):
             banks.extend(_lone_span(m, head=m).params.banks)

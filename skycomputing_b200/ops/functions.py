@@ -972,6 +972,55 @@ class PreTrainingHeadFn(torch.autograd.Function):
         return (None, dx, None, *([None] * ctx.n_params))
 
 
+def split_span_labels(labels: torch.Tensor):
+    """The labels of a question-answering item are ONE int64 tensor ``[..., 5]``: the gold
+    answer's first and last token positions ``start`` and ``end``, the positions ``start_lo`` ..
+    ``start_hi`` where a predicted answer may start, and ``end_hi``, the last position where it
+    may end.  Returns ``(start, end, start_lo, start_hi, end_hi)`` as views.  A padded evaluation
+    row is ``ignore_index`` in every column.  One tensor keeps the engine's chunking, label
+    buffers, label routing and evaluation padding unchanged; this function is the only place that
+    knows the layout."""
+    return labels[..., 0], labels[..., 1], labels[..., 2], labels[..., 3], labels[..., 4]
+
+
+class QuestionAnsweringParams:
+    """Parameter banks of ``BertTailForQuestionAnswering``: ``qa_outputs`` (fp32 weight [2, H] and
+    bias [2], read by the kernels as they are, so no bf16 shadow)."""
+
+    def __init__(self, mod):
+        self.w = ParamBank([mod.qa_outputs.weight], False)
+        self.b = ParamBank([mod.qa_outputs.bias], False)
+        self.banks = [self.w, self.b]
+
+    def all_params(self):
+        return [p for b in self.banks for p in b.params]
+
+
+class QuestionAnsweringFn(torch.autograd.Function):
+    """BertTailForQuestionAnswering on sm_90a: ``qa_logits_fwd`` reads the bf16 hidden states once
+    and writes fp32 logits [B, 2, S]; backward (``qa_logits_bwd``) writes the bf16 input gradient
+    in one pass over the rows and adds dW / db into the fp32 bank gradients in a fixed order."""
+
+    @staticmethod
+    def infer(hp: QuestionAnsweringParams, hidden: torch.Tensor) -> torch.Tensor:
+        """Eval-mode forward without autograd: the same logits, nothing kept for backward."""
+        return nat.qa_logits(hidden.contiguous(), hp.w.master(), hp.b.master())
+
+    @staticmethod
+    def forward(ctx, hp, hidden, *params):
+        hidden = hidden.contiguous()
+        ctx.hp, ctx.hidden = hp, hidden
+        ctx.n_params = len(params)
+        return nat.qa_logits(hidden, hp.w.master(), hp.b.master())
+
+    @staticmethod
+    def backward(ctx, dlogits):
+        hp = ctx.hp
+        dx = nat.qa_logits_bwd(ctx.hidden, dlogits, hp.w.master(), hp.w.grad(), hp.b.grad())
+        ctx.hidden = None
+        return (None, dx, *([None] * ctx.n_params))
+
+
 class SoftmaxCrossEntropyFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits, labels):
@@ -983,3 +1032,19 @@ class SoftmaxCrossEntropyFn(torch.autograd.Function):
     def backward(ctx, dloss):
         (dlogits,) = ctx.saved_tensors
         return dlogits * dloss, None
+
+
+class SpanCrossEntropyFn(torch.autograd.Function):
+    """The span loss (``runner.QuestionAnsweringLoss``) as an autograd node on ``qa_span_ce``."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, ignore_index: int):
+        loss, dlogits = nat.qa_span_ce(logits.detach().float().contiguous(), labels,
+                                       ignore_index=ignore_index)
+        ctx.save_for_backward(dlogits)
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, dloss):
+        (dlogits,) = ctx.saved_tensors
+        return dlogits * dloss, None, None

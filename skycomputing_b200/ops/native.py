@@ -39,6 +39,7 @@ _KERNELS_PER_CALL = {
     "attention_fwd": 1, "attention_bwd": 1, "embed_fwd": 1, "embed_bwd": 1,
     "small_linear_fwd": 1, "small_linear_bwd": 2, "softmax_ce": 1, "classify_eval": 1,
     "vocab_ce": -1, "mlm_gather": 1, "mlm_scatter": 1,
+    "qa_logits_fwd": 1, "qa_logits_bwd": 2, "qa_span_ce": 1, "qa_span_eval": 1,
     "sgd_multi": 1, "adam_multi": 1, "lamb_moments": 1, "lamb_update": 1,
     "grad_sumsq_multi": 1, "optim_finalize": 1,
     "cast_f32_to_bf16": 1, "cast_bf16_to_f32": 1, "advance_counter": 1, "advance_epoch": 1,
@@ -555,6 +556,122 @@ def masked_softmax_ce(logits: torch.Tensor, labels: torch.Tensor, grad_scale: fl
                             dlogits=dlogits.data_ptr(), grad_scale=float(grad_scale),
                             loss=loss.data_ptr(), loss_acc=_ptr(loss_acc), stream=_stream())
     return loss, dlogits
+
+
+def _qa_labels(labels: torch.Tensor, B: int) -> torch.Tensor:
+    if not labels.is_cuda or labels.dtype != torch.int64 or labels.numel() != B * 5:
+        raise ValueError("labels must be a CUDA int64 tensor [B, 5] (ops.functions."
+                         "split_span_labels)")
+    return labels.reshape(B, 5).contiguous()
+
+
+def _qa_logits_check(logits: torch.Tensor):
+    _check(logits, torch.float32, "logits")
+    if logits.dim() != 3 or logits.shape[1] != 2 or not logits.is_contiguous():
+        raise ValueError("logits must be a contiguous [B, 2, S] tensor")
+    return logits.shape[0], logits.shape[2]
+
+
+def qa_logits(hidden: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """Start / end logits of a question-answering head: ``hidden`` bf16 [B, S, H] (H % 8 == 0),
+    ``w`` fp32 [2, H], ``b`` fp32 [2] -> fp32 [B, 2, S] (row 0 start, row 1 end).  One launch."""
+    _check(hidden, torch.bfloat16, "hidden")
+    _check(w, torch.float32, "w")
+    _check(b, torch.float32, "b")
+    if hidden.dim() != 3 or not hidden.is_contiguous():
+        raise ValueError("hidden must be a contiguous [B, S, H] tensor")
+    B, S, H = hidden.shape
+    if tuple(w.shape) != (2, H) or not w.is_contiguous() or b.numel() != 2:
+        raise ValueError("w must be a contiguous [2, {}] tensor and b [2]".format(H))
+    logits = torch.empty((B, 2, S), dtype=torch.float32, device=hidden.device)
+    ext().qa_logits_fwd(hidden=hidden.data_ptr(), B=B, S=S, H=H, w=w.data_ptr(), b=b.data_ptr(),
+                        logits=logits.data_ptr(), stream=_stream())
+    return logits
+
+
+def qa_logits_bwd(hidden: torch.Tensor, dlogits: torch.Tensor, w: torch.Tensor,
+                  dw: torch.Tensor, db: torch.Tensor) -> torch.Tensor:
+    """Backward of ``qa_logits``: returns ``dhidden`` bf16 [B, S, H] and adds the weight and bias
+    gradients into the fp32 ``dw`` [2, H] / ``db`` [2] in a fixed order.  Two launches."""
+    _check(hidden, torch.bfloat16, "hidden")
+    _check(w, torch.float32, "w")
+    _check(dw, torch.float32, "dw")
+    _check(db, torch.float32, "db")
+    B, S, H = hidden.shape
+    dlogits = dlogits.float().contiguous()
+    if tuple(dlogits.shape) != (B, 2, S):
+        raise ValueError("dlogits must be [B, 2, S] = {}".format([B, 2, S]))
+    if tuple(dw.shape) != (2, H) or not dw.is_contiguous() or db.numel() != 2:
+        raise ValueError("dw must be a contiguous [2, H] tensor and db [2]")
+    dhidden = torch.empty_like(hidden)
+    ws = torch.empty(ext().qa_logits_bwd_workspace_bytes(B, S, H) // 4, dtype=torch.float32,
+                     device=hidden.device)
+    ext().qa_logits_bwd(hidden=hidden.data_ptr(), dlogits=dlogits.data_ptr(), B=B, S=S, H=H,
+                        w=w.data_ptr(), dhidden=dhidden.data_ptr(), workspace=ws.data_ptr(),
+                        dw=dw.data_ptr(), db=db.data_ptr(), stream=_stream())
+    return dhidden
+
+
+def qa_span_ce(logits: torch.Tensor, labels: torch.Tensor, grad_scale: float = 1.0,
+               loss_acc: Optional[torch.Tensor] = None, ignore_index: int = -100):
+    """The span loss over fp32 logits ``[B, 2, S]`` and labels ``[B, 5]``: ``(mean start CE +
+    mean end CE) / 2``, each mean over the sequences whose label is in [0, S) (0 without one).
+    Returns ``(loss [1], dlogits [B, 2, S])``, d(loss * grad_scale)/dlogits with an exact 0 on
+    ignored rows; a label neither ``ignore_index`` nor in [0, S) makes the loss NaN.
+    ``loss_acc[0] += loss * grad_scale`` when given.  One launch, deterministic."""
+    B, S = _qa_logits_check(logits)
+    labels = _qa_labels(labels, B)
+    loss = torch.empty(1, dtype=torch.float32, device=logits.device)
+    dlogits = torch.empty_like(logits)
+    ext().qa_span_ce(logits=logits.data_ptr(), labels=labels.data_ptr(), B=B, S=S,
+                     ignore_index=int(ignore_index), dlogits=dlogits.data_ptr(),
+                     grad_scale=float(grad_scale), loss=loss.data_ptr(),
+                     loss_acc=_ptr(loss_acc), stream=_stream())
+    return loss, dlogits
+
+
+class SpanEvalAccumulator:
+    """Device-side accumulator of a span head's evaluation pass (``sky::SpanEvalAccum``): fp64
+    start / end cross-entropy and F1 sums, the counted sequences, top-1 start / end hits, exact
+    spans, invalid labels, and the best span and score of every sequence, stored at a device
+    cursor in buffers of ``capacity`` sequences (later ones are counted as overflow).
+
+    ``reset()`` is two memsets and ``add()`` one ``qa_span_eval`` launch, capturable into a CUDA
+    graph (a replay appends at the cursor); ``read()`` copies the totals and predictions once."""
+
+    def __init__(self, max_answer_length: int, capacity: int, device=None):
+        if max_answer_length < 1 or capacity < 0:
+            raise ValueError("max_answer_length must be >= 1 and capacity >= 0")
+        dev = device if device is not None else "cuda"
+        self.max_answer_length = int(max_answer_length)
+        self.capacity = int(capacity)
+        self.buffer = torch.zeros(ext().qa_span_eval_accum_bytes() // 8, dtype=torch.int64,
+                                  device=dev)
+        self.spans = torch.full((max(self.capacity, 1), 2), -1, dtype=torch.int32, device=dev)
+        self.scores = torch.zeros(max(self.capacity, 1), dtype=torch.float32, device=dev)
+
+    def reset(self) -> None:
+        self.buffer.zero_()
+        self.spans.fill_(-1)
+
+    def add(self, logits: torch.Tensor, labels: torch.Tensor, ignore_index: int = -100) -> None:
+        logits = logits.detach().float().contiguous()
+        B, S = _qa_logits_check(logits)
+        labels = _qa_labels(labels, B)
+        ext().qa_span_eval(logits=logits.data_ptr(), labels=labels.data_ptr(), B=B, S=S,
+                           max_answer_length=self.max_answer_length,
+                           ignore_index=int(ignore_index), acc=self.buffer.data_ptr(),
+                           pred_spans=self.spans.data_ptr(), pred_scores=self.scores.data_ptr(),
+                           capacity=self.capacity, stream=_stream())
+
+    def read(self) -> dict:
+        host = self.buffer.cpu()
+        f = host[0:3].view(torch.float64)
+        n = min(int(host[8]), self.capacity)
+        return dict(start_loss_sum=float(f[0]), end_loss_sum=float(f[1]), f1_sum=float(f[2]),
+                    count=int(host[3]), start_correct=int(host[4]), end_correct=int(host[5]),
+                    exact=int(host[6]), invalid=int(host[7]), overflow=int(host[9]),
+                    spans=self.spans[:n].cpu().long(), scores=self.scores[:n].cpu())
 
 
 class TokenEvalAccumulator:

@@ -16,6 +16,11 @@ counted per labelled token instead, without a confusion matrix: ``TorchTokenAccu
 oracle) and ``ops.native.TokenEvalAccumulator`` collect the loss sum, the labelled tokens, the
 correct top-1 predictions and the invalid labels, and ``token_metrics`` reports ``n``, ``loss``,
 ``accuracy`` and ``perplexity``.
+
+A span head (``BertTailForQuestionAnswering``: logits ``[B, 2, S]``, labels ``[B, 5]``) is
+evaluated by ``TorchSpanAccumulator`` (the oracle) or ``ops.native.SpanEvalAccumulator``: the best
+answer span of every sequence and the totals ``span_metrics`` turns into ``n``, ``loss``,
+``start_accuracy``, ``end_accuracy``, ``exact`` and ``f1``.
 """
 from __future__ import annotations
 
@@ -125,12 +130,127 @@ def make_accumulator(C: int, device) -> object:
     return TorchEvalAccumulator(C, device)
 
 
+class TorchSpanAccumulator:
+    """Same totals, spans and tie rule as the ``qa_span_eval`` kernel, in plain torch with fp64
+    sums (the CPU path and the kernel's oracle).  ``add`` takes logits ``[B, 2, S]`` and labels
+    ``[B, 5]`` (``ops.functions.split_span_labels``).
+
+    Best span of a sequence: the maximum of ``start[i] + end[j]`` (one fp32 add, NaN counts as
+    -inf) over ``max(start_lo, 0) <= i <= min(start_hi, S - 1)`` and ``i <= j <= min(i + L - 1,
+    end_hi, S - 1)``; among equal scores the smallest ``(i, j)`` wins; an empty range gives
+    ``(-1, -1)`` with score -inf.  Totals run over the sequences whose gold start and end are both
+    in [0, S): start / end cross entropy (fp64), top-1 start / end hits (``torch.argmax``), exact
+    spans and SQuAD's token F1 on position intervals.  Predictions of the first ``capacity``
+    sequences since ``reset`` are kept, later ones counted as overflow."""
+
+    def __init__(self, max_answer_length: int = 30, capacity: int = 0, device=None):
+        self.max_answer_length = int(max_answer_length)
+        self.capacity = int(capacity)
+        self.device = torch.device(device) if device is not None else torch.device("cpu")
+        self.reset()
+
+    def reset(self) -> None:
+        self.sums = torch.zeros(3, dtype=torch.float64)
+        self.counts = dict(count=0, start_correct=0, end_correct=0, exact=0, invalid=0, overflow=0)
+        self.spans, self.scores = [], []
+        self.seen = 0
+
+    @staticmethod
+    def best_span(start: torch.Tensor, end: torch.Tensor, lo: int, hi: int, end_hi: int, L: int):
+        """``(i, j, score)`` of one sequence's fp32 start / end logits [S]."""
+        S = start.numel()
+        lo, hi, end_hi = max(int(lo), 0), min(int(hi), S - 1), min(int(end_hi), S - 1)
+        if hi < lo:
+            return -1, -1, float("-inf")
+        i = torch.arange(S).view(S, 1)
+        j = torch.arange(S).view(1, S)
+        ok = (i >= lo) & (i <= hi) & (j >= i) & (j <= i + L - 1) & (j <= end_hi)
+        if not bool(ok.any()):
+            return -1, -1, float("-inf")
+        score = start.float().view(S, 1) + end.float().view(1, S)
+        score = torch.where(torch.isnan(score), float("-inf"), score)
+        best = score[ok].max()
+        k = int(torch.nonzero((ok & (score == best)).reshape(-1))[0])   # the first (i, j)
+        return k // S, k % S, float(best)
+
+    @staticmethod
+    def span_f1(pi: int, pj: int, gs: int, ge: int) -> float:
+        overlap = min(pj, ge) - max(pi, gs) + 1
+        if pi < 0 or overlap <= 0:
+            return 0.0
+        p, r = overlap / (pj - pi + 1), overlap / (ge - gs + 1)
+        return 2 * p * r / (p + r)
+
+    @torch.no_grad()
+    def add(self, logits: torch.Tensor, labels: torch.Tensor, ignore_index: int = -100) -> None:
+        logits = logits.detach().float().cpu()
+        labels = labels.detach().reshape(-1, 5).cpu().to(torch.int64)
+        B, _, S = logits.shape
+        for b in range(B):
+            gs, ge, lo, hi, ehi = (int(v) for v in labels[b])
+            st, en = logits[b, 0], logits[b, 1]
+            pi, pj, score = self.best_span(st, en, lo, hi, ehi, self.max_answer_length)
+            if self.seen < self.capacity:
+                self.spans.append((pi, pj))
+                self.scores.append(score)
+            else:
+                self.counts["overflow"] += 1
+            self.seen += 1
+            ok_s, ok_e = 0 <= gs < S, 0 <= ge < S
+            if (gs != ignore_index and not ok_s) or (ge != ignore_index and not ok_e):
+                self.counts["invalid"] += 1
+                continue
+            if not (ok_s and ok_e):
+                continue
+            c = self.counts
+            c["count"] += 1
+            c["start_correct"] += int(int(torch.argmax(st)) == gs)
+            c["end_correct"] += int(int(torch.argmax(en)) == ge)
+            c["exact"] += int(pi == gs and pj == ge)
+            self.sums[0] += float(torch.logsumexp(st.double(), 0) - st.double()[gs])
+            self.sums[1] += float(torch.logsumexp(en.double(), 0) - en.double()[ge])
+            self.sums[2] += self.span_f1(pi, pj, gs, ge)
+
+    def read(self) -> dict:
+        return dict(start_loss_sum=float(self.sums[0]), end_loss_sum=float(self.sums[1]),
+                    f1_sum=float(self.sums[2]), **self.counts,
+                    spans=torch.tensor(self.spans, dtype=torch.int64).reshape(-1, 2),
+                    scores=torch.tensor(self.scores, dtype=torch.float32))
+
+
+def make_span_accumulator(max_answer_length: int, capacity: int, device) -> object:
+    """The native span accumulator where the native kernels run, the torch one elsewhere."""
+    device = torch.device(device)
+    if device.type == "cuda":
+        from ..models.bert_layers import get_backend
+        from ..ops import native as nat
+
+        if get_backend() != "torch" and nat.available():
+            return nat.SpanEvalAccumulator(max_answer_length, capacity, device)
+    return TorchSpanAccumulator(max_answer_length, capacity, device)
+
+
+def span_metrics(totals: dict) -> dict:
+    """``n`` counted sequences, ``loss`` = (mean start CE + mean end CE) / 2, ``start_accuracy``,
+    ``end_accuracy``, ``exact`` (best span == gold span) and ``f1`` (mean token F1), as fractions;
+    None each when n == 0."""
+    n = int(totals["count"])
+    if n == 0:
+        return dict(n=0, loss=None, start_accuracy=None, end_accuracy=None, exact=None, f1=None)
+    return dict(n=n, loss=(totals["start_loss_sum"] + totals["end_loss_sum"]) / (2 * n),
+                start_accuracy=totals["start_correct"] / n, end_accuracy=totals["end_correct"] / n,
+                exact=totals["exact"] / n, f1=totals["f1_sum"] / n)
+
+
 class LazyEvalAccumulator:
     """Creates its accumulator on the first ``add`` (from the logits' class count and device) and
-    keeps it, so that a captured evaluation graph always adds into the same buffer."""
+    keeps it, so that a captured evaluation graph always adds into the same buffer.  ``span =
+    (max_answer_length, capacity)`` makes it a span accumulator (a head whose ``evaluated_by`` is
+    "span"): the logit shapes alone cannot tell a span head from a token-level one."""
 
-    def __init__(self, ignore_index: int = -100):
+    def __init__(self, ignore_index: int = -100, span=None):
         self.ignore_index = ignore_index
+        self.span = span
         self.inner = None
 
     def reset(self) -> None:
@@ -138,6 +258,8 @@ class LazyEvalAccumulator:
             self.inner.reset()
 
     def add(self, logits, labels: torch.Tensor) -> None:
+        if self.inner is None and self.span is not None:
+            self.inner = make_span_accumulator(self.span[0], self.span[1], logits.device)
         if self.inner is None and isinstance(logits, (tuple, list)):
             # pretraining head: (masked-LM logits, next-sentence logits)
             self.inner = PreTrainingAccumulator(logits[0].shape[-1], logits[0].device)
@@ -226,7 +348,8 @@ def token_metrics(loss_sum: float, count: int, correct: int) -> dict:
 def format_metrics(metrics: dict) -> str:
     parts = []
     for k in ("n", "loss", "accuracy", "perplexity", "f1", "mcc", "mlm_n", "mlm_loss",
-              "mlm_accuracy", "nsp_n", "nsp_loss", "nsp_accuracy"):
+              "mlm_accuracy", "nsp_n", "nsp_loss", "nsp_accuracy", "start_accuracy",
+              "end_accuracy", "exact", "text_exact_match", "text_f1"):
         if k in metrics:
             v = metrics[k]
             parts.append("{}={}".format(k, "None" if v is None else (
@@ -236,5 +359,6 @@ def format_metrics(metrics: dict) -> str:
 
 __all__ = ["TorchEvalAccumulator", "TorchTokenAccumulator", "LazyEvalAccumulator",
            "make_accumulator", "make_token_accumulator", "classification_metrics", "token_metrics",
-           "PreTrainingAccumulator", "pretraining_metrics",
+           "PreTrainingAccumulator", "pretraining_metrics", "TorchSpanAccumulator",
+           "make_span_accumulator", "span_metrics",
            "format_metrics"]

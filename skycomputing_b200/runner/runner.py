@@ -122,9 +122,65 @@ class _NativePreTrainingLoss(PreTrainingLoss):
         return dmlm, dnsp
 
 
+class QuestionAnsweringLoss(nn.Module):
+    """The span loss of a question-answering head (HF ``BertForQuestionAnswering``'s
+    ``total_loss``): ``(mean start CE + mean end CE) / 2`` over logits ``[B, 2, S]``, each mean
+    over the sequences whose label is in [0, S) (0 without one), labels the ``[B, 5]`` layout of
+    ``ops.functions.split_span_labels``.  ``ignore_index`` rows add nothing; any other label
+    outside [0, S) makes the loss NaN (HF clamps such positions and ignores them)."""
+
+    def __init__(self, ignore_index: int = -100):
+        super().__init__()
+        self.ignore_index = int(ignore_index)
+
+    def forward(self, logits, labels):
+        from ..ops.functions import split_span_labels
+
+        S = logits.shape[-1]
+        start, end = split_span_labels(labels.reshape(-1, 5))[:2]
+        total = 0.0
+        for row, lab in ((logits[:, 0].float(), start), (logits[:, 1].float(), end)):
+            keep = lab != self.ignore_index
+            valid = keep & (lab >= 0) & (lab < S)
+            ce = torch.logsumexp(row, 1) - row.gather(1, torch.where(valid, lab, 0)[:, None])[:, 0]
+            mean = torch.where(valid, ce, 0.0).sum() / valid.sum().clamp(min=1)
+            # an invalid label is never silent (and never used as an index)
+            total = total + torch.where((keep & ~valid).any(), float("nan"), mean)
+        return total / 2
+
+
+class _NativeQuestionAnsweringLoss(QuestionAnsweringLoss):
+    def forward(self, logits, labels):
+        from ..ops.functions import SpanCrossEntropyFn
+
+        return SpanCrossEntropyFn.apply(logits, labels, self.ignore_index)
+
+    def fused(self, logits, labels, scale: float, loss_acc: torch.Tensor) -> torch.Tensor:
+        """Engine fast path (see ``_NativeCrossEntropy.fused``): ``qa_span_ce`` adds ``loss *
+        scale`` into ``loss_acc`` and returns the [B, 2, S] gradient of the logits."""
+        from ..ops import native as nat
+
+        _, dlogits = nat.qa_span_ce(logits.detach().float().contiguous(), labels,
+                                    grad_scale=scale, loss_acc=loss_acc,
+                                    ignore_index=self.ignore_index)
+        return dlogits
+
+
+def _native_loss_ok(device: torch.device) -> bool:
+    if device.type != "cuda":
+        return False
+    from ..models.bert_layers import get_backend
+    from ..ops import native as nat
+
+    return get_backend() != "torch" and nat.available()
+
+
 def build_loss(loss_cfg: dict, device: torch.device) -> nn.Module:
     cfg = dict(loss_cfg)
     name = cfg.pop("type")
+    if name == "QuestionAnsweringLoss":
+        return (_NativeQuestionAnsweringLoss if _native_loss_ok(device)
+                else QuestionAnsweringLoss)(**cfg)
     if name == "PreTrainingLoss":
         if device.type == "cuda":
             from ..models.bert_layers import get_backend
@@ -389,7 +445,12 @@ class Runner:
         """Classification metrics of the model on ``data_loader`` (collective: every rank calls
         it and every rank gets the same dict, broadcast by the last stage).  For a token-level
         head (3-D logits / 2-D labels, e.g. ``BertTailForMaskedLM``) the metrics are those of
-        ``token_metrics``: labelled tokens, loss, top-1 accuracy and perplexity.  For a
+        ``token_metrics``: labelled tokens, loss, top-1 accuracy and perplexity.  For a head
+        evaluated by span (``BertTailForQuestionAnswering``) they are those of ``span_metrics``
+        (``n``, ``loss``, ``start_accuracy``, ``end_accuracy``, ``exact``, ``f1``), plus
+        ``text_exact_match`` and ``text_f1`` when the loader's dataset has ``text_scores(spans,
+        scores)``; more predictions than ``len(data_loader.dataset)`` rounded up to the batch
+        raise ``ValueError``.  For a
         pretraining head (``BertTailForPreTraining``) they are those of ``pretraining_metrics``:
         the masked-LM ones with an ``mlm_`` prefix (and ``perplexity``), the next-sentence ``nsp_n``,
         ``nsp_loss`` and ``nsp_accuracy``, and ``loss`` = the sum of the two losses.
@@ -409,8 +470,10 @@ class Runner:
 
         eng = self.engine
         m = int(micro_batches or self.micro_batches)
-        if self._eval_accum is None or self._eval_accum.ignore_index != ignore_index:
-            self._eval_accum = LazyEvalAccumulator(ignore_index)
+        span = self._span_spec(data_loader) if eng.is_last else None
+        if (self._eval_accum is None or self._eval_accum.ignore_index != ignore_index
+                or self._eval_accum.span != span):
+            self._eval_accum = LazyEvalAccumulator(ignore_index, span)
         acc = self._eval_accum
         was_training = self.model.training
         cpu_rng = torch.random.get_rng_state()   # iterating a DataLoader draws a base seed
@@ -444,7 +507,9 @@ class Runner:
                 self._call_hook("after_val_iter")
             totals = acc.read() if eng.is_last else None
             payload = None
-            if totals is not None and "mlm" in totals:   # pretraining head: both objectives
+            if totals is not None and "spans" in totals:   # question-answering head
+                payload = self._span_payload(totals, data_loader)
+            elif totals is not None and "mlm" in totals:   # pretraining head: both objectives
                 m, n = totals["mlm"], totals["nsp"]
                 payload = dict(pretraining_metrics(totals), invalid=m["invalid"] + n["invalid"],
                                classes=m["classes"], nsp_invalid=n["invalid"])
@@ -488,6 +553,35 @@ class Runner:
             with open(self._metrics_path, "a") as f:
                 f.write(json.dumps(dict(mode="val", name=name, iter=self._iter, **payload)) + "\n")
         self.last_eval = dict(payload, name=name)
+        return payload
+
+    def _span_spec(self, data_loader):
+        """``(max_answer_length, capacity)`` when the last layer is evaluated by span, else None:
+        the prediction buffer holds every example of the loader, its length rounded up to the
+        batch (a padded last batch is stored too)."""
+        layers = getattr(self.engine.stages[-1], "layers", None)
+        head = layers[-1] if layers is not None and len(layers) else None
+        if getattr(head, "evaluated_by", None) != "span":
+            return None
+        n = len(data_loader.dataset)
+        bs = int(getattr(data_loader, "batch_size", None) or 1)
+        return (int(head.max_answer_length), (n + bs - 1) // bs * bs)
+
+    @staticmethod
+    def _span_payload(totals: dict, data_loader) -> dict:
+        """The span metrics of a pass and, when the loader's dataset scores answer texts
+        (``text_scores``), the official SQuAD ``text_exact_match`` / ``text_f1``."""
+        from .metrics import span_metrics
+
+        if totals["overflow"]:
+            raise ValueError("evaluation: {} span predictions did not fit the prediction buffer "
+                             "of {} sequences".format(totals["overflow"], len(totals["spans"])))
+        payload = dict(span_metrics(totals), invalid=totals["invalid"],
+                       classes="S (the sequence length)")
+        ds = data_loader.dataset
+        if hasattr(ds, "text_scores"):
+            n = len(ds)
+            payload.update(ds.text_scores(totals["spans"][:n], totals["scores"][:n]))
         return payload
 
     def _batch_shape_ok(self, data) -> bool:

@@ -21,6 +21,8 @@ pipelines cut at different places can be compared (dropout off => the same math 
                    printed for every step (``tied_checksums``: [first rank's, last rank's])
     --nsp          the pretraining head (BertTailForPreTraining: masked-LM + next-sentence
                    prediction) with PreTrainingLoss on SynthPretrainingDataset
+    --qa           the question-answering head (BertTailForQuestionAnswering) with
+                   QuestionAnsweringLoss on SynthQADataset at --seq tokens (default 384 with --qa)
 """
 import argparse
 import json
@@ -47,6 +49,8 @@ def main():
     ap.add_argument("--max-predictions", type=int, default=None)
     ap.add_argument("--tie", action="store_true")
     ap.add_argument("--nsp", action="store_true")
+    ap.add_argument("--qa", action="store_true")
+    ap.add_argument("--seq", type=int, default=None)
     ap.add_argument("--optim", default="SGD")
     ap.add_argument("--virtual-stages", type=int, default=1)
     ap.add_argument("--max-grad-norm", type=float, default=None)
@@ -67,6 +71,8 @@ def main():
            dict(layer_type="BertLayer_Tail", config=cfg.__dict__)] * a.layers
     head = dict(layer_type="BertTailForPreTraining" if a.nsp else "BertTailForMaskedLM",
                 config=cfg.__dict__)
+    if a.qa:
+        head = dict(layer_type="BertTailForQuestionAnswering", config=cfg.__dict__)
     if a.max_predictions is not None:
         head["max_predictions"] = a.max_predictions
     if a.tie:
@@ -109,17 +115,23 @@ def main():
                     if n_.endswith("LayerNorm.weight"):
                         p.fill_(1.0)
     lr = 0.01 if a.optim == "SGD" else 1e-3
+    loss = ("QuestionAnsweringLoss" if a.qa else "PreTrainingLoss" if a.nsp else "MaskedLMLoss")
     opt = sky.build_optimizer(model.optim_module, dict(optim_type=a.optim, lr=lr),
                               grad_clip=(dict(max_norm=a.max_grad_norm)
                                          if a.max_grad_norm is not None else None))
     runner = sky.Runner(model=model, parameter_server=None, worker_manager=wm, optimizer=opt,
-                        max_epochs=1, max_iters=10 ** 9, loss_cfg=dict(type="PreTrainingLoss" if a.nsp else "MaskedLMLoss"),
+                        max_epochs=1, max_iters=10 ** 9, loss_cfg=dict(type=loss),
                         timer_cfg=dict(root="/tmp/sky_check_mlm"), logging_cfg=None,
                         micro_batches=a.micro_batches, schedule="1f1b", boundary=a.boundary,
                         device=dev)
     model.train(True)
-    data_cls = sky.SynthPretrainingDataset if a.nsp else sky.SynthMLMDataset
-    ds = data_cls(num_samples=a.batch * 2, max_seq_length=128, vocab_size=30528, seed=3)
+    seq = a.seq or (384 if a.qa else 128)
+    if a.qa:
+        ds = sky.SynthQADataset(num_samples=a.batch * 2, max_seq_length=seq, vocab_size=30528,
+                                seed=3)
+    else:
+        data_cls = sky.SynthPretrainingDataset if a.nsp else sky.SynthMLMDataset
+        ds = data_cls(num_samples=a.batch * 2, max_seq_length=seq, vocab_size=30528, seed=3)
     batches = list(torch.utils.data.DataLoader(ds, batch_size=a.batch))
     losses, checksums, norms = [], [], []
     eng = runner.engine
