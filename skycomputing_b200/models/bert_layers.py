@@ -60,16 +60,20 @@ def _nat():
     return native
 
 
+def native_active(device: torch.device) -> bool:
+    """Do the sm_90a kernels run on ``device`` (CUDA, backend not "torch", extension built)?"""
+    return device.type == "cuda" and _BACKEND != "torch" and _nat().available()
+
+
 def _native_enabled(t: torch.Tensor) -> bool:
+    if native_active(t.device):
+        return True
     if _BACKEND == "torch" or not t.is_cuda:
         if _BACKEND == "native" and not t.is_cuda:
             raise RuntimeError("backend 'native' requires CUDA tensors")
         return False
-    nat = _nat()
-    if nat.available():
-        return True
     if _BACKEND == "native":
-        nat.ext()  # raises with the build hint
+        _nat().ext()  # raises with the build hint
     raise RuntimeError(
         "CUDA tensors reached a skycomputing_b200 layer but the sm_90a extension is not built; "
         "run __graft_entry__.build() (or set_backend('torch') to use the eager oracle on purpose)"
@@ -468,6 +472,8 @@ class BertPooler(nn.Module):
 
 @LAYER.register_module
 class BertTailForClassification(nn.Module):
+    objective = "classification"   # how Runner.evaluate scores it: runner.metrics.OBJECTIVES
+
     def __init__(self, hidden_dropout_prob, hidden_size, num_classes):
         super().__init__()
         self.num_classes = num_classes
@@ -538,6 +544,7 @@ class BertTailForMaskedLM(nn.Module):
     marks empty slots with it, and a loss with another value counts them as invalid labels."""
 
     MAX_PREDICTIONS_LIMIT = 8192   # csrc/kernels/api.h: kMlmMaxPredictions
+    objective = "masked_lm"
 
     def __init__(self, config, max_predictions=None, ignore_index: int = -100,
                  tie_word_embeddings: bool = False):
@@ -639,6 +646,7 @@ class BertTailForPreTraining(BertTailForMaskedLM):
 
     # the outputs the loss differentiates: masked-LM logits first, next-sentence logits last
     logit_outputs = (0, -1)
+    objective = "pretraining"
 
     def __init__(self, config, max_predictions=None, ignore_index: int = -100,
                  tie_word_embeddings: bool = False):
@@ -672,7 +680,7 @@ class BertTailForPreTraining(BertTailForMaskedLM):
             if not self.training and not torch.is_grad_enabled():
                 return PreTrainingHeadFn.infer(hp, x, labels)
             return PreTrainingHeadFn.apply(hp, x, labels, *hp.all_params())
-        if hidden_states.is_cuda and _BACKEND != "torch" and super()._supports(hidden_states):
+        if native_active(hidden_states.device) and super()._supports(hidden_states):
             _warn_eager_batch(hidden_states.shape[0])
         nsp = self.seq_relationship(self.pooler.dense_act(hidden_states[:, 0].float()))
         mlm = super().forward(hidden_states, attention_mask,
@@ -690,10 +698,10 @@ class BertTailForQuestionAnswering(nn.Module):
     The native path (``QuestionAnsweringFn``) runs on a bf16 3-D input with ``H % 8 == 0``, any B
     and S; other inputs, the CPU and ``backend="torch"`` run the eager fp32 path.  Labels are the
     ``[B, 5]`` layout of ``ops.functions.split_span_labels``; the head is evaluated by span
-    (``evaluated_by``), and ``max_answer_length`` bounds the predicted answer in tokens."""
+    (``objective``), and ``max_answer_length`` bounds the predicted answer in tokens."""
 
-    # the accumulator Runner.evaluate builds for this head: logit shapes alone are ambiguous
-    evaluated_by = "span"
+    # logit shapes alone would not tell this head from a token-level one
+    objective = "span"
 
     def __init__(self, config, max_answer_length: int = 30):
         super().__init__()

@@ -512,10 +512,9 @@ class EngineBase:
 
     # ------------------------------------------------------------------ backend
     def _native_active(self) -> bool:
-        from ..models.bert_layers import get_backend
-        from ..ops import native as nat
+        from ..models.bert_layers import native_active
 
-        return self.device.type == "cuda" and get_backend() != "torch" and nat.available()
+        return native_active(self.device)
 
     # ------------------------------------------------------------------ weight gradients
     def _configure_wgrad(self, multi: bool) -> None:

@@ -819,12 +819,9 @@ def _build_optimizer(module: nn.Module, optim_cfg: dict, prefer_fused: bool):
     cfg = dict(optim_cfg)
     optim_type = cfg.pop("optim_type", "SGD")
     params = [p for p in module.parameters() if p.requires_grad]
-    fused = False
-    if prefer_fused and any(p.is_cuda for p in params):
-        from ..models.bert_layers import get_backend
-        from ..ops import native as nat
+    from ..models.bert_layers import native_active
 
-        fused = get_backend() != "torch" and nat.available()
+    fused = prefer_fused and any(native_active(p.device) for p in params)
     if optim_type == "LAMB":
         # no torch.optim class to fall back to: every option is checked here, on every backend
         cfg = check_lamb_cfg(cfg)

@@ -8,8 +8,8 @@ GLUE classification tasks report.
 
 * ``TorchEvalAccumulator``: plain torch on any device, fp64 losses.  Used for CPU runs and
   ``backend="torch"``, and the oracle of the native ``ops.native.EvalAccumulator``;
-* ``LazyEvalAccumulator``: what ``Runner.evaluate`` hands to the engine - picks the native or the
-  torch accumulator from the first logits it sees (the class count is only known there).
+* ``LazyEvalAccumulator``: what ``Runner.evaluate`` hands to the engine (``eval_accumulator``) -
+  the accumulator ``OBJECTIVES`` maps the ``objective`` of the model's last layer to.
 
 Token-level outputs (a masked-language-model head: logits ``[B, S, V]``, labels ``[B, S]``) are
 counted per labelled token instead, without a confusion matrix: ``TorchTokenAccumulator`` (the
@@ -25,8 +25,11 @@ answer span of every sequence and the totals ``span_metrics`` turns into ``n``, 
 from __future__ import annotations
 
 import math
+from typing import Callable, NamedTuple
 
 import torch
+
+from ..models.bert_layers import native_active
 
 
 class TorchEvalAccumulator:
@@ -105,27 +108,22 @@ class TorchTokenAccumulator:
                     correct=int(self.correct), invalid=int(self.invalid), classes=self.V)
 
 
-def make_token_accumulator(V: int, device) -> object:
+def _token_accumulator(V: int, device) -> object:
     """The native token accumulator where the native kernels run, the torch one elsewhere."""
-    device = torch.device(device)
-    if device.type == "cuda":
-        from ..models.bert_layers import get_backend
+    if native_active(device):
         from ..ops import native as nat
 
-        if get_backend() != "torch" and nat.available() and V <= nat.ext().vocab_ce_max_v():
+        if V <= nat.ext().vocab_ce_max_v():
             return nat.TokenEvalAccumulator(V, device)
     return TorchTokenAccumulator(V, device)
 
 
-def make_accumulator(C: int, device) -> object:
-    """The native accumulator where the native kernels run (CUDA, backend != "torch", C within
-    the kernel's limit), the torch one elsewhere."""
-    device = torch.device(device)
-    if device.type == "cuda":
-        from ..models.bert_layers import get_backend
+def _classification_accumulator(C: int, device) -> object:
+    """The native accumulator where the native kernels run and take C, the torch one elsewhere."""
+    if native_active(device):
         from ..ops import native as nat
 
-        if get_backend() != "torch" and nat.available() and C <= nat.ext().eval_max_classes():
+        if C <= nat.ext().eval_max_classes():
             return nat.EvalAccumulator(C, device)
     return TorchEvalAccumulator(C, device)
 
@@ -218,15 +216,12 @@ class TorchSpanAccumulator:
                     scores=torch.tensor(self.scores, dtype=torch.float32))
 
 
-def make_span_accumulator(max_answer_length: int, capacity: int, device) -> object:
+def _span_accumulator(max_answer_length: int, capacity: int, device) -> object:
     """The native span accumulator where the native kernels run, the torch one elsewhere."""
-    device = torch.device(device)
-    if device.type == "cuda":
-        from ..models.bert_layers import get_backend
+    if native_active(device):
         from ..ops import native as nat
 
-        if get_backend() != "torch" and nat.available():
-            return nat.SpanEvalAccumulator(max_answer_length, capacity, device)
+        return nat.SpanEvalAccumulator(max_answer_length, capacity, device)
     return TorchSpanAccumulator(max_answer_length, capacity, device)
 
 
@@ -243,14 +238,14 @@ def span_metrics(totals: dict) -> dict:
 
 
 class LazyEvalAccumulator:
-    """Creates its accumulator on the first ``add`` (from the logits' class count and device) and
-    keeps it, so that a captured evaluation graph always adds into the same buffer.  ``span =
-    (max_answer_length, capacity)`` makes it a span accumulator (a head whose ``evaluated_by`` is
-    "span"): the logit shapes alone cannot tell a span head from a token-level one."""
+    """Creates the accumulator of ``objective`` from ``args`` on the first ``add`` and keeps it, so
+    that a captured evaluation graph always adds into the same buffer.  A last layer that declares
+    no objective is scored per token when its first logits are 3-D or its labels 2-D, per sequence
+    otherwise, with the class count of those logits."""
 
-    def __init__(self, ignore_index: int = -100, span=None):
-        self.ignore_index = ignore_index
-        self.span = span
+    def __init__(self, ignore_index: int = -100, objective=None, args=None):
+        self.key = (objective, ignore_index, args)
+        self.ignore_index, self.objective, self.args = ignore_index, objective, args
         self.inner = None
 
     def reset(self) -> None:
@@ -258,16 +253,12 @@ class LazyEvalAccumulator:
             self.inner.reset()
 
     def add(self, logits, labels: torch.Tensor) -> None:
-        if self.inner is None and self.span is not None:
-            self.inner = make_span_accumulator(self.span[0], self.span[1], logits.device)
-        if self.inner is None and isinstance(logits, (tuple, list)):
-            # pretraining head: (masked-LM logits, next-sentence logits)
-            self.inner = PreTrainingAccumulator(logits[0].shape[-1], logits[0].device)
         if self.inner is None:
-            # one prediction per token (MLM head: [B, S, V] logits, [B, S] labels) or per sequence
-            per_token = logits.dim() == 3 or labels.dim() == 2
-            make = make_token_accumulator if per_token else make_accumulator
-            self.inner = make(logits.shape[-1], logits.device)
+            if self.objective is None:
+                per_token = logits.dim() == 3 or labels.dim() == 2
+                self.objective = "masked_lm" if per_token else "classification"
+                self.args = (logits.shape[-1],)
+            self.inner = OBJECTIVES[self.objective].accumulator(*self.args, labels.device)
         self.inner.add(logits, labels, self.ignore_index)
 
     def read(self) -> dict:
@@ -275,16 +266,21 @@ class LazyEvalAccumulator:
             return dict(loss_sum=0.0, count=0, invalid=0, confusion=torch.zeros(0, 0, dtype=torch.int64))
         return self.inner.read()
 
+    def payload(self, head, loader) -> dict:
+        """The metrics of the pass and ``error``, the text of the ValueError its labels raise."""
+        objective = self.objective if self.inner is not None else "classification"
+        return OBJECTIVES[objective].payload(self.read(), head, loader, self.ignore_index)
+
 
 class PreTrainingAccumulator:
     """Both objectives of a pretraining head: the masked-LM token totals and the next-sentence
-    classification totals (two classes), each in the accumulator ``make_token_accumulator`` /
-    ``make_accumulator`` picks for the device.  ``add`` takes ``(mlm_logits, nsp_logits)`` and
-    the one-tensor labels of ``ops.functions.split_pretraining_labels``."""
+    classification totals (two classes), each native or torch as for a head of that kind.  ``add``
+    takes ``(mlm_logits, nsp_logits)`` and the one-tensor labels of
+    ``ops.functions.split_pretraining_labels``."""
 
     def __init__(self, V: int, device):
-        self.mlm = make_token_accumulator(V, device)
-        self.nsp = make_accumulator(2, device)
+        self.mlm = _token_accumulator(V, device)
+        self.nsp = _classification_accumulator(2, device)
 
     def reset(self) -> None:
         self.mlm.reset()
@@ -345,6 +341,88 @@ def token_metrics(loss_sum: float, count: int, correct: int) -> dict:
                 perplexity=math.exp(min(loss, 700.0)) if n else None)
 
 
+def _labels_error(invalid: int, classes, ignore_index: int, *notes: str):
+    """The text of the ValueError a pass with ``invalid`` labels raises; None without one."""
+    return "{} labels are outside [0, {}) and not ignore_index ({}){}".format(
+        invalid, classes, ignore_index, "".join(notes)) if invalid else None
+
+
+def _max_predictions_note(head, V: int) -> str:
+    if not getattr(head, "consumes_labels", False):
+        return ""
+    return ("; the sparse masked-language-model head decodes at most max_predictions = {} "
+            "labelled positions per sequence, and a sequence with more gets the out-of-range "
+            "label {} in its last slot: raise max_predictions or label fewer positions".format(
+                head.max_predictions, V))
+
+
+def _classification_payload(totals: dict, head, loader, ignore_index: int) -> dict:
+    return dict(classification_metrics(totals["confusion"], totals["loss_sum"], totals["count"]),
+                error=_labels_error(totals["invalid"], len(totals["confusion"]), ignore_index))
+
+
+def _token_payload(totals: dict, head, loader, ignore_index: int) -> dict:
+    return dict(token_metrics(totals["loss_sum"], totals["count"], totals["correct"]),
+                error=_labels_error(totals["invalid"], totals["classes"], ignore_index,
+                                    _max_predictions_note(head, totals["classes"])))
+
+
+def _pretraining_payload(totals: dict, head, loader, ignore_index: int) -> dict:
+    m, n = totals["mlm"], totals["nsp"]
+    return dict(pretraining_metrics(totals), error=_labels_error(
+        m["invalid"] + n["invalid"], m["classes"], ignore_index,
+        " ({} of them next-sentence labels, which must be in [0, 2))".format(n["invalid"]),
+        _max_predictions_note(head, m["classes"])))
+
+
+def _span_args(head, loader) -> tuple:
+    """``(max_answer_length, capacity)``: the prediction buffer holds every example of the loader,
+    its length rounded up to the batch (a padded last batch is stored too)."""
+    n = len(loader.dataset)
+    bs = int(getattr(loader, "batch_size", None) or 1)
+    return int(head.max_answer_length), (n + bs - 1) // bs * bs
+
+
+def _span_payload(totals: dict, head, loader, ignore_index: int) -> dict:
+    """Span metrics, and the dataset's ``text_scores`` (SQuAD answer-text scores) if it has any."""
+    if totals["overflow"]:
+        raise ValueError("evaluation: {} span predictions did not fit the prediction buffer "
+                         "of {} sequences".format(totals["overflow"], len(totals["spans"])))
+    payload = dict(span_metrics(totals), error=_labels_error(
+        totals["invalid"], "S (the sequence length)", ignore_index))
+    ds = loader.dataset
+    if hasattr(ds, "text_scores"):
+        n = len(ds)
+        payload.update(ds.text_scores(totals["spans"][:n], totals["scores"][:n]))
+    return payload
+
+
+class Objective(NamedTuple):     # how an evaluation pass scores a last layer's ``objective``
+    args: Callable          # (head, loader) -> the arguments the accumulator is built from
+    accumulator: Callable   # (*args, device) -> the accumulator, native where the kernels run
+    payload: Callable       # (totals, head, loader, ignore_index) -> the metrics and ``error``
+
+
+OBJECTIVES = {
+    "classification": Objective(lambda head, loader: (head.num_classes,),
+                                _classification_accumulator, _classification_payload),
+    "masked_lm": Objective(lambda head, loader: (head.decoder.out_features,),
+                           _token_accumulator, _token_payload),
+    "pretraining": Objective(lambda head, loader: (head.decoder.out_features,),
+                             PreTrainingAccumulator, _pretraining_payload),
+    "span": Objective(_span_args, _span_accumulator, _span_payload),
+}
+
+
+def eval_accumulator(head, ignore_index: int, loader, previous=None) -> LazyEvalAccumulator:
+    """``previous`` if built alike (a captured evaluation graph adds into it), else a new one."""
+    objective = getattr(head, "objective", None)
+    args = OBJECTIVES[objective].args(head, loader) if objective else None
+    if previous is None or previous.key != (objective, ignore_index, args):
+        previous = LazyEvalAccumulator(ignore_index, objective, args)
+    return previous
+
+
 def format_metrics(metrics: dict) -> str:
     parts = []
     for k in ("n", "loss", "accuracy", "perplexity", "f1", "mcc", "mlm_n", "mlm_loss",
@@ -357,8 +435,7 @@ def format_metrics(metrics: dict) -> str:
     return ", ".join(parts)
 
 
-__all__ = ["TorchEvalAccumulator", "TorchTokenAccumulator", "LazyEvalAccumulator",
-           "make_accumulator", "make_token_accumulator", "classification_metrics", "token_metrics",
-           "PreTrainingAccumulator", "pretraining_metrics", "TorchSpanAccumulator",
-           "make_span_accumulator", "span_metrics",
-           "format_metrics"]
+__all__ = ["TorchEvalAccumulator", "TorchTokenAccumulator", "classification_metrics",
+           "token_metrics", "PreTrainingAccumulator", "pretraining_metrics",
+           "TorchSpanAccumulator", "span_metrics", "OBJECTIVES", "LazyEvalAccumulator",
+           "eval_accumulator", "format_metrics"]

@@ -166,44 +166,24 @@ class _NativeQuestionAnsweringLoss(QuestionAnsweringLoss):
         return dlogits
 
 
-def _native_loss_ok(device: torch.device) -> bool:
-    if device.type != "cuda":
-        return False
-    from ..models.bert_layers import get_backend
-    from ..ops import native as nat
-
-    return get_backend() != "torch" and nat.available()
+_LOSSES = {
+    "CrossEntropyLoss": (nn.CrossEntropyLoss, _NativeCrossEntropy),
+    "MaskedLMLoss": (MaskedLMLoss, _NativeMaskedLMLoss),
+    "PreTrainingLoss": (PreTrainingLoss, _NativePreTrainingLoss),
+    "QuestionAnsweringLoss": (QuestionAnsweringLoss, _NativeQuestionAnsweringLoss),
+}
 
 
 def build_loss(loss_cfg: dict, device: torch.device) -> nn.Module:
+    from ..models.bert_layers import native_active
+
     cfg = dict(loss_cfg)
     name = cfg.pop("type")
-    if name == "QuestionAnsweringLoss":
-        return (_NativeQuestionAnsweringLoss if _native_loss_ok(device)
-                else QuestionAnsweringLoss)(**cfg)
-    if name == "PreTrainingLoss":
-        if device.type == "cuda":
-            from ..models.bert_layers import get_backend
-            from ..ops import native as nat
-
-            if get_backend() != "torch" and nat.available():
-                return _NativePreTrainingLoss(**cfg)
-        return PreTrainingLoss(**cfg)
-    if name == "MaskedLMLoss":
-        if device.type == "cuda":
-            from ..models.bert_layers import get_backend
-            from ..ops import native as nat
-
-            if get_backend() != "torch" and nat.available():
-                return _NativeMaskedLMLoss(**cfg)
-        return MaskedLMLoss(**cfg)
-    if name == "CrossEntropyLoss" and not cfg and device.type == "cuda":
-        from ..models.bert_layers import get_backend
-        from ..ops import native as nat
-
-        if get_backend() != "torch" and nat.available():
-            return _NativeCrossEntropy()
-    return getattr(nn, name)(**cfg)
+    # the native cross entropy takes no options (label_smoothing, weight, ...)
+    if name not in _LOSSES or (name == "CrossEntropyLoss" and cfg):
+        return getattr(nn, name)(**cfg)
+    torch_loss, native_loss = _LOSSES[name]
+    return (native_loss if native_active(device) else torch_loss)(**cfg)
 
 
 class Runner:
@@ -444,13 +424,13 @@ class Runner:
                  ignore_index: int = -100) -> dict:
         """Classification metrics of the model on ``data_loader`` (collective: every rank calls
         it and every rank gets the same dict, broadcast by the last stage).  For a token-level
-        head (3-D logits / 2-D labels, e.g. ``BertTailForMaskedLM``) the metrics are those of
-        ``token_metrics``: labelled tokens, loss, top-1 accuracy and perplexity.  For a head
-        evaluated by span (``BertTailForQuestionAnswering``) they are those of ``span_metrics``
-        (``n``, ``loss``, ``start_accuracy``, ``end_accuracy``, ``exact``, ``f1``), plus
-        ``text_exact_match`` and ``text_f1`` when the loader's dataset has ``text_scores(spans,
-        scores)``; more predictions than ``len(data_loader.dataset)`` rounded up to the batch
-        raise ``ValueError``.  For a
+        head (``BertTailForMaskedLM``, or a last layer without an ``objective`` whose logits are
+        3-D or labels 2-D) the metrics are those of ``token_metrics``: labelled tokens, loss,
+        top-1 accuracy and perplexity.  For a head evaluated by span
+        (``BertTailForQuestionAnswering``) they are those of ``span_metrics`` (``n``, ``loss``,
+        ``start_accuracy``, ``end_accuracy``, ``exact``, ``f1``), plus ``text_exact_match`` and
+        ``text_f1`` when the loader's dataset has ``text_scores(spans, scores)``; more predictions
+        than ``len(data_loader.dataset)`` rounded up to the batch raise ``ValueError``.  For a
         pretraining head (``BertTailForPreTraining``) they are those of ``pretraining_metrics``:
         the masked-LM ones with an ``mlm_`` prefix (and ``perplexity``), the next-sentence ``nsp_n``,
         ``nsp_loss`` and ``nsp_accuracy``, and ``loss`` = the sum of the two losses.
@@ -465,16 +445,14 @@ class Runner:
         """
         import torch.distributed as dist
 
-        from .metrics import (LazyEvalAccumulator, classification_metrics, format_metrics,
-                              pretraining_metrics, token_metrics)
+        from .metrics import eval_accumulator, format_metrics
 
         eng = self.engine
         m = int(micro_batches or self.micro_batches)
-        span = self._span_spec(data_loader) if eng.is_last else None
-        if (self._eval_accum is None or self._eval_accum.ignore_index != ignore_index
-                or self._eval_accum.span != span):
-            self._eval_accum = LazyEvalAccumulator(ignore_index, span)
-        acc = self._eval_accum
+        layers = getattr(eng.stages[-1], "layers", None)
+        head = layers[-1] if layers is not None and len(layers) else None
+        acc = self._eval_accum = eval_accumulator(head, ignore_index, data_loader,
+                                                  self._eval_accum)
         was_training = self.model.training
         cpu_rng = torch.random.get_rng_state()   # iterating a DataLoader draws a base seed
         self.model.train(False)
@@ -505,26 +483,7 @@ class Runner:
                 eng.eval_step(inputs, lab, acc, micro_batches=m)
                 self.val_iter += 1
                 self._call_hook("after_val_iter")
-            totals = acc.read() if eng.is_last else None
-            payload = None
-            if totals is not None and "spans" in totals:   # question-answering head
-                payload = self._span_payload(totals, data_loader)
-            elif totals is not None and "mlm" in totals:   # pretraining head: both objectives
-                m, n = totals["mlm"], totals["nsp"]
-                payload = dict(pretraining_metrics(totals), invalid=m["invalid"] + n["invalid"],
-                               classes=m["classes"], nsp_invalid=n["invalid"])
-            elif totals is not None and "confusion" not in totals:   # token-level (MLM head)
-                payload = dict(token_metrics(totals["loss_sum"], totals["count"],
-                                             totals["correct"]),
-                               invalid=totals["invalid"], classes=totals["classes"])
-            elif totals is not None:
-                payload = dict(classification_metrics(totals["confusion"], totals["loss_sum"],
-                                                      totals["count"]),
-                               invalid=totals["invalid"], classes=len(totals["confusion"]))
-            if payload is not None:
-                last = eng.stages[-1]
-                payload["max_predictions"] = (getattr(last.layers[-1], "max_predictions", None)
-                                              if getattr(last, "consumes_labels", False) else None)
+            payload = acc.payload(head, data_loader) if eng.is_last else None
             if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
                 box = [payload]
                 dist.broadcast_object_list(box, src=self.model.stage_to_rank[-1])
@@ -532,56 +491,15 @@ class Runner:
         finally:
             self.model.train(was_training)
             torch.random.set_rng_state(cpu_rng)
-        invalid, classes = payload.pop("invalid"), payload.pop("classes")
-        max_predictions = payload.pop("max_predictions")
-        nsp_invalid = payload.pop("nsp_invalid", None)
-        if invalid:
-            msg = "evaluation {}: {} labels are outside [0, {}) and not ignore_index ({})".format(
-                name, invalid, classes, ignore_index)
-            if nsp_invalid is not None:
-                msg += " ({} of them next-sentence labels, which must be in [0, 2))".format(
-                    nsp_invalid)
-            if max_predictions is not None:
-                msg += ("; the sparse masked-language-model head decodes at most max_predictions = "
-                        "{} labelled positions per sequence, and a sequence with more gets the "
-                        "out-of-range label {} in its last slot: raise max_predictions or label "
-                        "fewer positions".format(max_predictions, classes))
-            raise ValueError(msg)
+        error = payload.pop("error")
+        if error:
+            raise ValueError("evaluation {}: {}".format(name, error))
         self._call_hook("after_val_epoch")
         self._log("eval {}: {}".format(name, format_metrics(payload)))
         if self._metrics_path is not None:
             with open(self._metrics_path, "a") as f:
                 f.write(json.dumps(dict(mode="val", name=name, iter=self._iter, **payload)) + "\n")
         self.last_eval = dict(payload, name=name)
-        return payload
-
-    def _span_spec(self, data_loader):
-        """``(max_answer_length, capacity)`` when the last layer is evaluated by span, else None:
-        the prediction buffer holds every example of the loader, its length rounded up to the
-        batch (a padded last batch is stored too)."""
-        layers = getattr(self.engine.stages[-1], "layers", None)
-        head = layers[-1] if layers is not None and len(layers) else None
-        if getattr(head, "evaluated_by", None) != "span":
-            return None
-        n = len(data_loader.dataset)
-        bs = int(getattr(data_loader, "batch_size", None) or 1)
-        return (int(head.max_answer_length), (n + bs - 1) // bs * bs)
-
-    @staticmethod
-    def _span_payload(totals: dict, data_loader) -> dict:
-        """The span metrics of a pass and, when the loader's dataset scores answer texts
-        (``text_scores``), the official SQuAD ``text_exact_match`` / ``text_f1``."""
-        from .metrics import span_metrics
-
-        if totals["overflow"]:
-            raise ValueError("evaluation: {} span predictions did not fit the prediction buffer "
-                             "of {} sequences".format(totals["overflow"], len(totals["spans"])))
-        payload = dict(span_metrics(totals), invalid=totals["invalid"],
-                       classes="S (the sequence length)")
-        ds = data_loader.dataset
-        if hasattr(ds, "text_scores"):
-            n = len(ds)
-            payload.update(ds.text_scores(totals["spans"][:n], totals["scores"][:n]))
         return payload
 
     def _batch_shape_ok(self, data) -> bool:

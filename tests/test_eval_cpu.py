@@ -10,7 +10,9 @@ import torch
 import torch.nn.functional as F
 
 import skycomputing_b200 as sky
-from skycomputing_b200.runner.metrics import TorchEvalAccumulator, classification_metrics
+from skycomputing_b200.runner.metrics import (PreTrainingAccumulator, TorchEvalAccumulator,
+                                              TorchTokenAccumulator, classification_metrics,
+                                              eval_accumulator)
 from tests._dist_helpers import free_port, run_distributed
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -52,6 +54,33 @@ def test_torch_accumulator_skips_ignored_and_counts_invalid():
     assert r["confusion"].tolist() == [[1, 0, 0], [0, 1, 0], [0, 0, 0]]
     want = F.cross_entropy(logits[:2].double(), torch.tensor([1, 0]), reduction="sum")
     assert r["loss_sum"] == pytest.approx(float(want), rel=1e-12)
+
+
+@pytest.mark.parametrize("layer_type", ["BertTailForClassification", "BertTailForMaskedLM",
+                                        "BertTailForPreTraining"])
+def test_declared_objective_picks_the_torch_accumulator_on_the_cpu(layer_type):
+    c = sky.BertConfig(100, hidden_size=32, num_hidden_layers=1, num_attention_heads=4,
+                       intermediate_size=64, max_position_embeddings=32).__dict__
+    kw = (dict(hidden_dropout_prob=0.1, hidden_size=32, num_classes=3)
+          if layer_type == "BertTailForClassification" else dict(config=c))
+    head = sky.build_layer(layer_type, **kw)
+    acc = eval_accumulator(head, -100, None)   # only a span head reads the loader
+    assert acc.objective == head.objective
+    pooled = layer_type == "BertTailForClassification"
+    with torch.no_grad():
+        logits = head(torch.randn(2, 32) if pooled else torch.randn(2, 4, 32))
+    # the accumulator is made on the first batch: labels [B], [B, S] and [B, S + 1]
+    S_labels = 5 if layer_type == "BertTailForPreTraining" else 4
+    acc.add(logits, torch.zeros((2,) if pooled else (2, S_labels), dtype=torch.long))
+    inner = acc.inner
+    if layer_type == "BertTailForClassification":
+        assert type(inner) is TorchEvalAccumulator and inner.C == 3
+    elif layer_type == "BertTailForMaskedLM":
+        assert type(inner) is TorchTokenAccumulator and inner.V == 100
+    else:
+        assert type(inner) is PreTrainingAccumulator
+        assert type(inner.mlm) is TorchTokenAccumulator and inner.mlm.V == 100
+        assert type(inner.nsp) is TorchEvalAccumulator and inner.nsp.C == 2
 
 
 # ---------------------------------------------------------------------------------------------

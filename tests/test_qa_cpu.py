@@ -17,7 +17,7 @@ from skycomputing_b200.dynamics.estimator import Estimator
 from skycomputing_b200.dynamics.parameter_server import ParameterServer
 from skycomputing_b200.ops.functions import split_span_labels
 from skycomputing_b200.runner import QuestionAnsweringLoss, TorchSpanAccumulator, span_metrics
-from skycomputing_b200.runner.metrics import LazyEvalAccumulator
+from skycomputing_b200.runner.metrics import eval_accumulator
 from tests._dist_helpers import run_distributed
 
 V, H, S = 64, 64, 16
@@ -43,7 +43,7 @@ def test_head_matches_hf_formulas_in_fp64():
     torch.manual_seed(0)
     head = sky.build_layer("BertTailForQuestionAnswering", config=_cfg().__dict__)
     assert set(head.state_dict()) == {"qa_outputs.weight", "qa_outputs.bias"}
-    assert head.evaluated_by == "span" and head.max_answer_length == 30
+    assert head.objective == "span" and head.max_answer_length == 30
     x = torch.randn(3, S, H)
     logits = head(x, None)
     assert logits.shape == (3, 2, S) and logits.dtype == torch.float32
@@ -177,13 +177,15 @@ def test_accumulator_totals_and_predictions():
     assert span_metrics(dict(t, count=0))["loss"] is None
 
 
-def test_lazy_accumulator_follows_the_head_declaration():
+def test_eval_accumulator_follows_the_head_declaration():
     logits, lab = torch.randn(2, 2, S), torch.zeros(2, 5, dtype=torch.long)
-    acc = LazyEvalAccumulator(-100, span=(30, 8))
+    loader = torch.utils.data.DataLoader(list(range(8)), batch_size=4)
+    head = sky.build_layer("BertTailForQuestionAnswering", config=_cfg().__dict__)
+    acc = eval_accumulator(head, -100, loader)
     acc.add(logits, lab)
     assert isinstance(acc.inner, TorchSpanAccumulator)
     # without the declaration the same shapes reach the token accumulator
-    acc = LazyEvalAccumulator(-100)
+    acc = eval_accumulator(torch.nn.Linear(H, 2), -100, loader)
     acc.add(logits, lab[:, :2])
     assert not isinstance(acc.inner, TorchSpanAccumulator)
 
