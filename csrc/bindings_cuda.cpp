@@ -263,10 +263,12 @@ void small_linear_bwd(uintptr_t x, bool x_bf16, int ldx, uintptr_t w, uintptr_t 
                                      S(stream)),
         "small_linear_bwd");
 }
-void softmax_ce(uintptr_t logits, uintptr_t labels, uintptr_t loss, uintptr_t dlogits, int M,
-                int C, float grad_scale, uintptr_t loss_acc, uintptr_t stream) {
-  check(sky::launch_softmax_ce(P<const float>(logits), P<const int64_t>(labels), P<float>(loss),
-                               P<float>(dlogits), M, C, grad_scale, P<float>(loss_acc), S(stream)),
+void softmax_ce(uintptr_t logits, int ldl, uintptr_t labels, int label_ld, int N, int G, int C,
+                long long ignore_index, uintptr_t dlogits, float grad_scale, uintptr_t loss,
+                uintptr_t loss_acc, uintptr_t stream) {
+  check(sky::launch_softmax_ce(P<const float>(logits), ldl, P<const int64_t>(labels), label_ld, N,
+                               G, C, ignore_index, P<float>(dlogits), grad_scale, P<float>(loss),
+                               P<float>(loss_acc), S(stream)),
         "softmax_ce");
 }
 void classify_eval(uintptr_t logits, int ldl, uintptr_t labels, int M, int C,
@@ -313,14 +315,6 @@ void cls_grad_add(uintptr_t dhidden, uintptr_t dcls, int B, int seq, int H, uint
   check(sky::launch_cls_grad_add(P<void>(dhidden), P<const void>(dcls), B, seq, H, S(stream)),
         "cls_grad_add");
 }
-void masked_softmax_ce(uintptr_t logits, int ldl, uintptr_t labels, int M, int C,
-                       long long ignore_index, uintptr_t dlogits, float grad_scale, uintptr_t loss,
-                       uintptr_t loss_acc, uintptr_t stream) {
-  check(sky::launch_masked_softmax_ce(P<const float>(logits), ldl, P<const int64_t>(labels), M, C,
-                                      ignore_index, P<float>(dlogits), grad_scale, P<float>(loss),
-                                      P<float>(loss_acc), S(stream)),
-        "masked_softmax_ce");
-}
 void qa_logits_fwd(uintptr_t hidden, int B, int seq, int H, uintptr_t w, uintptr_t b,
                    uintptr_t logits, uintptr_t stream) {
   check(sky::launch_qa_logits_fwd(P<const void>(hidden), B, seq, H, P<const float>(w),
@@ -334,14 +328,6 @@ void qa_logits_bwd(uintptr_t hidden, uintptr_t dlogits, int B, int seq, int H, u
                                   P<const float>(w), P<void>(dhidden), P<float>(workspace),
                                   P<float>(dw), P<float>(db), S(stream)),
         "qa_logits_bwd");
-}
-void qa_span_ce(uintptr_t logits, uintptr_t labels, int B, int seq, long long ignore_index,
-                uintptr_t dlogits, float grad_scale, uintptr_t loss, uintptr_t loss_acc,
-                uintptr_t stream) {
-  check(sky::launch_qa_span_ce(P<const float>(logits), P<const int64_t>(labels), B, seq,
-                               ignore_index, P<float>(dlogits), grad_scale, P<float>(loss),
-                               P<float>(loss_acc), S(stream)),
-        "qa_span_ce");
 }
 void qa_span_eval(uintptr_t logits, uintptr_t labels, int B, int seq, int max_answer_length,
                   long long ignore_index, uintptr_t acc, uintptr_t pred_spans,
@@ -619,8 +605,9 @@ PYBIND11_MODULE(_cuda, m) {
         py::arg("lddx"), py::arg("dw"), py::arg("db"), py::arg("M"), py::arg("N"), py::arg("K"),
         py::arg("act_tanh") = 0, py::arg("dropout_p") = 0.f, py::arg("rng_state") = 0,
         py::arg("rng_stream") = 0, py::arg("stream") = 0);
-  m.def("softmax_ce", &softmax_ce, py::arg("logits"), py::arg("labels"), py::arg("loss"),
-        py::arg("dlogits"), py::arg("M"), py::arg("C"), py::arg("grad_scale") = 1.f,
+  m.def("softmax_ce", &softmax_ce, py::arg("logits"), py::arg("ldl"), py::arg("labels"),
+        py::arg("label_ld"), py::arg("N"), py::arg("G"), py::arg("C"), py::arg("ignore_index"),
+        py::arg("dlogits"), py::arg("grad_scale") = 1.f, py::arg("loss") = 0,
         py::arg("loss_acc") = 0, py::arg("stream") = 0);
   m.def("classify_eval", &classify_eval, py::arg("logits"), py::arg("ldl"), py::arg("labels"),
         py::arg("M"), py::arg("C"), py::arg("ignore_index"), py::arg("acc"),
@@ -640,10 +627,6 @@ PYBIND11_MODULE(_cuda, m) {
         py::arg("S") = 1);
   m.def("cls_grad_add", &cls_grad_add, py::arg("dhidden"), py::arg("dcls"), py::arg("B"),
         py::arg("S"), py::arg("H"), py::arg("stream") = 0);
-  m.def("masked_softmax_ce", &masked_softmax_ce, py::arg("logits"), py::arg("ldl"),
-        py::arg("labels"), py::arg("M"), py::arg("C"), py::arg("ignore_index"), py::arg("dlogits"),
-        py::arg("grad_scale") = 1.f, py::arg("loss") = 0, py::arg("loss_acc") = 0,
-        py::arg("stream") = 0);
   m.def("mlm_max_predictions", []() { return sky::kMlmMaxPredictions; });
   m.def("qa_logits_fwd", &qa_logits_fwd, py::arg("hidden"), py::arg("B"), py::arg("S"),
         py::arg("H"), py::arg("w"), py::arg("b"), py::arg("logits"), py::arg("stream") = 0);
@@ -653,9 +636,6 @@ PYBIND11_MODULE(_cuda, m) {
   m.def("qa_logits_bwd_workspace_bytes", [](int B, int seq, int H) {
     return sky::qa_logits_bwd_workspace_bytes(B, seq, H);
   });
-  m.def("qa_span_ce", &qa_span_ce, py::arg("logits"), py::arg("labels"), py::arg("B"),
-        py::arg("S"), py::arg("ignore_index"), py::arg("dlogits"), py::arg("grad_scale") = 1.f,
-        py::arg("loss") = 0, py::arg("loss_acc") = 0, py::arg("stream") = 0);
   m.def("qa_span_eval", &qa_span_eval, py::arg("logits"), py::arg("labels"), py::arg("B"),
         py::arg("S"), py::arg("max_answer_length"), py::arg("ignore_index"), py::arg("acc"),
         py::arg("pred_spans"), py::arg("pred_scores"), py::arg("capacity"),

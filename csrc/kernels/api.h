@@ -230,9 +230,22 @@ int launch_small_linear_bwd(const void* x, bool x_bf16, int ldx, const float* w,
                             const float* dy, void* dx, bool dx_bf16, int lddx, float* dw, float* db,
                             int M, int N, int K, int act_tanh, float dropout_p,
                             const uint64_t* rng_state, uint32_t rng_stream, cudaStream_t stream);
-// loss = mean_m CE(logits[m,:], labels[m]);  dlogits = (softmax - onehot) / M * grad_scale
-int launch_softmax_ce(const float* logits, const int64_t* labels, float* loss, float* dlogits,
-                      int M, int C, float grad_scale, float* loss_acc, cudaStream_t stream);
+// Softmax cross entropy over N * G rows of C fp32 classes, G in {1, 2} groups per item: the
+// classification loss (G = 1), the next-sentence loss (G = 1, C = 2) and the span loss (G = 2,
+// start and end rows of [B, 2, S] logits).  Row r starts at logits + r * ldl (ldl >= C); its
+// label is labels[(r / G) * label_ld + r % G] (label_ld >= G).  n_g = the rows of group g whose
+// label is in [0, C).
+//   loss = (1 / G) * sum_g (mean CE over group g's n_g rows; 0 when n_g == 0), so 0 for N == 0.
+//   dlogits [N * G, C] (packed) = (softmax - onehot) * grad_scale / (G * n_g) on such a row of
+//   group g, an exact 0 on every other row.  A label neither ignore_index nor in [0, C) is never
+//   used as an index and makes the loss NaN.
+//   loss[0] = loss, loss_acc[0] += loss * grad_scale; either may be null.
+// One CTA, fixed-order fp64 sum, no float atomics (graph replays are bit-identical), no host
+// sync.  Errors: 985 bad shape (N < 0, C < 1, G not 1 or 2, ldl < C, label_ld < G, N * G * C
+// beyond int range), 986 null logits / labels / dlogits with N > 0.
+int launch_softmax_ce(const float* logits, int ldl, const int64_t* labels, int label_ld, int N,
+                      int G, int C, long long ignore_index, float* dlogits, float grad_scale,
+                      float* loss, float* loss_acc, cudaStream_t stream);
 // Evaluation accumulator: the header is followed by C x C confusion counters [label * C + pred].
 struct EvalAccum {
   double loss_sum;                  // sum of the per-row cross entropies (fp32 rows, fp64 sum)
@@ -315,22 +328,11 @@ int launch_mlm_scatter(const void* dx_c, const int* slot_of_row, long long rows,
 // positive multiple of 8), 983 null pointer, 984 a buffer is not 16-byte aligned.
 int launch_cls_grad_add(void* dhidden, const void* dcls, int B, int S, int H, cudaStream_t stream);
 
-// Cross entropy over fp32 logits [M, C] (row stride ldl) with ignore_index, the next-sentence-
-// prediction loss.  n_valid = rows whose label is in [0, C).  dlogits [M, C] (contiguous) =
-// (softmax - onehot) * grad_scale / n_valid on those rows and an exact 0 on every other row.
-// loss[0] = mean over the n_valid rows (0 when n_valid == 0), NaN when any label is neither
-// ignore_index nor in [0, C) (such a label is never used as an index); loss_acc[0] += loss *
-// grad_scale.  loss / loss_acc may be null.  One CTA, fixed-order fp64 reduction, no host sync,
-// graph-capturable.  Errors: 985 bad shape (M < 0, C < 1, ldl < C), 986 null pointer.
-int launch_masked_softmax_ce(const float* logits, int ldl, const int64_t* labels, int M, int C,
-                             long long ignore_index, float* dlogits, float grad_scale,
-                             float* loss, float* loss_acc, cudaStream_t stream);
-
 // Question-answering span head (HF BertForQuestionAnswering's qa_outputs = Linear(H, 2)).
 // logits / dlogits are fp32 [B, 2, S]: row 2b holds sequence b's start logits, row 2b + 1 its end
 // logits.  labels are int64 [B, kQaLabelCols] per sequence: start, end (the gold answer's first and
 // last token), start_lo, start_hi (where a predicted answer may start), end_hi (the last position
-// where it may end).  All four kernels use fixed reduction orders and no float atomics (two calls
+// where it may end).  All three kernels use fixed reduction orders and no float atomics (two calls
 // or graph replays give identical bits) and never synchronise with the host.
 // Errors: 990 bad shape (B, S >= 1, H a positive multiple of 8, B * S within int range,
 // max_answer_length >= 1, capacity >= 0), 991 null pointer, 992 hidden / dhidden / w not 16-byte
@@ -348,14 +350,8 @@ int launch_qa_logits_bwd(const void* hidden, const float* dlogits, int B, int S,
                          const float* w, void* dhidden, float* workspace, float* dw, float* db,
                          cudaStream_t stream);
 size_t qa_logits_bwd_workspace_bytes(int B, int S, int H);
-// Span loss: (mean start CE + mean end CE) / 2, each mean over the sequences whose label is in
-// [0, S) (0 without one).  dlogits = d(loss * grad_scale)/dlogits, an exact 0 on a row whose label
-// is ignore_index or invalid; any label neither ignore_index nor in [0, S) makes the loss NaN and
-// is never used as an index.  loss[0] = the loss, loss_acc[0] += loss * grad_scale (either may be
-// null).  One CTA, one launch.
-int launch_qa_span_ce(const float* logits, const int64_t* labels, int B, int S,
-                      long long ignore_index, float* dlogits, float grad_scale, float* loss,
-                      float* loss_acc, cudaStream_t stream);
+// The span loss, (mean start CE + mean end CE) / 2, is launch_softmax_ce with N = B, G = 2,
+// C = ldl = S and label_ld = kQaLabelCols.
 // Evaluation accumulator of a span head.  Totals over the sequences whose gold start and end are
 // both in [0, S); `invalid` counts sequences with a gold label that is neither ignore_index nor in
 // [0, S).  Predictions go to pred_spans[cursor + b] / pred_scores[cursor + b] while that is below

@@ -35,6 +35,12 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
 __device__ __forceinline__ void warp_wait_panel(const uint32_t* flags, int panel, uint32_t target,
                                                 int* error_flag, int lane) {
   if (lane == 0) {
@@ -645,38 +651,95 @@ small_linear_dw_kernel(const void* __restrict__ x, bool x_bf16, long long ldx,
   if (db != nullptr && k == 0) db[n] += accb;
 }
 
-// softmax cross entropy, mean reduction; single block.
-__global__ void __launch_bounds__(256)
-softmax_ce_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels,
-                  float* __restrict__ loss, float* __restrict__ dlogits, int M, int C,
-                  float grad_scale, float* __restrict__ loss_acc) {
-  __shared__ float red[256];
-  float local = 0.f;
-  for (int m = threadIdx.x; m < M; m += blockDim.x) {
-    const float* l = logits + static_cast<long long>(m) * C;
-    float mx = -INFINITY;
-    for (int c = 0; c < C; ++c) mx = fmaxf(mx, l[c]);
-    float se = 0.f;
-    for (int c = 0; c < C; ++c) se += expf(l[c] - mx);
-    const float lse = mx + logf(se);
-    const int lab = static_cast<int>(labels[m]);
-    local += lse - l[lab];
-    if (dlogits != nullptr) {
-      for (int c = 0; c < C; ++c) {
-        const float pc = expf(l[c] - lse);
-        dlogits[static_cast<long long>(m) * C + c] =
-            (pc - (c == lab ? 1.f : 0.f)) * grad_scale / static_cast<float>(M);
-      }
+// ------------------------------------------------------------------------------------------
+// Softmax cross entropy over rows of a few fp32 classes: the classification, next-sentence and
+// span losses (launch_softmax_ce).  One CTA: its threads first count each group's labelled rows
+// and the invalid labels (integer atomics: the counts do not depend on the order), then warp w
+// owns rows w, w + 16, ... of each kCeChunk-row chunk and its lanes stride over the classes.
+// A row's max and exp-sum are reduced with one fixed xor pattern, the rows' CE / n_g go into an
+// fp64 chunk summed by a fixed tree, and thread 0 adds the chunk sums in chunk order.  An
+// invalid label is never used as an index.  No float atomics, no host sync: graph replays are
+// bit-identical.
+// ------------------------------------------------------------------------------------------
+constexpr int kCeWarps = 16;
+constexpr int kCeChunk = 256;  // rows per fixed-order fp64 reduction chunk
+
+// sums[0..n_arr) of the chunk's per-row values, a fixed tree over kCeChunk entries each
+__device__ __forceinline__ void chunk_tree(double (*vals)[kCeChunk], int n_arr) {
+  for (int s = kCeChunk / 2; s > 0; s >>= 1) {
+    for (int i = threadIdx.x; i < n_arr * s; i += blockDim.x) {
+      const int a = i / s, j = i - a * s;
+      vals[a][j] += vals[a][j + s];
     }
+    __syncthreads();
   }
-  red[threadIdx.x] = local;
+}
+
+// row r = item r / G, group r % G; G is a template parameter so that both are shifts
+template <int G>
+__global__ void __launch_bounds__(kCeWarps * 32)
+softmax_ce_kernel(const float* __restrict__ logits, int ldl, const int64_t* __restrict__ labels,
+                  int label_ld, int N, int C, long long ignore_index, float* __restrict__ dlogits,
+                  float grad_scale, float* __restrict__ loss, float* __restrict__ loss_acc) {
+  __shared__ double row_loss[1][kCeChunk];
+  __shared__ int cnt[3];  // labelled rows of group 0, of group 1; invalid labels
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int R = N * G;
+  if (threadIdx.x < 3) cnt[threadIdx.x] = 0;
   __syncthreads();
-  for (int s = 128; s > 0; s >>= 1) {
-    if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+  int n0 = 0, n1 = 0, nbad = 0;
+  for (int r = threadIdx.x; r < R; r += blockDim.x) {
+    const int g = r % G;
+    const long long lab = labels[static_cast<long long>(r / G) * label_ld + g];
+    if (lab == ignore_index) continue;
+    if (lab < 0 || lab >= C) ++nbad;
+    else if (g) ++n1;
+    else ++n0;
+  }
+  if (n0) atomicAdd(&cnt[0], n0);
+  if (n1) atomicAdd(&cnt[1], n1);
+  if (nbad) atomicAdd(&cnt[2], nbad);
+  __syncthreads();
+  n0 = cnt[0];
+  n1 = cnt[1];
+  const float scale0 = n0 > 0 ? grad_scale / (G * static_cast<float>(n0)) : 0.f;
+  const float scale1 = n1 > 0 ? grad_scale / (G * static_cast<float>(n1)) : 0.f;
+  double total = 0.0;
+  for (int base = 0; base < R; base += kCeChunk) {
+    for (int rr = warp; rr < kCeChunk; rr += kCeWarps) {
+      const int r = base + rr;
+      double contrib = 0.0;
+      if (r < R) {
+        const int g = r % G;
+        const float* l = logits + static_cast<long long>(r) * ldl;
+        float* d = dlogits + static_cast<long long>(r) * C;
+        const long long lab = labels[static_cast<long long>(r / G) * label_ld + g];
+        if (lab == ignore_index || lab < 0 || lab >= C) {
+          for (int c = lane; c < C; c += 32) d[c] = 0.f;
+        } else {
+          float mx = -INFINITY;
+          for (int c = lane; c < C; c += 32) mx = fmaxf(mx, l[c]);
+          mx = warp_max(mx);
+          float se = 0.f;
+          for (int c = lane; c < C; c += 32) se += expf(l[c] - mx);
+          se = warp_sum(se);
+          const float lse = mx + logf(se);
+          const float sc = g ? scale1 : scale0;
+          for (int c = lane; c < C; c += 32)
+            d[c] = (expf(l[c] - lse) - (c == lab ? 1.f : 0.f)) * sc;
+          contrib = static_cast<double>(lse - l[lab]) / (g ? n1 : n0);
+        }
+      }
+      if (lane == 0) row_loss[0][rr] = contrib;
+    }
+    __syncthreads();
+    chunk_tree(row_loss, 1);
+    if (threadIdx.x == 0) total += row_loss[0][0];
     __syncthreads();
   }
   if (threadIdx.x == 0) {
-    const float mean = red[0] / static_cast<float>(M);
+    float mean = static_cast<float>(total / G);
+    if (cnt[2] > 0) mean = __int_as_float(0x7fc00000);  // NaN: an invalid label is never silent
     if (loss != nullptr) loss[0] = mean;
     // micro-batched training: the step loss is the sum of the scaled micro-batch losses
     if (loss_acc != nullptr) loss_acc[0] += mean * grad_scale;
@@ -699,6 +762,35 @@ __device__ __forceinline__ bool eval_better(float a, int ia, float b, int ib) {
   return a > b || (a == b && ia < ib);
 }
 
+// argmax (eval_better) and lse = max + log(sum exp(l - max)) of one row of C > 0 classes,
+// warp-wide: lanes stride over the classes, one fixed xor pattern reduces them
+__device__ __forceinline__ void warp_row_stats(const float* __restrict__ l, int C, int lane,
+                                               int* arg_out, float* lse_out) {
+  float mx = -INFINITY;
+  int arg = C;  // no candidate yet (C > 0: every row has one after the reduction)
+  for (int c = lane; c < C; c += 32) {
+    const float v = l[c];
+    if (arg == C || eval_better(v, c, mx, arg)) {
+      mx = v;
+      arg = c;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float omx = __shfl_xor_sync(0xffffffffu, mx, o);
+    const int oarg = __shfl_xor_sync(0xffffffffu, arg, o);
+    if (oarg < C && (arg == C || eval_better(omx, oarg, mx, arg))) {
+      mx = omx;
+      arg = oarg;
+    }
+  }
+  float se = 0.f;
+  for (int c = lane; c < C; c += 32) se += expf(l[c] - mx);
+  se = warp_sum(se);
+  *arg_out = arg;
+  *lse_out = mx + logf(se);
+}
+
 __global__ void __launch_bounds__(kEvalWarps * 32)
 classify_eval_kernel(const float* __restrict__ logits, long long ldl,
                      const int64_t* __restrict__ labels, int M, int C, long long ignore_index,
@@ -713,34 +805,15 @@ classify_eval_kernel(const float* __restrict__ logits, long long ldl,
       double contrib = 0.0;
       if (m < M) {
         const float* l = logits + static_cast<long long>(m) * ldl;
-        float mx = -INFINITY;
-        int arg = C;  // no candidate yet (C > 0: every row has one after the reduction)
-        for (int c = lane; c < C; c += 32) {
-          const float v = l[c];
-          if (arg == C || eval_better(v, c, mx, arg)) {
-            mx = v;
-            arg = c;
-          }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          const float omx = __shfl_xor_sync(0xffffffffu, mx, o);
-          const int oarg = __shfl_xor_sync(0xffffffffu, arg, o);
-          if (oarg < C && (arg == C || eval_better(omx, oarg, mx, arg))) {
-            mx = omx;
-            arg = oarg;
-          }
-        }
-        // lse = mx + log(sum exp(l - mx)), as in softmax_ce_kernel
-        float se = 0.f;
-        for (int c = lane; c < C; c += 32) se += expf(l[c] - mx);
-        se = warp_sum(se);
+        int arg;
+        float lse;
+        warp_row_stats(l, C, lane, &arg, &lse);
         const long long lab = labels[m];
         if (lab != ignore_index) {
           if (lab < 0 || lab >= C) {
             ++invalid;
           } else {
-            const float loss = (mx + logf(se)) - l[lab];
+            const float loss = lse - l[lab];
             contrib = static_cast<double>(loss);
             ++counted;
             if (lane == 0) atomicAdd(&acc->confusion[lab * C + arg], 1ull);
@@ -1101,74 +1174,6 @@ cls_grad_add_kernel(uint4* __restrict__ dhidden, const uint4* __restrict__ dcls,
 }
 
 // ------------------------------------------------------------------------------------------
-// Cross entropy over a few classes with ignore_index (the next-sentence-prediction loss).  One
-// CTA: pass 1 counts the labelled rows (label != ignore_index) and the invalid ones (outside
-// [0, C)), pass 2 writes every gradient row and the row losses, which are summed in a fixed fp64
-// tree.  An invalid label is never dereferenced: its row gradient is 0 and the loss NaN.  No
-// float atomics, no host sync: graph replays are bit-identical.
-// ------------------------------------------------------------------------------------------
-constexpr int kMaskedCeThreads = 256;
-
-__global__ void __launch_bounds__(kMaskedCeThreads)
-masked_softmax_ce_kernel(const float* __restrict__ logits, int ldl,
-                         const int64_t* __restrict__ labels, int M, int C, long long ignore_index,
-                         float* __restrict__ dlogits, float grad_scale, float* __restrict__ loss,
-                         float* __restrict__ loss_acc) {
-  __shared__ double red[kMaskedCeThreads];
-  __shared__ int cnt[kMaskedCeThreads], bad[kMaskedCeThreads];
-  const int tid = threadIdx.x;
-  int n = 0, nbad = 0;
-  for (int m = tid; m < M; m += kMaskedCeThreads) {
-    const long long lab = labels[m];
-    if (lab != ignore_index) {
-      if (lab < 0 || lab >= C) ++nbad;
-      else ++n;
-    }
-  }
-  cnt[tid] = n;
-  bad[tid] = nbad;
-  __syncthreads();
-  for (int s = kMaskedCeThreads / 2; s > 0; s >>= 1) {
-    if (tid < s) {
-      cnt[tid] += cnt[tid + s];
-      bad[tid] += bad[tid + s];
-    }
-    __syncthreads();
-  }
-  const int n_valid = cnt[0];
-  const float gscale = n_valid > 0 ? grad_scale / static_cast<float>(n_valid) : 0.f;
-  double local = 0.0;
-  for (int m = tid; m < M; m += kMaskedCeThreads) {
-    const float* l = logits + static_cast<long long>(m) * ldl;
-    float* d = dlogits + static_cast<long long>(m) * C;
-    const long long lab = labels[m];
-    if (lab == ignore_index || lab < 0 || lab >= C) {
-      for (int c = 0; c < C; ++c) d[c] = 0.f;
-      continue;
-    }
-    float mx = -INFINITY;
-    for (int c = 0; c < C; ++c) mx = fmaxf(mx, l[c]);
-    float se = 0.f;
-    for (int c = 0; c < C; ++c) se += expf(l[c] - mx);
-    const float lse = mx + logf(se);
-    local += static_cast<double>(lse - l[lab]);
-    for (int c = 0; c < C; ++c) d[c] = (expf(l[c] - lse) - (c == lab ? 1.f : 0.f)) * gscale;
-  }
-  red[tid] = local;
-  __syncthreads();
-  for (int s = kMaskedCeThreads / 2; s > 0; s >>= 1) {
-    if (tid < s) red[tid] += red[tid + s];
-    __syncthreads();
-  }
-  if (tid == 0) {
-    float mean = n_valid > 0 ? static_cast<float>(red[0] / n_valid) : 0.f;
-    if (bad[0] > 0) mean = __int_as_float(0x7fc00000);  // NaN: an invalid label is never silent
-    if (loss != nullptr) loss[0] = mean;
-    if (loss_acc != nullptr) loss_acc[0] += mean * grad_scale;
-  }
-}
-
-// ------------------------------------------------------------------------------------------
 // Question-answering span head (HF BertForQuestionAnswering: qa_outputs = Linear(H, 2)).
 //   qa_logits_fwd_kernel       one warp per row: the bf16 row (16-byte loads) dotted with w[0]
 //                              and w[1] in fp32, plus the bias, stored as logits [B, 2, S]
@@ -1176,8 +1181,8 @@ masked_softmax_ce_kernel(const float* __restrict__ logits, int ldl,
 //                              dhidden = g0 w0 + g1 w1 (bf16, every row written once) and that
 //                              row range's partial dW [2, H] / db [2]
 //   qa_logits_finalize_kernel  the partials summed in row-block order (fp64), added into dW / db
-//   qa_span_ce_kernel          one CTA: the span loss and its [B, 2, S] gradient
 //   qa_span_eval_kernel        one CTA: best span per row, totals, predictions at a device cursor
+// The span loss is softmax_ce_kernel over the 2B rows, start and end as two groups.
 // Warp reductions use one fixed xor pattern and every float sum a fixed order, no float atomics:
 // two calls or graph replays give identical bits.
 // ------------------------------------------------------------------------------------------
@@ -1185,8 +1190,6 @@ constexpr int kQaFwdWarps = 8;
 constexpr int kQaColChunks = 32;  // bwd CTA: 32 x 8 threads, 32 16-byte chunks = 256 columns
 constexpr int kQaRowLanes = 8;
 constexpr int kQaRowUnroll = 4;   // rows a bwd thread loads before it computes
-constexpr int kQaWarps = 16;      // span_ce / span_eval: one CTA of 16 warps
-constexpr int kQaChunk = 256;     // rows per fixed-order fp64 reduction chunk
 
 __device__ __forceinline__ void unpack_bf16x8(const uint4& u, float* x) {
   const float2 f0 = unpack_bf16x2(u.x), f1 = unpack_bf16x2(u.y);
@@ -1346,88 +1349,6 @@ qa_logits_finalize_kernel(const float* __restrict__ partial, int n_blocks, int H
   }
 }
 
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
-// sums[0..n_arr) of the chunk's per-row values, a fixed tree over kQaChunk entries each
-__device__ __forceinline__ void qa_chunk_tree(double (*vals)[kQaChunk], int n_arr) {
-  for (int s = kQaChunk / 2; s > 0; s >>= 1) {
-    for (int i = threadIdx.x; i < n_arr * s; i += blockDim.x) {
-      const int a = i / s, j = i - a * s;
-      vals[a][j] += vals[a][j + s];
-    }
-    __syncthreads();
-  }
-}
-
-__global__ void __launch_bounds__(kQaWarps * 32)
-qa_span_ce_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels, int B,
-                  int S, long long ignore_index, float* __restrict__ dlogits, float grad_scale,
-                  float* __restrict__ loss, float* __restrict__ loss_acc) {
-  __shared__ double row_loss[1][kQaChunk];
-  __shared__ int cnt[3];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x < 3) cnt[threadIdx.x] = 0;
-  __syncthreads();
-  int n0 = 0, n1 = 0, nbad = 0;
-  for (int i = threadIdx.x; i < 2 * B; i += blockDim.x) {
-    const long long lab = labels[static_cast<long long>(i >> 1) * kQaLabelCols + (i & 1)];
-    if (lab == ignore_index) continue;
-    if (lab < 0 || lab >= S) ++nbad;
-    else if (i & 1) ++n1;
-    else ++n0;
-  }
-  // integer atomics: the counts do not depend on the order
-  if (n0) atomicAdd(&cnt[0], n0);
-  if (n1) atomicAdd(&cnt[1], n1);
-  if (nbad) atomicAdd(&cnt[2], nbad);
-  __syncthreads();
-  const int n_start = cnt[0], n_end = cnt[1];
-  const float scale0 = n_start > 0 ? grad_scale / (2.f * static_cast<float>(n_start)) : 0.f;
-  const float scale1 = n_end > 0 ? grad_scale / (2.f * static_cast<float>(n_end)) : 0.f;
-  double total = 0.0;
-  for (int base = 0; base < 2 * B; base += kQaChunk) {
-    for (int rr = warp; rr < kQaChunk; rr += kQaWarps) {
-      const int row = base + rr;  // row 2b: start logits of sequence b, 2b + 1: end logits
-      double contrib = 0.0;
-      if (row < 2 * B) {
-        const float* l = logits + static_cast<long long>(row) * S;
-        float* d = dlogits + static_cast<long long>(row) * S;
-        const long long lab = labels[static_cast<long long>(row >> 1) * kQaLabelCols + (row & 1)];
-        if (lab == ignore_index || lab < 0 || lab >= S) {
-          for (int s = lane; s < S; s += 32) d[s] = 0.f;
-        } else {
-          float mx = -INFINITY;
-          for (int s = lane; s < S; s += 32) mx = fmaxf(mx, l[s]);
-          mx = warp_max(mx);
-          float se = 0.f;
-          for (int s = lane; s < S; s += 32) se += expf(l[s] - mx);
-          se = warp_sum(se);
-          const float lse = mx + logf(se);
-          const float sc = (row & 1) ? scale1 : scale0;
-          for (int s = lane; s < S; s += 32)
-            d[s] = (expf(l[s] - lse) - (s == lab ? 1.f : 0.f)) * sc;
-          contrib = static_cast<double>(lse - l[lab]) / ((row & 1) ? n_end : n_start);
-        }
-      }
-      if (lane == 0) row_loss[0][rr] = contrib;
-    }
-    __syncthreads();
-    qa_chunk_tree(row_loss, 1);
-    if (threadIdx.x == 0) total += row_loss[0][0];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    float mean = static_cast<float>(total * 0.5);
-    if (cnt[2] > 0) mean = __int_as_float(0x7fc00000);  // NaN: an invalid label is never silent
-    if (loss != nullptr) loss[0] = mean;
-    if (loss_acc != nullptr) loss_acc[0] += mean * grad_scale;
-  }
-}
-
 // (v, i, j) is a better span than (w, k, l): a higher score, then the smaller (i, j); i < 0 marks
 // "no candidate"
 __device__ __forceinline__ bool qa_span_better(float v, int i, int j, float w, int k, int l) {
@@ -1436,48 +1357,20 @@ __device__ __forceinline__ bool qa_span_better(float v, int i, int j, float w, i
   return v > w || (v == w && (i < k || (i == k && j < l)));
 }
 
-// argmax (eval_better: first maximum, NaN is the maximum) and lse of one row, warp-wide
-__device__ __forceinline__ void qa_row_stats(const float* __restrict__ l, int S, int lane,
-                                             int* arg_out, float* lse_out) {
-  float mx = -INFINITY;
-  int arg = S;
-  for (int c = lane; c < S; c += 32) {
-    const float v = l[c];
-    if (arg == S || eval_better(v, c, mx, arg)) {
-      mx = v;
-      arg = c;
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float omx = __shfl_xor_sync(0xffffffffu, mx, o);
-    const int oarg = __shfl_xor_sync(0xffffffffu, arg, o);
-    if (oarg < S && (arg == S || eval_better(omx, oarg, mx, arg))) {
-      mx = omx;
-      arg = oarg;
-    }
-  }
-  float se = 0.f;
-  for (int c = lane; c < S; c += 32) se += expf(l[c] - mx);
-  se = warp_sum(se);
-  *arg_out = arg;
-  *lse_out = mx + logf(se);
-}
-
-__global__ void __launch_bounds__(kQaWarps * 32)
+__global__ void __launch_bounds__(kCeWarps * 32)
 qa_span_eval_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels, int B,
                     int S, int L, long long ignore_index, SpanEvalAccum* __restrict__ acc,
                     int* __restrict__ pred_spans, float* __restrict__ pred_scores,
                     long long capacity) {
-  __shared__ double vals[3][kQaChunk];  // start CE, end CE, F1 of the chunk's rows
+  __shared__ double vals[3][kCeChunk];  // start CE, end CE, F1 of the chunk's rows
   __shared__ unsigned long long cursor;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (threadIdx.x == 0) cursor = acc->cursor;
   __syncthreads();
   unsigned long long counted = 0, start_ok = 0, end_ok = 0, exact = 0, invalid = 0, overflow = 0;
   double tot[3] = {0.0, 0.0, 0.0};
-  for (int base = 0; base < B; base += kQaChunk) {
-    for (int rr = warp; rr < kQaChunk; rr += kQaWarps) {
+  for (int base = 0; base < B; base += kCeChunk) {
+    for (int rr = warp; rr < kCeChunk; rr += kCeWarps) {
       const int b = base + rr;
       double ce_s = 0.0, ce_e = 0.0, f1 = 0.0;
       if (b < B) {
@@ -1532,8 +1425,8 @@ qa_span_eval_kernel(const float* __restrict__ logits, const int64_t* __restrict_
         } else if (ok_s && ok_e) {
           int arg_s, arg_e;
           float lse_s, lse_e;
-          qa_row_stats(st, S, lane, &arg_s, &lse_s);
-          qa_row_stats(en, S, lane, &arg_e, &lse_e);
+          warp_row_stats(st, S, lane, &arg_s, &lse_s);
+          warp_row_stats(en, S, lane, &arg_e, &lse_e);
           ce_s = static_cast<double>(lse_s - st[gs]);
           ce_e = static_cast<double>(lse_e - en[ge]);
           // SQuAD's token F1 on position intervals: overlap / predicted and overlap / gold length
@@ -1559,7 +1452,7 @@ qa_span_eval_kernel(const float* __restrict__ logits, const int64_t* __restrict_
       }
     }
     __syncthreads();
-    qa_chunk_tree(vals, 3);
+    chunk_tree(vals, 3);
     if (threadIdx.x == 0) {
       tot[0] += vals[0][0];
       tot[1] += vals[1][0];
@@ -2314,10 +2207,16 @@ int launch_small_linear_bwd(const void* x, bool x_bf16, int ldx, const float* w,
   SKY_LAUNCH_CHECK();
 }
 
-int launch_softmax_ce(const float* logits, const int64_t* labels, float* loss, float* dlogits,
-                      int M, int C, float grad_scale, float* loss_acc, cudaStream_t stream) {
-  softmax_ce_kernel<<<1, 256, 0, stream>>>(logits, labels, loss, dlogits, M, C, grad_scale,
-                                           loss_acc);
+int launch_softmax_ce(const float* logits, int ldl, const int64_t* labels, int label_ld, int N,
+                      int G, int C, long long ignore_index, float* dlogits, float grad_scale,
+                      float* loss, float* loss_acc, cudaStream_t stream) {
+  if (N < 0 || C < 1 || (G != 1 && G != 2) || ldl < C || label_ld < G ||
+      static_cast<long long>(N) * G * C > 0x7fffffffLL)
+    return 985;
+  if (N > 0 && (!logits || !labels || !dlogits)) return 986;
+  auto kern = G == 2 ? softmax_ce_kernel<2> : softmax_ce_kernel<1>;
+  kern<<<1, kCeWarps * 32, 0, stream>>>(logits, ldl, labels, label_ld, N, C, ignore_index, dlogits,
+                                        grad_scale, loss, loss_acc);
   SKY_LAUNCH_CHECK();
 }
 
@@ -2453,16 +2352,6 @@ int launch_cls_grad_add(void* dhidden, const void* dcls, int B, int S, int H,
   SKY_LAUNCH_CHECK();
 }
 
-int launch_masked_softmax_ce(const float* logits, int ldl, const int64_t* labels, int M, int C,
-                             long long ignore_index, float* dlogits, float grad_scale,
-                             float* loss, float* loss_acc, cudaStream_t stream) {
-  if (M < 0 || C < 1 || ldl < C) return 985;
-  if (M > 0 && (!logits || !labels || !dlogits)) return 986;
-  masked_softmax_ce_kernel<<<1, kMaskedCeThreads, 0, stream>>>(
-      logits, ldl, labels, M, C, ignore_index, dlogits, grad_scale, loss, loss_acc);
-  SKY_LAUNCH_CHECK();
-}
-
 namespace {
 bool qa_shape_ok(int B, int S, int H) {
   return B >= 1 && S >= 1 && H >= 8 && H % 8 == 0 &&
@@ -2511,16 +2400,6 @@ int launch_qa_logits_bwd(const void* hidden, const float* dlogits, int B, int S,
   SKY_LAUNCH_CHECK();
 }
 
-int launch_qa_span_ce(const float* logits, const int64_t* labels, int B, int S,
-                      long long ignore_index, float* dlogits, float grad_scale, float* loss,
-                      float* loss_acc, cudaStream_t stream) {
-  if (B < 1 || S < 1 || static_cast<long long>(B) * S > 0x3fffffffLL) return 990;
-  if (!logits || !labels || !dlogits) return 991;
-  qa_span_ce_kernel<<<1, kQaWarps * 32, 0, stream>>>(logits, labels, B, S, ignore_index, dlogits,
-                                                     grad_scale, loss, loss_acc);
-  SKY_LAUNCH_CHECK();
-}
-
 int launch_qa_span_eval(const float* logits, const int64_t* labels, int B, int S,
                         int max_answer_length, long long ignore_index, SpanEvalAccum* acc,
                         int* pred_spans, float* pred_scores, long long capacity,
@@ -2529,7 +2408,7 @@ int launch_qa_span_eval(const float* logits, const int64_t* labels, int B, int S
       static_cast<long long>(B) * S > 0x3fffffffLL)
     return 990;
   if (!logits || !labels || !acc || (capacity > 0 && (!pred_spans || !pred_scores))) return 991;
-  qa_span_eval_kernel<<<1, kQaWarps * 32, 0, stream>>>(logits, labels, B, S, max_answer_length,
+  qa_span_eval_kernel<<<1, kCeWarps * 32, 0, stream>>>(logits, labels, B, S, max_answer_length,
                                                        ignore_index, acc, pred_spans, pred_scores,
                                                        capacity);
   SKY_LAUNCH_CHECK();

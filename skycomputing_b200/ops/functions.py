@@ -978,9 +978,15 @@ def split_span_labels(labels: torch.Tensor):
     ``start_hi`` where a predicted answer may start, and ``end_hi``, the last position where it
     may end.  Returns ``(start, end, start_lo, start_hi, end_hi)`` as views.  A padded evaluation
     row is ``ignore_index`` in every column.  One tensor keeps the engine's chunking, label
-    buffers, label routing and evaluation padding unchanged; this function is the only place that
-    knows the layout."""
+    buffers, label routing and evaluation padding unchanged; this function and
+    ``span_answer_labels`` are the only places that know the layout."""
     return labels[..., 0], labels[..., 1], labels[..., 2], labels[..., 3], labels[..., 4]
+
+
+def span_answer_labels(labels: torch.Tensor) -> torch.Tensor:
+    """``(start, end)`` of ``split_span_labels``' layout as one ``[B, 2]`` view of ``labels``
+    (``[B, 5]`` or flat): the labels of the span loss's start and end logit rows."""
+    return labels.reshape(-1, 5)[:, :2]
 
 
 class QuestionAnsweringParams:
@@ -1022,24 +1028,13 @@ class QuestionAnsweringFn(torch.autograd.Function):
 
 
 class SoftmaxCrossEntropyFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, logits, labels):
-        loss, dlogits = nat.softmax_ce(logits.contiguous().float(), labels.contiguous())
-        ctx.save_for_backward(dlogits)
-        return loss.reshape(())
-
-    @staticmethod
-    def backward(ctx, dloss):
-        (dlogits,) = ctx.saved_tensors
-        return dlogits * dloss, None
-
-
-class SpanCrossEntropyFn(torch.autograd.Function):
-    """The span loss (``runner.QuestionAnsweringLoss``) as an autograd node on ``qa_span_ce``."""
+    """``nat.softmax_ce`` as an autograd node: the classification loss on [M, C] logits, and the
+    span loss (``runner.QuestionAnsweringLoss``) on [B, 2, S] logits with [B, 2] labels
+    (``span_answer_labels``)."""
 
     @staticmethod
     def forward(ctx, logits, labels, ignore_index: int):
-        loss, dlogits = nat.qa_span_ce(logits.detach().float().contiguous(), labels,
+        loss, dlogits = nat.softmax_ce(logits.float().contiguous(), labels,
                                        ignore_index=ignore_index)
         ctx.save_for_backward(dlogits)
         return loss.reshape(())

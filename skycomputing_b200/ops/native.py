@@ -38,8 +38,8 @@ _KERNELS_PER_CALL = {
     "gemm": 1, "layernorm_fwd": 1, "layernorm_bwd": 1, "ln_param_grad": 1, "colsum": 1, "dgelu_mul": 1,
     "attention_fwd": 1, "attention_bwd": 1, "embed_fwd": 1, "embed_bwd": 1,
     "small_linear_fwd": 1, "small_linear_bwd": 2, "softmax_ce": 1, "classify_eval": 1,
-    "vocab_ce": -1, "mlm_gather": 1, "mlm_scatter": 1,
-    "qa_logits_fwd": 1, "qa_logits_bwd": 2, "qa_span_ce": 1, "qa_span_eval": 1,
+    "vocab_ce": -1, "mlm_gather": 1, "mlm_scatter": 1, "cls_grad_add": 1,
+    "qa_logits_fwd": 1, "qa_logits_bwd": 2, "qa_span_eval": 1,
     "sgd_multi": 1, "adam_multi": 1, "lamb_moments": 1, "lamb_update": 1,
     "grad_sumsq_multi": 1, "optim_finalize": 1,
     "cast_f32_to_bf16": 1, "cast_bf16_to_f32": 1, "advance_counter": 1, "advance_epoch": 1,
@@ -400,21 +400,36 @@ def cast_f32_to_bf16_(src: torch.Tensor, dst: torch.Tensor) -> None:
 
 
 def softmax_ce(logits: torch.Tensor, labels: torch.Tensor, grad_scale: float = 1.0,
-               loss_acc: Optional[torch.Tensor] = None):
-    """Mean cross entropy and d(loss * grad_scale)/dlogits; ``loss_acc[0] += loss * grad_scale``
-    when given (the step loss of a micro-batched step, accumulated without extra launches)."""
+               loss_acc: Optional[torch.Tensor] = None, ignore_index: int = -100):
+    """Cross entropy over fp32 logits ``[N, C]``, or ``[N, G, C]`` with G = 2 groups of rows per
+    item (the span loss's start and end rows), with labels ``[N]`` or ``[N, G]`` int64 (unit
+    column stride, any row stride: a column of a wider label tensor is read in place).
+
+    Returns ``(loss [1], dlogits)``: the mean CE over each group's rows whose label is in
+    [0, C), averaged over the groups (a group without such a row adds 0), and d(loss *
+    grad_scale)/dlogits in the logits' shape, an exact 0 on every other row.  A label neither
+    ``ignore_index`` nor in [0, C) makes the loss NaN and is never used as an index.
+    ``loss_acc[0] += loss * grad_scale`` when given (the step loss of a micro-batched step,
+    accumulated without extra launches).  One launch, no host synchronisation, deterministic."""
     _check(logits, torch.float32, "logits")
-    if logits.dim() != 2 or not logits.is_contiguous():
-        raise ValueError("logits must be a contiguous 2-D [M, C] tensor")
-    M, C = logits.shape
-    if not labels.is_cuda or labels.dtype != torch.int64 or labels.numel() != M:
+    if logits.dim() not in (2, 3):
+        raise ValueError("logits must be [N, C] or [N, G, C]")
+    N, C = logits.shape[0], logits.shape[-1]
+    G = logits.shape[1] if logits.dim() == 3 else 1
+    if not labels.is_cuda or labels.dtype != torch.int64 or labels.numel() != N * G:
         raise ValueError("labels must be a CUDA int64 tensor with one entry per logits row")
-    labels = labels.reshape(-1).contiguous()
+    rows = logits.reshape(N * G, C)
+    labels = labels.reshape(N, G)
+    if G > 1 and labels.stride(1) != 1:
+        raise ValueError("labels must have a unit column stride")
     loss = torch.empty(1, dtype=torch.float32, device=logits.device)
-    dlogits = torch.empty_like(logits)
-    ext().softmax_ce(logits=logits.data_ptr(), labels=labels.data_ptr(), loss=loss.data_ptr(),
-                     dlogits=dlogits.data_ptr(), M=M, C=C, grad_scale=grad_scale,
-                     loss_acc=_ptr(loss_acc), stream=_stream())
+    dlogits = torch.empty(logits.shape, dtype=torch.float32, device=logits.device)
+    # a single row's stride is arbitrary: it is never stepped over
+    ext().softmax_ce(logits=rows.data_ptr(), ldl=rows.stride(0) if N * G > 1 else C,
+                     labels=labels.data_ptr(), label_ld=labels.stride(0) if N > 1 else G, N=N,
+                     G=G, C=C, ignore_index=int(ignore_index), dlogits=dlogits.data_ptr(),
+                     grad_scale=float(grad_scale), loss=loss.data_ptr(), loss_acc=_ptr(loss_acc),
+                     stream=_stream())
     return loss, dlogits
 
 
@@ -534,30 +549,6 @@ def cls_grad_add_(dhidden: torch.Tensor, dcls: torch.Tensor) -> torch.Tensor:
     return dhidden
 
 
-def masked_softmax_ce(logits: torch.Tensor, labels: torch.Tensor, grad_scale: float = 1.0,
-                      loss_acc: Optional[torch.Tensor] = None, ignore_index: int = -100):
-    """Cross entropy over fp32 logits ``[M, C]`` with ``ignore_index`` (the next-sentence loss).
-    Returns ``(loss [1], dlogits [M, C])``: the mean over the labelled rows and d(loss *
-    grad_scale)/dlogits, exact 0 on every other row; 0 and an all-zero gradient without a
-    labelled row; a NaN loss and a zero gradient row for a label outside [0, C) that is not
-    ``ignore_index``.  ``loss_acc[0] += loss * grad_scale`` when given.  One launch, no host
-    synchronisation, deterministic."""
-    _check(logits, torch.float32, "logits")
-    if logits.dim() != 2 or logits.stride(1) != 1:
-        raise ValueError("logits must be a 2-D [M, C] tensor with unit column stride")
-    M, C = logits.shape
-    if not labels.is_cuda or labels.dtype != torch.int64 or labels.numel() != M:
-        raise ValueError("labels must be a CUDA int64 tensor with one entry per logits row")
-    labels = labels.reshape(-1).contiguous()
-    loss = torch.empty(1, dtype=torch.float32, device=logits.device)
-    dlogits = torch.empty((M, C), dtype=torch.float32, device=logits.device)
-    ext().masked_softmax_ce(logits=logits.data_ptr(), ldl=max(logits.stride(0), C),
-                            labels=labels.data_ptr(), M=M, C=C, ignore_index=int(ignore_index),
-                            dlogits=dlogits.data_ptr(), grad_scale=float(grad_scale),
-                            loss=loss.data_ptr(), loss_acc=_ptr(loss_acc), stream=_stream())
-    return loss, dlogits
-
-
 def _qa_labels(labels: torch.Tensor, B: int) -> torch.Tensor:
     if not labels.is_cuda or labels.dtype != torch.int64 or labels.numel() != B * 5:
         raise ValueError("labels must be a CUDA int64 tensor [B, 5] (ops.functions."
@@ -610,24 +601,6 @@ def qa_logits_bwd(hidden: torch.Tensor, dlogits: torch.Tensor, w: torch.Tensor,
                         w=w.data_ptr(), dhidden=dhidden.data_ptr(), workspace=ws.data_ptr(),
                         dw=dw.data_ptr(), db=db.data_ptr(), stream=_stream())
     return dhidden
-
-
-def qa_span_ce(logits: torch.Tensor, labels: torch.Tensor, grad_scale: float = 1.0,
-               loss_acc: Optional[torch.Tensor] = None, ignore_index: int = -100):
-    """The span loss over fp32 logits ``[B, 2, S]`` and labels ``[B, 5]``: ``(mean start CE +
-    mean end CE) / 2``, each mean over the sequences whose label is in [0, S) (0 without one).
-    Returns ``(loss [1], dlogits [B, 2, S])``, d(loss * grad_scale)/dlogits with an exact 0 on
-    ignored rows; a label neither ``ignore_index`` nor in [0, S) makes the loss NaN.
-    ``loss_acc[0] += loss * grad_scale`` when given.  One launch, deterministic."""
-    B, S = _qa_logits_check(logits)
-    labels = _qa_labels(labels, B)
-    loss = torch.empty(1, dtype=torch.float32, device=logits.device)
-    dlogits = torch.empty_like(logits)
-    ext().qa_span_ce(logits=logits.data_ptr(), labels=labels.data_ptr(), B=B, S=S,
-                     ignore_index=int(ignore_index), dlogits=dlogits.data_ptr(),
-                     grad_scale=float(grad_scale), loss=loss.data_ptr(),
-                     loss_acc=_ptr(loss_acc), stream=_stream())
-    return loss, dlogits
 
 
 class SpanEvalAccumulator:

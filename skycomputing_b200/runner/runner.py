@@ -32,10 +32,17 @@ from .hooks import Hook
 
 
 class _NativeCrossEntropy(nn.Module):
+    """``nn.CrossEntropyLoss()`` on the ``softmax_ce`` kernel.  As in torch, rows labelled
+    ``ignore_index`` (-100) are left out of the mean and get a zero gradient.  Differences from
+    torch: with every row ignored the loss and the gradient are 0 (torch gives NaN), and any other
+    label outside [0, C) makes the loss NaN and its gradient row 0 (torch raises an error)."""
+
+    ignore_index = -100
+
     def forward(self, logits, labels):
         from ..ops.functions import SoftmaxCrossEntropyFn
 
-        return SoftmaxCrossEntropyFn.apply(logits, labels)
+        return SoftmaxCrossEntropyFn.apply(logits, labels, self.ignore_index)
 
     def fused(self, logits, labels, scale: float, loss_acc: torch.Tensor) -> torch.Tensor:
         """Engine fast path: one launch computes the micro-batch loss, adds ``loss * scale`` to
@@ -43,8 +50,9 @@ class _NativeCrossEntropy(nn.Module):
         ``logits.backward`` (no scalar-loss autograd nodes, no scaling / accumulation kernels)."""
         from ..ops import native as nat
 
-        _, dlogits = nat.softmax_ce(logits.detach().contiguous().float(), labels.contiguous(),
-                                    grad_scale=scale, loss_acc=loss_acc)
+        _, dlogits = nat.softmax_ce(logits.detach().contiguous().float(), labels,
+                                    grad_scale=scale, loss_acc=loss_acc,
+                                    ignore_index=self.ignore_index)
         return dlogits
 
 
@@ -109,16 +117,16 @@ class _NativePreTrainingLoss(PreTrainingLoss):
         self.mlm = _NativeMaskedLMLoss(ignore_index)
 
     def fused(self, logits, labels, scale: float, loss_acc: torch.Tensor):
-        """Engine fast path: ``vocab_ce`` and ``masked_softmax_ce`` each add their ``loss *
-        scale`` into ``loss_acc``; returns the gradients of (mlm_logits, nsp_logits)."""
+        """Engine fast path: ``vocab_ce`` and ``softmax_ce`` each add their ``loss * scale`` into
+        ``loss_acc``; returns the gradients of (mlm_logits, nsp_logits)."""
         from ..ops import native as nat
         from ..ops.functions import split_pretraining_labels
 
         mlm_logits, nsp_logits = logits
         mlm_labels, nsp_labels = split_pretraining_labels(labels)
         dmlm = self.mlm.fused(mlm_logits, mlm_labels, scale, loss_acc)
-        _, dnsp = nat.masked_softmax_ce(nsp_logits.detach().float(), nsp_labels, grad_scale=scale,
-                                        loss_acc=loss_acc, ignore_index=self.ignore_index)
+        _, dnsp = nat.softmax_ce(nsp_logits.detach().float(), nsp_labels, grad_scale=scale,
+                                 loss_acc=loss_acc, ignore_index=self.ignore_index)
         return dmlm, dnsp
 
 
@@ -151,18 +159,20 @@ class QuestionAnsweringLoss(nn.Module):
 
 class _NativeQuestionAnsweringLoss(QuestionAnsweringLoss):
     def forward(self, logits, labels):
-        from ..ops.functions import SpanCrossEntropyFn
+        from ..ops.functions import SoftmaxCrossEntropyFn, span_answer_labels
 
-        return SpanCrossEntropyFn.apply(logits, labels, self.ignore_index)
+        return SoftmaxCrossEntropyFn.apply(logits, span_answer_labels(labels), self.ignore_index)
 
     def fused(self, logits, labels, scale: float, loss_acc: torch.Tensor) -> torch.Tensor:
-        """Engine fast path (see ``_NativeCrossEntropy.fused``): ``qa_span_ce`` adds ``loss *
-        scale`` into ``loss_acc`` and returns the [B, 2, S] gradient of the logits."""
+        """Engine fast path (see ``_NativeCrossEntropy.fused``): ``softmax_ce`` over the start and
+        end rows adds ``loss * scale`` into ``loss_acc`` and returns the [B, 2, S] gradient of the
+        logits."""
         from ..ops import native as nat
+        from ..ops.functions import span_answer_labels
 
-        _, dlogits = nat.qa_span_ce(logits.detach().float().contiguous(), labels,
-                                    grad_scale=scale, loss_acc=loss_acc,
-                                    ignore_index=self.ignore_index)
+        _, dlogits = nat.softmax_ce(logits.detach().float().contiguous(),
+                                    span_answer_labels(labels), grad_scale=scale,
+                                    loss_acc=loss_acc, ignore_index=self.ignore_index)
         return dlogits
 
 

@@ -362,8 +362,9 @@ def test_small_linear_pooler_fallback(nat, B):
 # ---------------------------------------------------------------------------------------------
 def _softmax_ce_ref(logits, labels, gs, acc0=None, calls=1):
     """Mean cross entropy and (softmax - onehot) * gs / M in fp64, with worst-case errors of the
-    kernel's fp32 row max / __expf / __logf / block reduction (fast-math intrinsics: __expf is off
-    by 2 + |1.173 x| ulp, __logf by 2^-21.41 absolute on [0.5, 2] and 3 ulp elsewhere)."""
+    kernel's fp32 row max / __expf / __logf / exp-sum and its fp64 sum of the rows (fast-math
+    intrinsics: __expf is off by 2 + |1.173 x| ulp, __logf by 2^-21.41 absolute on [0.5, 2] and
+    3 ulp elsewhere)."""
     M, C = logits.shape
     lf = logits.to(F64)
     lab = labels[:, None]
@@ -378,13 +379,14 @@ def _softmax_ce_ref(logits, labels, gs, acc0=None, calls=1):
     d_lse = 1.01 * se_rel + log_err + U * lse.abs()
     d_row = d_lse.squeeze(1) + U * (lse.squeeze(1).abs() + lf.gather(1, lab).squeeze(1).abs())
     mean = row.mean()
-    # the block sum of M rows, then the fast-math division by M (2 ulp)
-    d_mean = ((M + 9) * U * row.abs().sum() + d_row.sum()) / M + 5 * U * mean.abs()
+    # each fp32 row CE / M in fp64 (1 rounding), a fp64 sum of M terms (at most M - 1 roundings
+    # on any term), then one rounding to fp32
+    d_mean = ((M + 1) * 2.0 ** -53 * row.abs().sum() + d_row.sum()) / M + 2 * U * mean.abs()
     onehot = torch.zeros_like(lf).scatter_(1, lab, 1.0)
     p = torch.exp(lf - lse)
     d = (p - onehot) * gs / M
     p_err = p * ((3 + EXPF_ULPS * (lf - lse).abs()) * ulp + 1.01 * d_lse + U * (lf - lse).abs())
-    # p - onehot, * grad_scale, / M (fast-math division: 2 ulp)
+    # p - onehot, times grad_scale / M (fast-math division: 2 ulp)
     d_err = (p_err + 6 * U * (p - onehot).abs()) * gs / M
     out = dict(loss=mean, d_loss=d_mean, dlogits=d, d_dlogits=d_err)
     if acc0 is not None:
@@ -399,8 +401,8 @@ def _softmax_ce_ref(logits, labels, gs, acc0=None, calls=1):
 @pytest.mark.parametrize("C", [2, 3, 17])
 @pytest.mark.parametrize("M", [1, 32, 300, 1000])
 def test_softmax_ce(nat, M, C, gs, with_acc):
-    """What the engine's fused loss uses (grad_scale = 1/m, loss_acc), and M > 256, where a
-    thread loops over several rows."""
+    """What the engine's fused loss uses (grad_scale = 1/m, loss_acc), and M > 256, where the
+    kernel sums several 256-row chunks."""
     torch.manual_seed(500 + M + C)
     logits = torch.randn(M, C, device=DEV) * 3
     labels = torch.randint(0, C, (M,), device=DEV)
@@ -424,6 +426,31 @@ def test_softmax_ce_rejects_bad_labels(nat):
                 torch.randint(0, 3, (8,))):
         with pytest.raises(ValueError, match="labels"):
             nat.softmax_ce(logits, bad)
+
+
+def test_native_cross_entropy_ignores_minus_100(nat):
+    """The native CrossEntropyLoss leaves rows labelled -100 out of the mean, as
+    nn.CrossEntropyLoss() does; with every row ignored it gives 0 and a zero gradient."""
+    from skycomputing_b200.runner import build_loss
+
+    fn = build_loss(dict(type="CrossEntropyLoss"), torch.device(DEV))
+    assert type(fn) is not torch.nn.CrossEntropyLoss
+    torch.manual_seed(510)
+    logits = (torch.randn(64, 3, device=DEV) * 3).requires_grad_(True)
+    labels = torch.randint(0, 3, (64,), device=DEV)
+    labels[::3] = -100
+    loss = fn(logits, labels)
+    loss.backward()
+    x = logits.detach().to(F64).requires_grad_(True)
+    want = torch.nn.CrossEntropyLoss()(x, labels)
+    want.backward()
+    assert float(loss.detach()) == pytest.approx(float(want.detach()), rel=1e-6)
+    assert torch.allclose(logits.grad.to(F64), x.grad, rtol=1e-5, atol=1e-7)
+    assert torch.count_nonzero(logits.grad[::3]) == 0
+    logits.grad = None
+    loss = fn(logits, torch.full_like(labels, -100))
+    loss.backward()
+    assert float(loss.detach()) == 0.0 and torch.count_nonzero(logits.grad) == 0
 
 
 # ---------------------------------------------------------------------------------------------

@@ -58,13 +58,13 @@ def test_scatter_joins_the_cls_gradient(nat, B, S, H):
     assert torch.equal(dense, want)
 
 
-def test_masked_softmax_ce_matches_torch(nat):
+def test_next_sentence_softmax_ce_matches_torch(nat):
     M, C = 32, 2
     logits = torch.randn(M, C, device="cuda") * 3
     labels = torch.randint(0, C, (M,), device="cuda")
     labels[::5] = -100
     acc = torch.zeros(1, device="cuda")
-    loss, d = nat.masked_softmax_ce(logits, labels, grad_scale=0.5, loss_acc=acc)
+    loss, d = nat.softmax_ce(logits, labels, grad_scale=0.5, loss_acc=acc)
     x = logits.double().requires_grad_(True)
     want = torch.nn.functional.cross_entropy(x, labels, ignore_index=-100)
     (want * 0.5).backward()
@@ -73,25 +73,32 @@ def test_masked_softmax_ce_matches_torch(nat):
     assert float(acc) == pytest.approx(0.5 * float(want), rel=1e-6)
     assert torch.allclose(d.double(), x.grad, rtol=1e-5, atol=1e-7)
     assert torch.count_nonzero(d[::5]) == 0
-    loss2, d2 = nat.masked_softmax_ce(logits, labels, grad_scale=0.5)
+    loss2, d2 = nat.softmax_ce(logits, labels, grad_scale=0.5)
     assert torch.equal(loss2, loss) and torch.equal(d2, d)
+    # the labels read in place as the next-sentence column of a [B, S + 1] label tensor
+    joined = torch.full((M, 17), -100, dtype=torch.int64, device="cuda")
+    joined[:, -1] = labels
+    column = split_pretraining_labels(joined)[1]
+    assert column.stride(0) == 17
+    loss3, d3 = nat.softmax_ce(logits, column, grad_scale=0.5)
+    assert torch.equal(loss3, loss) and torch.equal(d3, d)
     # no labelled row: loss 0 and a zero gradient
-    loss, d = nat.masked_softmax_ce(logits, torch.full_like(labels, -100))
+    loss, d = nat.softmax_ce(logits, torch.full_like(labels, -100))
     assert float(loss) == 0.0 and torch.count_nonzero(d) == 0
     # an out-of-range label: NaN loss, its row 0, the other rows as without it
     bad = labels.clone()
     bad[1] = 7
-    loss, d = nat.masked_softmax_ce(logits, bad)
+    loss, d = nat.softmax_ce(logits, bad)
     assert math.isnan(float(loss)) and torch.count_nonzero(d[1]) == 0
     # graph capture: bit-equal replays
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(s):
-        nat.masked_softmax_ce(logits, labels)
+        nat.softmax_ce(logits, labels)
     torch.cuda.current_stream().wait_stream(s)
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.graph(graph):
-        gl, gd = nat.masked_softmax_ce(logits, labels)
+        gl, gd = nat.softmax_ce(logits, labels)
     graph.replay()
     first = (gl.clone(), gd.clone())
     graph.replay()

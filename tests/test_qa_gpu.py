@@ -1,13 +1,15 @@
-"""Extractive question answering on sm_90a: the four span-head kernels against fp64 references,
-determinism across calls and graph replays, argument errors, the native accumulator against
-TorchSpanAccumulator, the native head against its eager path, a one-GPU pipeline (graph, replays,
-evaluation), training on SynthQADataset and fine-tuning from a pretraining checkpoint."""
+"""Extractive question answering on sm_90a: the span-head kernels and the span loss against fp64
+references, determinism across calls and graph replays, argument errors, the native accumulator
+against TorchSpanAccumulator, the native head against its eager path, a one-GPU pipeline (graph,
+replays, evaluation), training on SynthQADataset and fine-tuning from a pretraining checkpoint."""
 from __future__ import annotations
 
 import math
 
 import pytest
 import torch
+
+from skycomputing_b200.ops.functions import span_answer_labels
 
 pytestmark = pytest.mark.gpu
 
@@ -87,13 +89,13 @@ def _ce_ref(logits, lab, S):
 
 
 @pytest.mark.parametrize("B,S,H", GEOMS)
-def test_span_ce_against_fp64(nat, B, S, H):
+def test_span_softmax_ce_against_fp64(nat, B, S, H):
     g = torch.Generator(device="cuda").manual_seed(S)
     logits = torch.randn(B, 2, S, device="cuda", generator=g) * 3
     lab = _span_labels(B, S, seed=S).cuda()
     lab[0, 1] = -100                                   # an ignored end row alone
     acc = torch.zeros(1, device="cuda")
-    loss, d = nat.qa_span_ce(logits, lab, grad_scale=0.5, loss_acc=acc)
+    loss, d = nat.softmax_ce(logits, span_answer_labels(lab), grad_scale=0.5, loss_acc=acc)
     assert float(loss) == pytest.approx(_ce_ref(logits, lab, S), rel=1e-6)
     assert float(acc) == pytest.approx(0.5 * float(loss), rel=1e-6)
     x = logits.double().requires_grad_(True)
@@ -104,15 +106,15 @@ def test_span_ce_against_fp64(nat, B, S, H):
     (ref * 0.5).backward()
     assert _rel(d, x.grad) <= 1e-5
     assert torch.all(d[0, 1] == 0)
-    loss2, d2 = nat.qa_span_ce(logits, lab, grad_scale=0.5)
+    loss2, d2 = nat.softmax_ce(logits, span_answer_labels(lab), grad_scale=0.5)
     assert torch.equal(loss, loss2) and torch.equal(d, d2)
     none = lab.clone()
     none[:, :2] = -100
-    l0, d0 = nat.qa_span_ce(logits, none)
+    l0, d0 = nat.softmax_ce(logits, span_answer_labels(none))
     assert float(l0) == 0.0 and torch.all(d0 == 0)
     bad = lab.clone()
     bad[1, 0] = S
-    lb, db_ = nat.qa_span_ce(logits, bad)
+    lb, db_ = nat.softmax_ce(logits, span_answer_labels(bad))
     assert math.isnan(float(lb)) and torch.all(db_[1, 0] == 0)
 
 
@@ -155,7 +157,7 @@ def test_span_eval_matches_the_torch_accumulator(nat, B, S, H):
     assert again["f1_sum"] * 2 == got["f1_sum"]
 
 
-def test_graph_replays_are_bit_equal_and_append(nat):
+def test_span_graph_replays_are_bit_equal_and_append(nat):
     B, S, H = 8, 128, 256
     g = torch.Generator(device="cuda").manual_seed(5)
     hidden = torch.randn(B, S, H, device="cuda", generator=g).to(torch.bfloat16)
@@ -173,7 +175,7 @@ def test_graph_replays_are_bit_equal_and_append(nat):
         db.zero_()
         loss_acc.zero_()
         logits = nat.qa_logits(hidden, w, b)
-        _, d = nat.qa_span_ce(logits, lab, loss_acc=loss_acc)
+        _, d = nat.softmax_ce(logits, span_answer_labels(lab), loss_acc=loss_acc)
         outs["dh"] = nat.qa_logits_bwd(hidden, d, w, dw, db)
         acc.add(logits, lab)
 
@@ -197,7 +199,7 @@ def test_graph_replays_are_bit_equal_and_append(nat):
     assert t["spans"].shape[0] == 2 * B and torch.equal(t["spans"][:B], t["spans"][B:])
 
 
-def test_argument_errors_and_launch_counter(nat):
+def test_span_argument_errors_and_launch_counter(nat):
     x = torch.zeros(2, 4, 12, dtype=torch.bfloat16, device="cuda")
     w = torch.zeros(2, 12, device="cuda")
     out = torch.zeros(2, 2, 4, device="cuda")
@@ -218,13 +220,13 @@ def test_argument_errors_and_launch_counter(nat):
         e.qa_span_eval(logits=out.data_ptr(), labels=lab.data_ptr(), B=2, S=4,
                        max_answer_length=0, ignore_index=-100, acc=out.data_ptr(),
                        pred_spans=0, pred_scores=0, capacity=0)
-    with pytest.raises(RuntimeError, match="991"):
-        e.qa_span_ce(logits=out.data_ptr(), labels=0, B=2, S=4, ignore_index=-100,
-                     dlogits=out.data_ptr())
+    with pytest.raises(RuntimeError, match="986"):
+        e.softmax_ce(logits=out.data_ptr(), ldl=4, labels=0, label_ld=5, N=2, G=2, C=4,
+                     ignore_index=-100, dlogits=out.data_ptr())
     nat.enable_launch_counter()
     nat.reset_launch_counter()
     logits = nat.qa_logits(x16, w16, w16[0, :2].contiguous())
-    _, d = nat.qa_span_ce(logits, lab)
+    _, d = nat.softmax_ce(logits, span_answer_labels(lab))
     nat.qa_logits_bwd(x16, d, w16, torch.zeros_like(w16), torch.zeros(2, device="cuda"))
     nat.SpanEvalAccumulator(30, 2, "cuda").add(logits, lab)
     assert nat.launch_count() == 5

@@ -13,9 +13,10 @@
 #         tied     the tied word-embedding gradient exchange (tied_grad_push / tied_grad_reduce)
 #                  in loopback on one GPU, and the tied masked-language-model head
 #         pretrain the pretraining head's kernels: mlm_scatter with the [CLS]-row gradient,
-#                  cls_grad_add, masked_softmax_ce, and the native head forward / backward
+#                  cls_grad_add, softmax_ce on the next-sentence labels, and the native head
+#                  forward / backward
 #         qa       the question-answering kernels: qa_logits_fwd / qa_logits_bwd (+ finalize),
-#                  qa_span_ce, qa_span_eval, and their graph replays
+#                  softmax_ce on the start / end rows, qa_span_eval, and their graph replays
 #         all      everything above (default)
 # Runs on ONE GPU; reports land in bench_out/sanitizer_<tool>_<suite>.log.  The sanitizer slows
 # kernels 10-100x: the 4 s flag-wait timeouts are only meaningful under memcheck / synccheck.
@@ -50,7 +51,7 @@ case "$SUITE" in layers|all)
   run layers tests/test_layers_gpu.py tests/test_kernels_gpu.py -k "embeddings_pooler_classifier or handshake or signals_panels" ;;
 esac
 case "$SUITE" in pretrain|all)
-  run pretrain tests/test_pretraining_gpu.py -k "scatter_joins or masked_softmax_ce or native_head_matches" ;;
+  run pretrain tests/test_pretraining_gpu.py -k "scatter_joins or next_sentence_softmax_ce or native_head_matches" ;;
 esac
 case "$SUITE" in qa|all)
   run qa tests/test_qa_gpu.py -k "against_fp64 or matches_the_torch_accumulator or replays_are_bit_equal_and_append" ;;
